@@ -49,7 +49,9 @@ def peaks():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        # device-to-device copy (bytes read + written) measured by tools/tuning_sweep.sh on an H100 80GB HBM3 at a
+        # 400 W power limit: 3029 GB/s; the data sheet's 3.35 TB/s is not reached by a copy
+        return 3029.0, "measured device-to-device copy, H100 80GB HBM3, 400 W power limit (tools/tuning_sweep.sh)"
 
 
 class ClockSampler(threading.Thread):
@@ -118,16 +120,6 @@ class ClockSampler(threading.Thread):
                 "samples": len(s)}
 
 
-def measured_traffic():
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the fused kernel, from the committed ncu
-    capture of this workload (profiles/roofline_traffic.json); None if absent."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "roofline_traffic.json")) as f:
-            return json.load(f)
-    except Exception:
-        return None
-
-
 def make_workload(n):
     from cupoch_b200.testing import datagen
     tgt, tn = datagen.surface(n, 11)
@@ -189,8 +181,11 @@ def run_reference(args, rank):
     if rank != 0:
         return
     src, tgt, tn = make_workload(args.points)
-    med, times, r, info = cpu_arm(src, tgt, tn, runs=max(args.steps, 3), budget_s=120.0, warm=min(args.warmup, 1))
+    med, times, r, info = cpu_arm(src, tgt, tn, runs=args.steps, budget_s=float("inf"), warm=min(args.warmup, 1))
     v = ITERS / med
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, r["transformation"], r["fitness"], r["inlier_rmse"], r["iterations"],
+                     r["correspondence_set"])
     print(json.dumps({
         "impl": "reference", "metric": "icp_iterations_per_sec", "value": v, "unit": "iter/s", "n_gpus": args.gpus,
         "steps": len(times), "warmup": min(args.warmup, 1), "ms_per_step": 1e3 * med, "higher_is_better": True,
@@ -256,7 +251,7 @@ def run_native(args, rank, world):
     s_pc = cph.geometry.PointCloud(src_local)
     t_pc = cph.geometry.PointCloud(tgt)
     t_pc.normals = tn
-    flush = DeviceArray((256 << 20,), np.uint8)  # > 126 MB L2
+    flush = DeviceArray((256 << 20,), np.uint8)  # > 50 MB L2
 
     def barrier():
         _lib.check(L.cphb_stream_synchronize(None))
@@ -301,6 +296,13 @@ def run_native(args, rank, world):
     resident_steps_ms = list(step_log)
     launches = L.cphb_launch_count() - launches0
     loop_ms, loop_launches = res.loop_ms, res.loop_launches
+    if args.dump_outputs:
+        cs = res.correspondence_set
+        if dist is not None:  # every rank holds its shard's pairs (global indices): gather the single-GPU list
+            from cupoch_b200.distributed import gather_correspondences
+            cs = gather_correspondences(dist, cs, 0, world)
+        if rank == 0:
+            dump_outputs(args.dump_outputs, res.transformation, res.fitness, res.inlier_rmse, res.iterations, cs)
 
     # ---- end-to-end through the public API with host (pinned) buffers ---------------------------
     h_src, p1 = pinned_array(L, src_local.shape)
@@ -350,8 +352,8 @@ def run_native(args, rank, world):
     q_pc = cph.geometry.PointCloud(np.ascontiguousarray(src[lo:hi]))   # queries: no collective, shard by index
     for _ in range(2):
         tree.search_radius(q_pc.points, MAX_DIST, 1)
-    knn_ms, _ = timed(lambda: tree.search_radius(q_pc.points, MAX_DIST, 1), max(args.steps, 3))
-    knn_steps = max(args.steps, 3)
+    knn_ms, _ = timed(lambda: tree.search_radius(q_pc.points, MAX_DIST, 1), args.steps)
+    knn_steps = args.steps
     # ---- sub-records (N = 1 only; each a few device milliseconds) -----------------------------------
     extra = {}
     if world == 1 and not args.no_extras:
@@ -361,10 +363,10 @@ def run_native(args, rank, world):
         os.environ["CPHB_CERT_GAIN"] = "0"
         for _ in range(2):
             step_resident()
-        nocert_ms, res_nc = timed(step_resident, max(args.steps, 3))
+        nocert_ms, res_nc = timed(step_resident, args.steps)
         del os.environ["CPHB_CERT_GAIN"]
         assert np.array_equal(res_nc.transformation, res.transformation), "certificates changed the result"
-        extra["certificates_off"] = {"value": ITERS * 1e3 / (nocert_ms / max(args.steps, 3)), "unit": "iter/s",
+        extra["certificates_off"] = {"value": ITERS * 1e3 / (nocert_ms / args.steps), "unit": "iter/s",
                                      "loop_iters_per_sec": ITERS * 1e3 / res_nc.loop_ms,
                                      "note": "same workload, every launch searches (CPHB_CERT_GAIN=0); identical result"}
         # (b) config 3 of BASELINE.json: VoxelDownSample(0.02) + SearchRadius(k=1, r=0.05) on 10 M points
@@ -377,8 +379,8 @@ def run_native(args, rank, world):
             extra["config4"] = c4
     if not args.no_extras and args.points5 > 0 and (world == 1 or args.config5_multi):
         # (d) config 5 of BASELINE.json: Colored-ICP pyramid on a 20 M-point pair.  In the default line at N = 1 only (the
-        #     run that was validated on hardware this round); --config5-multi adds it at N > 1, where tools/bench_configs.py
-        #     --config 5 is the maintained entry point (profiles/r1_n8_config5_n8.json)
+        #     run validated on hardware); --config5-multi adds it at N > 1, where tools/bench_configs.py
+        #     --config 5 is the maintained entry point
         c5 = config5_record(cph, L, timed, args, rank, world, comm, dist)
         if rank == 0:
             extra["config5"] = c5
@@ -394,7 +396,6 @@ def run_native(args, rank, world):
         total_ms, e2e_ms, knn_ms, loop_ms = [float(x) for x in t.tolist()]
     if rank == 0:
         peak, peak_src = peaks()
-        traffic = measured_traffic()
         ms_step = total_ms / args.steps
         value = ITERS * 1e3 / ms_step
         kern_ms = loop_ms / max(loop_launches, 1)
@@ -426,8 +427,6 @@ def run_native(args, rank, world):
                     "ms": knn_ms / knn_steps,
                     "note": "SearchRadius of all %d source points (sharded by index over the ranks, no collective) incl. query ordering; aggregate rate" % n},
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         "traffic": (traffic["traffic_bytes_per_launch"] if traffic and world == 1 and n == 1_000_000 else None),
-                         "traffic_source": (traffic["source"] if traffic else None),
                          "peak_source": peak_src, "kernel": "icp_iteration_kernel<PointToPlane>",
                          "launch_ms": fused_ms, "launches": n_fused,
                          "launch_definition": "loop device time / iterations (both instances of the iteration kernel: search or certified pass, fixed-order sum, solve)",
@@ -457,6 +456,27 @@ def run_native(args, rank, world):
         L.cphb_comm_destroy(comm)
     if dist is not None:
         dist.destroy_process_group()
+
+
+DUMP_MAX_ROWS = 2_000_000  # correspondence pairs kept by --dump-outputs: 2 float64 each, 32 MB at most
+
+
+def dump_outputs(d, transformation, fitness, inlier_rmse, iterations, correspondence_set):
+    """What a caller of the timed registration receives from its last timed step, as float64 .npy files:
+    transformation (4x4), fitness, inlier_rmse, iterations and correspondence_set (pairs of source / target indices;
+    at N > 1 the ranks' lists gathered into the single-GPU list; above DUMP_MAX_ROWS
+    pairs, a fixed seeded sample of its rows, with their row numbers in correspondence_rows)."""
+    os.makedirs(d, exist_ok=True)
+    cs = np.asarray(correspondence_set)
+    rows = np.arange(len(cs))
+    if len(cs) > DUMP_MAX_ROWS:
+        rows = np.sort(np.random.default_rng(0).choice(len(cs), DUMP_MAX_ROWS, replace=False))
+    out = {"transformation": np.asarray(transformation, np.float64),
+           "fitness": np.array([fitness], np.float64), "inlier_rmse": np.array([inlier_rmse], np.float64),
+           "iterations": np.array([iterations], np.float64),
+           "correspondence_set": cs[rows].astype(np.float64), "correspondence_rows": rows.astype(np.float64)}
+    for name, a in out.items():
+        np.save(os.path.join(d, name + ".npy"), a)
 
 
 def cpu_baseline(src, tgt, tn, gpu_res):
@@ -506,7 +526,7 @@ def config4_record(cph, L, timed, peak, args, rank, world, comm, dist):
         dist.barrier()
     for _ in range(2):
         run()
-    reps = 5
+    reps = args.steps
     steps, loops = [], []
     for _ in range(reps):   # one step at a time: per-step device times, max over ranks, then the median step
         m1, res = timed(run, 1)
@@ -568,7 +588,7 @@ def config5_record(cph, L, timed, args, rank, world, comm, dist):
         return T
     for _ in range(2):
         pyramid()
-    reps = 3
+    reps = args.steps
     steps = []
     for _ in range(reps):
         m1, _ = timed(pyramid, 1)
@@ -597,7 +617,7 @@ def config3_records(cph, L, timed, peak, args):
     pc = cph.geometry.PointCloud(p)
     for _ in range(2):
         down = pc.voxel_down_sample(0.02)
-    reps = 5
+    reps = args.steps
     v_ms, down = timed(lambda: pc.voxel_down_sample(0.02), reps)
     v_ms /= reps
     n_out = len(down)
@@ -633,6 +653,9 @@ def main():
     ap.add_argument("--points4", type=int, default=5_000_000, help="size of the config-4 sub-record (0 = skip)")
     ap.add_argument("--points5", type=int, default=20_000_000, help="size of the config-5 sub-record (0 = skip)")
     ap.add_argument("--config5-multi", action="store_true", help="also run the config-5 sub-record at N > 1")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's registration result to DIR/<name>.npy "
+                         "(native and reference arms; at N > 1 rank 0 writes the gathered result)")
     ap.add_argument("--comm", default="p2p", choices=["p2p", "nccl"],
                     help="N>1 exchange: p2p = peer-memory stores fused into the reduce kernel, nccl = ncclAllReduce")
     args = ap.parse_args()

@@ -1,8 +1,8 @@
-"""Build libcupoch_b200.so (sm_100a only) in-tree with nvcc.
+"""Build libcupoch_b200.so (sm_90a, H100, only) in-tree with nvcc.
 
     python -m cupoch_b200.build [--force]
 
-The .so is git-ignored but travels to the GPU box with the gpurun snapshot.
+The .so and the objects are build products (git-ignored).
 -fmad=false: the arithmetic contract (DESIGN.md) spells out every fused
 multiply-add with an explicit intrinsic, so results do not depend on the
 compiler's contraction choices.
@@ -22,7 +22,7 @@ LIB = os.path.join(HERE, "lib", "libcupoch_b200.so")
 SOURCES = ["index.cu", "sort.cu", "search.cu", "icp.cu", "voxel.cu", "features.cu", "filters.cu", "voxelgrid.cu", "comm.cu",
            "reduce.cu", "fpfh.cu", "cluster.cu", "occgrid.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-fmad=false",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-fmad=false",
          "-Xcompiler", "-fPIC", "-I" + os.path.join(ROOT, "include"), "-I" + SRC]
 
 
@@ -79,7 +79,7 @@ def build(force=False, verbose=False):
         res = list(ex.map(lambda x: _compile(x, manifest), srcs))
     objs = [o for o, _, _ in res]
     if any(ch for _, _, ch in res) or not os.path.exists(LIB):
-        cmd = [NVCC, "-shared", "-o", LIB] + objs + ["-cudart", "static", "-ldl", "-gencode", "arch=compute_100a,code=sm_100a"]
+        cmd = [NVCC, "-shared", "-o", LIB] + objs + ["-cudart", "static", "-ldl", "-gencode", "arch=compute_90a,code=sm_90a"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError("link failed:\n%s\n%s" % (r.stdout, r.stderr))

@@ -1,5 +1,5 @@
-// cphb_internal.cuh -- shared host/device definitions of the B200 engine.
-// sm_100a only.  Not part of the public interface (see include/cupoch_b200.h).
+// cphb_internal.cuh -- shared host/device definitions of the H100 engine.
+// sm_90a only.  Not part of the public interface (see include/cupoch_b200.h).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -23,6 +23,7 @@
 #define CPHB_LEAF 32
 #define CPHB_LEVELS 6 /* box levels always built: 32^5 * LEAF points max */
 #define CPHB_FULL 0xffffffffu
+#define CPHB_SMS 132 /* H100 SXM; grid caps of grid-stride kernels are CPHB_SMS * 8 blocks of 256 */
 
 struct Box {
     float4 lo;
@@ -200,7 +201,7 @@ __host__ __device__ __forceinline__ float ord2f(unsigned o) {
 
 // squared distance, fixed operation order (DESIGN.md "arithmetic contract"):
 // d = q - p per axis; d2 = fma(dz,dz, fma(dx,dx, dy*dy)) -- the order nvcc 12.9 gives the reference's own kernel for
-// sm_100a under its --use_fast_math flags (FLANN CudaL2::dist, kdtree_cuda_3d_index.cu:221-227: SASS of
+// sm_90a under its --use_fast_math flags (FLANN CudaL2::dist, kdtree_cuda_3d_index.cu:221-227: SASS of
 // oracle/_ref shows FMUL dy,dy; FFMA dx,dx; FFMA dz,dz; FFMA dw,dw with dw = 0), so squared distances are bit-identical
 // to the reference binary's (tests/test_gpu_flann_ref.py)
 __device__ __forceinline__ float dist2(float qx, float qy, float qz, float px, float py, float pz) {

@@ -226,8 +226,8 @@ extern "C" int cphb_icp_create(const cphb_cloud *source, const cphb_cloud *targe
     icp->stream = s;
     const unsigned n_full = (unsigned)source->n;
     // The source's Hilbert ordering (bounds, keys, radix sort) does not depend on the target index: it runs on a side
-    // stream, concurrently with the index build (both are short chains of small kernels: ~0.1 ms and ~0.25 ms at 1 M
-    // points), and joins right before the source is gathered.
+    // stream, concurrently with the index build (both are short chains of small kernels), and joins right before the
+    // source is gathered.
     int cur_dev = 0;
     cudaGetDevice(&cur_dev);
     if (!t_side.stream || t_side.device != cur_dev) {  // (a thread that moved to another device gets a new one)
@@ -272,7 +272,7 @@ extern "C" int cphb_icp_create(const cphb_cloud *source, const cphb_cloud *targe
     icp->n_src = n;
     icp->n_pad = n_pad;
     {
-        int dev = 0, sms = 148;
+        int dev = 0, sms = CPHB_SMS;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
         const unsigned n_tiles = n_pad / 32;
@@ -435,9 +435,9 @@ static void fill_args(const cphb_icp *icp, IcpArgs &a) {
     a.flag_words = icp->flag_words;
     a.reduce_grid = icp->reduce_grid;
     // certified regime: 1 block in 8 (at least 2 when the grid allows) only runs the tiles that needed a search last time:
-    // a search on an otherwise idle SM is one warp's dependent chain (~10 us), so a helper warp should not get more than
-    // one or two of them (config 2: ~85 flagged tiles; 18 / 36 / 72 / 144 helper blocks -> the helpers finish 36 / 30 / 22 /
-    // 22 us into a launch whose other warps need 31 us, profiles/r2_sweep_cert_helpers.txt)
+    // a search on an otherwise idle SM is one warp's dependent chain, so a helper warp should not get more than one or two
+    // of them (config 2 on the H100, profiles/h100_tuning_sweep.txt: 17 / 33 / 132 helper blocks -> 6429 / 7350 / 7330 it/s, the default
+    // 66 -> 7145-7381 it/s over three runs)
     a.helper_blocks = icp->grid >= 64 ? (icp->grid / 8 > 2 ? icp->grid / 8 : 2) : 0;
     if (const char *e = getenv("CPHB_HELPER_BLOCKS")) { int v = atoi(e); if (v >= 0 && (unsigned)v < icp->grid / 2) a.helper_blocks = (unsigned)v; }
     a.prev = icp->prev;
@@ -455,7 +455,7 @@ static void fill_args(const cphb_icp *icp, IcpArgs &a) {
     a.sg = (float)sqrt((double)lg);
     float lp = (float)(1.0 - (double)lg);
     a.sp = (float)sqrt((double)lp);
-    a.cert_gain = 4.f;   // measured on config 2 (profiles/r1_cert_sweep.txt): 2..8 within 6 %
+    a.cert_gain = 4.f;   // config 2 on the H100: gain 2 / 8 -> 7168 / 7187 it/s, 4 -> 7145-7381 (flat; profiles/h100_tuning_sweep.txt)
     a.cert_cap = 0.5f;
     if (const char *e = getenv("CPHB_CERT_GAIN")) a.cert_gain = (float)atof(e);  // tuning hooks; 0 = no certificates
     if (const char *e = getenv("CPHB_CERT_CAP")) a.cert_cap = (float)atof(e);
@@ -464,7 +464,7 @@ static void fill_args(const cphb_icp *icp, IcpArgs &a) {
     a.dbg = icp->dbg;
     a.claim_max = 8u;
     if (const char *e = getenv("CPHB_CLAIM_MAX")) { int v = atoi(e); if (v >= 1 && v <= 1024) a.claim_max = (unsigned)v; }
-    a.static_sched = 1;  // 43 vs 49 us per certified launch on config 2 (profiles/r1_cert_events.txt)
+    a.static_sched = 1;  // config 2 on the H100: 7145-7381 it/s vs 6870 with the dynamic schedule (profiles/h100_tuning_sweep.txt)
     if (const char *e = getenv("CPHB_STATIC_SCHED")) a.static_sched = atoi(e) != 0;
     a.tmax = CPHB_TRANSPOSE_MAX;
     if (const char *e = getenv("CPHB_TRANSPOSE_MAX")) {  // tuning hook
@@ -601,10 +601,9 @@ extern "C" int cphb_icp_run(cphb_icp *icp, const float h_init[16], cphb_comm *co
     // launches after "done" exit at their first instruction.
     const unsigned long long launches0 = g_cphb_launches;
     // Re-tiling (the working copy re-ordered by the target position of every point's current match) after the launches
-    // whose bit is set.  It paid for itself while the rows were gathered through the caller's arrays (round 1: mask 0x12);
-    // with the target attributes in index order and the certified regime's cp.async row pipeline the ~70 us of a
-    // re-tiling are no longer earned back (mask sweep, profiles/r2_sweep_retile.txt: 0x12 9590, 0x2 9764, 0x4 9828,
-    // 0x0 10103 it/s on config 2; 1103 vs 1142 it/s in the loop of config 4), so the default is none.
+    // whose bit is set.  It paid for itself while the rows were gathered through the caller's arrays; with the target
+    // attributes in index order and the certified regime's cp.async row pipeline a re-tiling is no longer earned back
+    // (config 2 on the H100: mask 0x12 / 0x4 -> 7059 / 7135 it/s, none -> 7145-7381; profiles/h100_tuning_sweep.txt), so the default is none.
     unsigned long long retile_mask = 0ull;
     if (const char *e = getenv("CPHB_RETILE_MASK")) retile_mask = strtoull(e, nullptr, 0);  // tuning hook
     static const bool dbg_events = getenv("CPHB_DEBUG_EVENTS") != nullptr;

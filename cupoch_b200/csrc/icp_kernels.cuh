@@ -46,11 +46,11 @@ __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_gr
 #ifndef ICP_DMMA
 #define ICP_DMMA 1
 #endif
-// float -> double.  F2F.F64.F32 runs on the XU pipe (shared with MUFU), which ncu shows as the busiest unit of a certified
-// launch (44 %) for nine conversions per row; the widening is exact, so it can also be done on the integer pipes (re-bias
-// the exponent, shift the mantissa by 29 bits; zero keeps its sign; denormals / inf / NaN take the hardware path).
-// Measured: the integer form is SLOWER (9365 vs 9570 it/s, A/B in profiles/r2_ab_f2d.txt) -- the XU pipe is busy but not
-// the limiter -- so the hardware conversion stays the default; -DICP_F2D_INT=1 selects the integer form.
+// float -> double.  F2F.F64.F32 runs on the XU pipe (shared with MUFU), which nine conversions per row keep busy in a
+// certified launch; the widening is exact, so it can also be done on the integer pipes (re-bias the exponent, shift the
+// mantissa by 29 bits; zero keeps its sign; denormals / inf / NaN take the hardware path).  Measured on config 2 (H100,
+// profiles/h100_tuning_sweep.txt): 7216 it/s with the integer form vs 7069 for the same build without it, inside the +-2 % run-to-run
+// spread, so the hardware conversion stays the default; -DICP_F2D_INT=1 selects the integer form.
 #ifndef ICP_F2D_INT
 #define ICP_F2D_INT 0
 #endif
@@ -87,19 +87,20 @@ __device__ __forceinline__ void prefetch_target(const IcpArgs &a, size_t p) {
 // Two instances of the kernel, launched back to back every iteration (the regime is decided on the DEVICE, so each
 // instance checks the state and the one whose regime is not current leaves at once):
 //   ROLE 0  searching regime.  The traversal is bound by instruction issue at low occupancy, so it is compiled for MORE
-//           resident warps (96 registers: 5 blocks = 20 warps / SM; ncu of the shared 128-register build: issue slots
-//           52 % busy at 16 warps / SM).
+//           resident warps (96 registers: 5 blocks = 20 warps / SM).
 //   ROLE 1  certified regime (needs the registers: 30 float64 accumulators per lane) -- and, when the launch before it
 //           searched, the fixed-order sum of its tile sums + solve (what used to be a third kernel, icp_reduce_kernel).
 #ifndef ICP_MIN_BLOCKS
 // ROLE 1: 4 blocks = 16 warps / SM.  The tensor-core accumulation would allow 24-32 warps (80-64 registers), but more
-// resident blocks make the certified launch SLOWER (A/B profiles/r2_ab_dmma_occupancy.txt: 4 / 5 / 6 / 7 / 8 blocks per SM
-// -> 9590 / 9300 / 9100 / 8970 / 8570 it/s): its SM throughput saturates near 16 warps and every extra block adds launch,
-// pipeline-fill and grid-sum work.
+// resident blocks buy nothing (config 2 on the H100, profiles/h100_tuning_sweep.txt: compiled for 6 blocks 7188 it/s vs 7069 for the same
+// build at 4, a grid of 2 / 3 blocks per SM 7166 / 7395, all inside the +-2 % spread): the certified launch's SM
+// throughput saturates near 16 warps and every extra block adds launch, pipeline-fill and grid-sum work.
 #define ICP_MIN_BLOCKS 4
 #endif
 #ifndef ICP_MIN_BLOCKS_SEARCH
-#define ICP_MIN_BLOCKS_SEARCH 5  // ROLE 0 (96 registers: 20 warps / SM; A/B of 4 / 5 / 6 / 8 in profiles/r2_ab_search_occupancy.txt)
+// ROLE 0: 96 registers = 20 warps / SM.  Config 2 on the H100 (profiles/h100_tuning_sweep.txt): a grid of 3 / 4 blocks per SM 6576 / 7047
+// it/s; compiled for 4 / 6 blocks 7058 / 7214 it/s against 7069 for the same build at 5.
+#define ICP_MIN_BLOCKS_SEARCH 5
 #endif
 // Programmatic dependent launch: the kernels of the loop are launched with stream serialisation relaxed, so the next
 // kernel's blocks are already resident (waiting in griddepcontrol.wait) while the last block of the current one sums and

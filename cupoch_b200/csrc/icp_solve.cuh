@@ -265,7 +265,7 @@ __device__ void kabsch_from_sums(const double *S, unsigned long long n_model, fl
 // S = m.S: the 32 sums of this iteration, staged in shared memory by the caller (also in st->total for the host).
 // PAR = false: runs in ONE WARP (all 32 lanes call it).
 // PAR = true : called by EVERY warp of a block of >= 2 warps, after a __syncthreads that made m.S visible.  The 6x6
-//              determinant (partial-pivot LU) and the LDLT solve are independent chains of ~2.5 us each on one lane:
+//              determinant (partial-pivot LU) and the LDLT solve are independent chains of equal length on one lane:
 //              warp 1 computes the determinant while warp 0 solves; one __syncthreads joins them.  Same operations,
 //              same results.
 template <int KIND, bool PAR = false>
@@ -331,8 +331,8 @@ __device__ void icp_finalize(const IcpArgs &a, IcpState *st, SolveSmem &m) {
             if (KIND == CPHB_EST_GENERALIZED_ICP && (!a.tgt_cov || !a.src_cov)) have = false;
             if (have) {
                 const float dt = (KIND == CPHB_EST_GENERALIZED_ICP) ? -1.f : a.det_thresh;
-                // one lane, everything in registers (the warp-parallel shared-memory version this replaces spent 7.4 us
-                // of a 60 us certified launch in __syncwarp-separated steps)
+                // one lane, everything in registers (a warp-parallel shared-memory version spends most of its time in
+                // __syncwarp-separated steps)
                 bool ok = true;
                 if (PAR) {
                     if (lane == 0) {  // solve first, learn the determinant afterwards (it only decides accept / reject)

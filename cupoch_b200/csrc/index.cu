@@ -155,7 +155,7 @@ __global__ void __launch_bounds__(256) bounds_kernel(const float *__restrict__ x
         lo[a] = __reduce_min_sync(CPHB_FULL, lo[a]);
         hi[a] = __reduce_max_sync(CPHB_FULL, hi[a]);
     }
-    // block-level combine first: ~10k same-address global atomics (one set per warp) serialise for ~40 us
+    // block-level combine first: one set of same-address global atomics per warp (~10k at 1 M points) would serialise
     __shared__ unsigned s_lo[8][3], s_hi[8][3];
     const int warp = threadIdx.x >> 5;
     if (lane_id() == 0) {
@@ -488,7 +488,7 @@ int cphb_hilbert_order_n(const float *xyz, size_t n, uint32_t *perm_out, float *
     if (!bounds_given) {
         CPHB_LAUNCH(bounds_init_kernel, 1, 32, 0, s, b);
         int grid = (int)((n + 255) / 256);
-        if (grid > 148 * 8) grid = 148 * 8;
+        if (grid > CPHB_SMS * 8) grid = CPHB_SMS * 8;
         CPHB_LAUNCH(bounds_kernel, grid, 256, 0, s, xyz, n, b);
     }
     // Curve resolution by cloud size: ceil(log2(n) / 3) + 1 levels (3 bits each), i.e. >= 8 curve cells per point of a
@@ -611,7 +611,7 @@ extern "C" int cphb_min_max_bound(const float *points, size_t n, float h_min[3],
     if (rc) return rc;
     CPHB_LAUNCH(bounds_init_kernel, 1, 32, 0, s, b);
     int grid = (int)((n + 255) / 256);
-    if (grid > 148 * 8) grid = 148 * 8;
+    if (grid > CPHB_SMS * 8) grid = CPHB_SMS * 8;
     CPHB_LAUNCH(bounds_kernel, grid, 256, 0, s, points, n, b);
     CPHB_CHECK_LAUNCH();
     unsigned h[6];

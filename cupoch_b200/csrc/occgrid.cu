@@ -263,7 +263,7 @@ extern "C" void cphb_occgrid_default_params(cphb_occgrid_params *p) {  // occupa
 }
 
 static void occ_reset(cphb_occgrid *g, cudaStream_t s) {
-    CPHB_LAUNCH(occ_fill_kernel, 148 * 8, 256, 0, s, g->prob, g->cells);
+    CPHB_LAUNCH(occ_fill_kernel, CPHB_SMS * 8, 256, 0, s, g->prob, g->cells);
     cudaMemsetAsync(g->occ_bits, 0, sizeof(unsigned) * 3 * g->words + 64, s);  // occ | free | idx bitmaps + scratch (contiguous)
     CPHB_LAUNCH(occ_bounds_init_kernel, 1, 32, 0, s, g->bounds, (unsigned)(g->res / 2));
 }

@@ -14,7 +14,7 @@
 //   order  : radix sort of the (few) voxel keys restores the reference's
 //            lexicographic (x,y,z) output order (helper.h:113-121)
 //   final  : mean; normals mean-then-normalise (down_sample.cu:78-90)
-// The table is sized by min(n, #grid cells) so for dense grids it stays L2 resident.
+// The table is sized by min(n, #grid cells), so for grids of few cells it stays small enough for L2.
 #include <float.h>
 #include <math.h>
 #include <stdlib.h>
@@ -164,9 +164,10 @@ __global__ void __launch_bounds__(256) voxel_final_kernel(const unsigned *__rest
 // Dense-grid path.  When the grid has no more cells than about twice the points (config 3 of BASELINE.json: 10 M points
 // in 2.0 M cells), hashing buys nothing: every cell gets one 32-byte-aligned accumulator row [sum x, sum y, sum z, count]
 // (+ the attribute sums) addressed directly by its lexicographic cell number, so
-//   * there is no insert pass, no probe, no dense-id table, and the accumulators of the whole grid (64 MB at config 3)
-//     stay L2-resident instead of competing with a 48 MB key / id table (the hash path's accumulate pass moved 980 MB of
-//     DRAM traffic for 120 MB of points: profiles/r2_ops_launches.md);
+//   * there is no insert pass, no probe and no dense-id table.  The accumulators of the whole grid (64 MB at config 3)
+//     exceed the H100's 50 MB L2, yet the dense path stays the faster one: 10 M points, VoxelDownSample on the H100
+//     (profiles/h100_tuning_sweep.txt) at 0.61 / 2.0 / 3.9 M cells (20 / 64 / 126 MB of accumulators): dense 0.68 / 1.08 / 1.26 ms, hash
+//     1.26 / 2.36 / 3.02 ms; 2 M points in 2.0 M cells: 0.35 vs 0.63 ms.  So the threshold (cells <= 2 n) stands;
 //   * a cell's atomics fall into one sector;
 //   * the cells are already in the reference's output order (helper.h:113-121): an ordered compaction replaces the
 //     radix sort of the voxel keys.

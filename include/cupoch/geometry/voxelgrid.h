@@ -1,4 +1,4 @@
 // Path-compatible with cupoch/geometry/voxelgrid.h: geometry::Voxel, geometry::VoxelGrid (creation from a point
-// cloud) on the B200 engine.  See cupoch/cupoch_b200_facade.h.
+// cloud) on the GPU engine.  See cupoch/cupoch_b200_facade.h.
 #pragma once
 #include "cupoch/cupoch_b200_facade.h"

@@ -1,5 +1,5 @@
 /*
- * cupoch_b200.h -- C ABI of the B200-native ICP / kNN / voxel-grid engine.
+ * cupoch_b200.h -- C ABI of the H100-native ICP / kNN / voxel-grid engine.
  *
  * This is the drop-in boundary for cupoch's hot path (SURVEY.md section 8b).
  * cupoch has no FFI/plugin registry: its boundary is the public C++ headers

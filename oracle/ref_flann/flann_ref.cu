@@ -3,8 +3,8 @@
 //
 // TEST INFRASTRUCTURE ONLY (oracle/): this file is the few lines of glue a test needs to call the reference's
 // index exactly the way cupoch::knn::KDTreeFlann does; it contains no reference code.  The reference sources are
-// compiled WHERE THEY LIE under /root/reference (oracle/ref_flann/Makefile) into oracle/_ref/libflann_ref.so,
-// which is git-ignored and only ever loaded by tests/ (never by cupoch_b200/).
+// compiled WHERE THEY LIE in a cupoch checkout (oracle/ref_flann/Makefile) into oracle/_ref/libflann_ref.so,
+// which is git-ignored and only ever loaded by tools/make_flann_golden.py (never by cupoch_b200/).
 //
 // Call sequence mirrored (reference file:line):
 //   SetRawData    src/cupoch/knn/kdtree_flann.inl:125-144  float3 -> float4 (w = 0), Matrix with 16-B stride,

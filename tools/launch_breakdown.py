@@ -1,5 +1,5 @@
 """Per-kernel breakdown of ONE registration from an ncu launch list (gpu__time_duration.sum CSV).
-usage: python tools/launch_breakdown.py gpurun_out/launches.csv [iteration_kernel_launches_per_registration]"""
+usage: python tools/launch_breakdown.py launches.csv [iteration_kernel_launches_per_registration]"""
 import csv
 import sys
 from collections import OrderedDict

@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
-"""Summarise an .ncu-rep (captured on the GPU box under gpurun) into a small markdown file for profiles/.
-usage: tools/ncu_summary.py gpurun_out/prof.ncu-rep profiles/name.md "title / command line"
+"""Summarise an .ncu-rep into a small markdown file for profiles/.
+usage: tools/ncu_summary.py prof.ncu-rep profiles/name.md "title / command line"
 """
 import csv
 import subprocess

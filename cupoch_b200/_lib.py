@@ -90,6 +90,8 @@ _SIGNATURES = {
     "cphb_gaussian_filter": (C.c_int, [_P, _P, _P, C.c_size_t, C.c_float, C.c_float, C.c_int, _P, _P, _P,
                                        C.POINTER(C.c_size_t), _P]),
     "cphb_select_by_index": (C.c_int, [_P, _P, _P, C.c_size_t, _P, C.c_size_t, _P, _P, _P, _P]),
+    "cphb_segment_plane": (C.c_int, [_P, C.c_size_t, C.c_float, C.c_int, C.c_int, _I3, _F3, _P, C.POINTER(C.c_size_t),
+                                     _I3, _F3, _F3, _P]),
     "cphb_covariances_from_normals": (C.c_int, [_P, C.c_size_t, C.c_float, _P, C.c_int, _P]),
     "cphb_color_gradient": (C.c_int, [_P, _P, _P, C.c_size_t, C.c_float, C.c_int, _P, _P]),
     "cphb_icp_create": (C.c_int, [C.POINTER(Cloud), C.POINTER(Cloud), C.POINTER(IcpParams), _P, C.POINTER(_P)]),

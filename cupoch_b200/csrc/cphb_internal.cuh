@@ -84,8 +84,9 @@ static inline size_t cphb_align(size_t x, size_t a) { return (x + a - 1) / a * a
 int cphb_alloc_async(void **p, size_t bytes, cudaStream_t s);
 void cphb_free_async(void *p, cudaStream_t s);
 
-// radix sort of (key,value) u32 pairs by the low `bits` bits (CUB; index build
-// and source ordering only -- never inside the per-iteration loop). sort.cu
+// radix sort of (key,value) u32 pairs by the low `bits` bits (CUB, stable; index
+// build, source ordering and SegmentPlane's sampler -- never inside the ICP
+// per-iteration loop). sort.cu
 int cphb_sort_pairs_u32(const uint32_t *keys_in, uint32_t *keys_out, const uint32_t *vals_in,
                         uint32_t *vals_out, size_t n, int bits, cudaStream_t s);
 int cphb_sort_pairs_u64(const uint64_t *keys_in, uint64_t *keys_out, const uint32_t *vals_in,

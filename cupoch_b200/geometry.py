@@ -4,6 +4,7 @@ Names, argument meaning and error behaviour follow src/python/cupoch_pybind/geom
 pointcloud.cpp and kdtree_flann.cpp; computation goes through the C ABI only.
 """
 import ctypes as C
+import sys
 
 import numpy as np
 
@@ -239,6 +240,29 @@ class PointCloud:
                                                                d_idx.ptr, C.byref(m), stats, None))
         self.last_outlier_stats = tuple(float(x) for x in stats)  # (cloud mean, std, threshold): diagnostics
         return self._filtered(d_idx, m.value)
+
+    def segment_plane(self, distance_threshold=0.01, ransac_n=3, num_iterations=100):
+        """PointCloud::SegmentPlane (segmentation.cu:187-267; bound as segment_plane, pointcloud.cpp) ->
+        (plane float32[4] = [a, b, c, d], inlier indices on the device, int32 ascending).  Iteration t's seed is drawn
+        from libc rand() -- the process-global stream the reference draws from, so srand() makes a run repeatable.
+        Diagnostics of the winning hypothesis go to last_ransac_stats = (best iteration or -1, fitness, inlier_rmse)."""
+        n, ransac_n, num_iterations = len(self), int(ransac_n), int(num_iterations)
+        plane = np.zeros(4, np.float32)
+        if ransac_n < 3:
+            print("[cupoch_b200][error] ransac_n should be set to higher than or equal to 3.", file=sys.stderr)
+            return plane, DeviceArray((0,), np.int32)
+        if n < ransac_n:
+            print("[cupoch_b200][error] There must be at least 'ransac_n' points.", file=sys.stderr)
+            return plane, DeviceArray((0,), np.int32)
+        rand = C.CDLL(None).rand
+        rand.restype = C.c_int
+        seeds = (C.c_int32 * max(num_iterations, 1))(*[rand() for _ in range(num_iterations)])
+        d_idx = DeviceArray((n,), np.int32)
+        h_plane, m, best, fr = (C.c_float * 4)(), C.c_size_t(0), C.c_int32(-1), (C.c_float * 2)()
+        _lib.check(_lib.lib().cphb_segment_plane(self._points.ptr, n, float(distance_threshold), ransac_n, num_iterations,
+                                                 seeds, h_plane, d_idx.ptr, C.byref(m), C.byref(best), fr, None, None))
+        self.last_ransac_stats = (int(best.value), float(fr[0]), float(fr[1]))
+        return np.array(h_plane, np.float32), DeviceArray((m.value,), np.int32, ptr=d_idx.ptr, base=d_idx)
 
     def cluster_dbscan(self, eps, min_points, print_progress=False, max_edges=100):
         """PointCloud::ClusterDBSCAN (pointcloud_cluster.cu:84-179; bound as cluster_dbscan, pointcloud.cpp:228-245) ->

@@ -44,6 +44,19 @@ def surface(n, seed, extent=1.0):
     return np.stack([x, y, z], 1).astype(np.float32), nrm.astype(np.float32)
 
 
+def plane_scene(n, seed, noise=0.003):
+    """SegmentPlane scene: 50 % on a noisy ground z = 0 (axis-aligned, the case where the refit cancels worst), 20 % on a
+    tilted wall, 30 % clutter in [-2, 2]^2 x [0, 2], rows shuffled."""
+    rng = np.random.Generator(np.random.PCG64(seed))
+    ng, nw = n // 2, n // 5
+    g = np.column_stack([rng.uniform(-2, 2, (ng, 2)), rng.normal(0, noise, ng)])
+    uv = rng.uniform(0, 2, (nw, 2))
+    w = np.column_stack([uv[:, 0] - 1, 1.5 + 0.3 * uv[:, 1], uv[:, 1]]) + rng.normal(0, noise, (nw, 3))
+    c = np.column_stack([rng.uniform(-2, 2, (n - ng - nw, 2)), rng.uniform(0, 2, n - ng - nw)])
+    p = np.concatenate([g, w, c]).astype(np.float32)
+    return p[rng.permutation(n)]
+
+
 def texture(p, seed=None, noise=0.0):
     """smooth colour field in [0,1]^3 (config 5)."""
     x, y = p[:, 0].astype(np.float64), p[:, 1].astype(np.float64)

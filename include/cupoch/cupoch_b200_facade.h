@@ -10,6 +10,7 @@
 #include <cmath>
 #include <cstdint>
 #include <cstdio>
+#include <cstdlib>
 #include <cstring>
 #include <memory>
 #include <stdexcept>
@@ -36,6 +37,16 @@ struct Vector3f {
     float &operator()(int i) { return v[i]; }
     float operator()(int i) const { return v[i]; }
     static Vector3f Zero() { return Vector3f(); }
+};
+struct Vector4f {
+    float v[4];
+    Vector4f() : v{0, 0, 0, 0} {}
+    Vector4f(float x, float y, float z, float w) : v{x, y, z, w} {}
+    float &operator[](int i) { return v[i]; }
+    float operator[](int i) const { return v[i]; }
+    float &operator()(int i) { return v[i]; }
+    float operator()(int i) const { return v[i]; }
+    static Vector4f Zero() { return Vector4f(); }
 };
 struct Vector3i {
     int v[3];
@@ -371,6 +382,32 @@ public:
             utility::check(cphb_remove_statistical_outliers(cfp(points_), points_.size(), (int)nb_neighbors, std_ratio, kept.data(),
                                                             &m, nullptr, nullptr));
         return finish_filter(kept, m);
+    }
+    /// PointCloud::SegmentPlane (segmentation.cu:187-267) -> (plane [a, b, c, d], ascending inlier indices).  Every
+    /// iteration draws its seed with ::rand() as the reference does, so srand() makes a run repeatable.
+    std::tuple<Eigen::Vector4f, utility::device_vector<size_t>> SegmentPlane(float distance_threshold = 0.01f, size_t ransac_n = 3,
+                                                                             size_t num_iterations = 100) const {
+        utility::device_vector<size_t> inliers;
+        if (ransac_n < 3) {
+            utility::LogError("ransac_n should be set to higher than or equal to 3.");
+            return std::make_tuple(Eigen::Vector4f(0.f, 0.f, 0.f, 0.f), std::move(inliers));
+        }
+        if (points_.size() < ransac_n) {
+            utility::LogError("There must be at least 'ransac_n' points.");
+            return std::make_tuple(Eigen::Vector4f(0.f, 0.f, 0.f, 0.f), std::move(inliers));
+        }
+        if (num_iterations > (size_t)std::numeric_limits<int>::max()) utility::check(CPHB_ERR_INVALID);
+        std::vector<int32_t> seeds(num_iterations);
+        for (int32_t &s : seeds) s = std::rand();
+        utility::device_vector<int32_t> kept(points_.size());
+        size_t m = 0;
+        float h[4];
+        utility::check(cphb_segment_plane(cfp(points_), points_.size(), distance_threshold, (int)ransac_n, (int)num_iterations,
+                                          seeds.data(), h, kept.data(), &m, nullptr, nullptr, nullptr, nullptr));
+        kept.resize(m);
+        std::vector<int32_t> h32 = kept.to_host();
+        inliers = std::vector<size_t>(h32.begin(), h32.end());
+        return std::make_tuple(Eigen::Vector4f(h[0], h[1], h[2], h[3]), std::move(inliers));
     }
     /// PointCloud::ClusterDBSCAN (pointcloud.h:195-199, pointcloud_cluster.cu:84-179): labels, -1 = noise
     std::unique_ptr<utility::device_vector<int>> ClusterDBSCAN(float eps, size_t min_points, bool print_progress = false,

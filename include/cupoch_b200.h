@@ -190,6 +190,20 @@ int cphb_gaussian_filter(const float *points, const float *normals, const float 
 int cphb_select_by_index(const float *points, const float *normals, const float *colors, size_t n,
                          const int32_t *indices, size_t n_indices, float *out_points, float *out_normals,
                          float *out_colors, void *stream);
+/* PointCloud::SegmentPlane (segmentation.cu:187-267): RANSAC plane [a,b,c,d] with |dot3(abc, p) + d| <
+ * distance_threshold inliers.  h_seeds (host, num_iterations ints) are the seeds the reference draws with rand(),
+ * one per iteration; iteration t samples d_cards[0..2] after a stable sort of d_cards by thrust's random_functor(
+ * h_seeds[t], n) keys, cumulative over t.  All hypotheses are scored in one pass; the best (fitness >, or == with
+ * "inlier_rmse" <) defines the final inliers (ascending, into inliers_out, device, room for n), which are refitted
+ * (GetPlaneFromPoints) into h_plane.  Sums over points / inliers follow the order of DESIGN.md's arithmetic
+ * contract (tiles of 1024 consecutive elements summed sequentially in double, then the tiles in order).
+ * ransac_n < 3 or n < ransac_n: zero plane, no inliers (the reference logs an error).  Optional outputs (NULL to
+ * skip): h_best_iteration (-1 if no hypothesis won), h_fitness_rmse = the winner's {fitness, inlier_rmse},
+ * h_phase_ms = CUDA-event times of {sampling, scoring + selection, final inliers + refit}.  num_iterations < 0 or
+ * n > 2^31-1: CPHB_ERR_INVALID.  Synchronises. */
+int cphb_segment_plane(const float *points, size_t n, float distance_threshold, int ransac_n, int num_iterations,
+                       const int32_t *h_seeds, float h_plane[4], int32_t *inliers_out, size_t *h_n_out,
+                       int32_t *h_best_iteration, float h_fitness_rmse[2], float h_phase_ms[3], void *stream);
 
 /* ------------------------------------------------------------------------ *
  * registration  (registration.h:35-91, transformation_estimation.h:36-143,

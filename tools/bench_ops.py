@@ -24,7 +24,11 @@ def main():
     ap.add_argument("--normals", type=int, default=0, help="also time EstimateNormals(KNN k) of the 10 M cloud (fused kernel, and the two-pass form)")
     ap.add_argument("--filters", action="store_true",
                     help="also time the SURVEY 8f rows: RemoveRadiusOutliers / RemoveStatisticalOutliers / VoxelGrid")
+    ap.add_argument("--segment-plane", action="store_true",
+                    help="instead: time PointCloud::SegmentPlane per phase at N = 1 M, 10 M and T = 100, 1000")
     args = ap.parse_args()
+    if args.segment_plane:
+        return segment_plane(args.reps)
     import cupoch_b200 as cph
     from cupoch_b200 import _lib
     from cupoch_b200.testing import datagen
@@ -144,6 +148,70 @@ def main():
         "knn_self": {"ms_median": s_med, "mqueries_per_sec": n / s_med * 1e-3},
         "properties": props, "launches": int(L.cphb_launch_count()), **extra,
     }))
+
+
+def segment_plane(reps):
+    """SegmentPlane(0.01, 3, T) on datagen.plane_scene(N): CUDA-event time of the whole call and of its three phases
+    (sampling = T key kernels + T stable radix sorts; scoring = planes + one pass over the cloud for all T hypotheses +
+    selection; final = flags, compaction, refit), the single-threaded oracle port on the same input (run once), and
+    whether the two agree.  Seeds: rand() after srand(1), as a fresh cupoch process draws them."""
+    import subprocess
+    import cupoch_b200 as cph
+    from cupoch_b200 import _lib
+    from cupoch_b200.testing import datagen
+    from cupoch_b200.utility import DeviceArray
+    from oracle import segment_plane_py as seg_oracle
+    L = _lib.lib()
+    gpu = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                         capture_output=True, text=True).stdout.strip()
+    libc = C.CDLL(None)
+    libc.rand.restype = C.c_int
+    ev = [L.cphb_event_create() for _ in range(2)]
+    rows = []
+    for n in (1_000_000, 10_000_000):
+        pts = datagen.plane_scene(n, 11)
+        pc = cph.geometry.PointCloud(pts)
+        d_idx = DeviceArray((n,), np.int32)
+        for T in (100, 1000):
+            libc.srand(1)
+            seeds = (C.c_int32 * T)(*[libc.rand() for _ in range(T)])
+            plane, fr, ph = (C.c_float * 4)(), (C.c_float * 2)(), (C.c_float * 3)()
+            m, best = C.c_size_t(0), C.c_int32(0)
+            calls, phases = [], []
+            for r in range(reps + 1):  # the first call warms the allocation pool and the modules
+                L.cphb_event_record(ev[0], None)
+                _lib.check(L.cphb_segment_plane(pc.points.ptr, n, 0.01, 3, T, seeds, plane, d_idx.ptr, C.byref(m),
+                                                C.byref(best), fr, ph, None))
+                L.cphb_event_record(ev[1], None)
+                ms = C.c_float(0)
+                L.cphb_event_elapsed_ms(ev[0], ev[1], C.byref(ms))
+                if r:
+                    calls.append(ms.value)
+                    phases.append(list(ph))
+            med = float(np.median(calls))
+            ph_med = [float(np.median([p[k] for p in phases])) for k in range(3)]
+            row = {"n": n, "iterations": T}
+            if n * T > 1e9:  # the sequential oracle needs minutes here (about 3 s per 1e8 point-iterations)
+                rows.append(dict(row, cpu_baseline=None, note="oracle not run at n * T > 1e9"))
+            else:
+                t0 = time.perf_counter()
+                o_plane, o_idx, o_best, _, _ = seg_oracle.segment_plane(pts, 0.01, 3, np.array(seeds, np.int32))
+                cpu_s = time.perf_counter() - t0
+                rows.append(dict(row, cpu_baseline={"seconds": cpu_s, "cores": 1, "kind": "port"},
+                                 speedup_vs_cpu_baseline=cpu_s * 1e3 / med,
+                                 parity_vs_cpu_baseline=bool(o_best == best.value
+                                                             and np.array_equal(o_plane, np.array(plane, np.float32))
+                                                             and np.array_equal(o_idx, d_idx.cpu()[:m.value]))))
+            rows[-1].update({
+                "call_ms_median": med, "call_ms_min": float(np.min(calls)),
+                "phase_ms_median": dict(zip(("sampling", "scoring", "final"), ph_med)),
+                "phase_share": dict(zip(("sampling", "scoring", "final"), [p / sum(ph_med) for p in ph_med])),
+                "sampling_us_per_iteration": ph_med[0] * 1e3 / T,
+                "scoring_point_hypotheses_per_s": n * T / (ph_med[1] * 1e-3),
+                "inliers": int(m.value), "best_iteration": int(best.value),
+            })
+    print(json.dumps({"op": "PointCloud::SegmentPlane(0.01, 3, T) on datagen.plane_scene(N, 11)", "gpu": gpu, "reps": reps,
+                      "launches": int(L.cphb_launch_count()), "rows": rows}))
 
 
 if __name__ == "__main__":

@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""Generate tests/golden/reference_vectors.json from the reference's own unit tests.
+"""Generate tests/golden/reference_vectors.json (and segment_plane_known.json) from the reference's own unit tests.
 
 Run in the development container only (needs /root/reference, which does not
 exist on the GPU box).  It reads
@@ -21,6 +21,7 @@ import numpy as np
 
 REF = os.environ.get("CUPOCH_REFERENCE", "/root/reference")
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "tests", "golden", "reference_vectors.json")
+OUT_SEG = os.path.join(os.path.dirname(OUT), "segment_plane_known.json")  # kept apart: the vectors above are frozen
 
 
 def read(rel):
@@ -158,9 +159,26 @@ def main():
         "cite": "src/tests/geometry/pointcloud.cpp:303-334 (output == the named rows, compared as sorted sets)",
     }
     assert len(g["select_by_index"]["indices"]) == 10
+    # ---- SegmentPlane known plane (pointcloud.cpp:659-673): all five coplanar points are inliers ----
+    b = test_body(pc, "PointCloud", "SegmentPlaneKnownPlane")
+    pat = re.compile(r"ref_points\.push_back\(Eigen::Vector3f\(\{\s*(-?[\d.]+)\s*,\s*(-?[\d.]+)\s*,\s*(-?[\d.]+)\s*\}\)\)")
+    sp_pts = [[float(x), float(y), float(z)] for x, y, z in pat.findall(b)]
+    m = re.search(r"SegmentPlane\(([\d.]+),\s*(\d+),\s*(\d+)\)", b)
+    assert len(sp_pts) == 5 and m and "SelectByIndex(inliers)" in b
+    seg = {"source": g["source"], "segment_plane_known": {
+        "points": sp_pts, "distance_threshold": float(m.group(1)), "ransac_n": int(m.group(2)),
+        "num_iterations": int(m.group(3)),
+        # ExpectEQ(SelectByIndex(inliers)->GetPoints(), ref_points).  (The test's comment names x + y + z + 1 = 0, but
+        # (1, 1, -1) is not on it; all five points satisfy x = y.)
+        "inliers": list(range(len(sp_pts))),
+        "cite": "src/tests/geometry/pointcloud.cpp:659-673",
+    }}
     os.makedirs(os.path.dirname(OUT), exist_ok=True)
     with open(OUT, "w") as f:
         json.dump(g, f)
+    with open(OUT_SEG, "w") as f:
+        json.dump(seg, f)
+    print("wrote", os.path.normpath(OUT_SEG), os.path.getsize(OUT_SEG), "bytes")
     print("wrote", os.path.normpath(OUT), os.path.getsize(OUT), "bytes")
 
 

@@ -25,6 +25,7 @@
 #include <string.h>
 
 #include "cphb_internal.cuh"
+#include <type_traits>
 #include <vector>
 #include "cphb_eigen3.cuh"
 
@@ -51,9 +52,6 @@ struct cphb_icp {
     float4 *work_xyz, *work_nrm, *work_cov;
     float4 *src_col;
     float4 *tix_nrm, *tix_grad, *tix_cov;  // target attributes in index order (icp_types.cuh)
-    float4 *alt_xyz, *alt_nrm, *alt_cov, *alt_col, *cur_col;  // re-tiling ping-pong buffers
-    int2 *alt_prev;
-    uint32_t *rt_keys, *rt_keys2, *rt_vals, *rt_order;
     IcpState *st;
     IcpState *h_st;  // pinned
     bool owns_host;
@@ -103,33 +101,46 @@ static bool is_identity4(const float *T) {  // Eigen isIdentity(1e-5), registrat
     return true;
 }
 
-// resident blocks / SM of the two instances of the iteration kernel (register-limited)
-template <int KIND, int ROLE>
-static int iteration_occupancy(bool top3) {
-    int nb = 0;
-    cudaError_t e = top3 ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, icp_iteration_kernel<KIND, 3, ROLE>, ICP_SEARCH_WARPS * 32, 0)
-                         : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, icp_iteration_kernel<KIND, 5, ROLE>, ICP_SEARCH_WARPS * 32, 0);
-    if (e != cudaSuccess) { cudaGetLastError(); return 0; }
-    return nb;
+// f(std::integral_constant<int, KIND>{}) for a fused estimator (the callers have validated `kind`): one switch selects
+// the kernel instances of every launch site
+template <class F>
+static void with_kind(int kind, F &&f) {
+    switch (kind) {
+        case CPHB_EST_POINT_TO_POINT: f(std::integral_constant<int, CPHB_EST_POINT_TO_POINT>{}); break;
+        case CPHB_EST_POINT_TO_PLANE: f(std::integral_constant<int, CPHB_EST_POINT_TO_PLANE>{}); break;
+        case CPHB_EST_SYMMETRIC: f(std::integral_constant<int, CPHB_EST_SYMMETRIC>{}); break;
+        case CPHB_EST_COLORED_ICP: f(std::integral_constant<int, CPHB_EST_COLORED_ICP>{}); break;
+        case CPHB_EST_GENERALIZED_ICP: f(std::integral_constant<int, CPHB_EST_GENERALIZED_ICP>{}); break;
+    }
 }
+// f(std::integral_constant<int, TOP>{}): the iteration kernel is compiled for traversal depths 3 and 5; an index whose
+// top level is at most 3 takes the shallow instance
+template <class F>
+static void with_top(int top, F &&f) {
+    if (top <= 3) f(std::integral_constant<int, 3>{});
+    else f(std::integral_constant<int, 5>{});
+}
+
+// resident blocks / SM of the two instances of the iteration kernel (register-limited)
 template <int ROLE>
-static int iteration_occupancy_kind(int kind, bool top3) {
+static int iteration_occupancy_kind(int kind, int top) {
     static int cache[8][2] = {};  // 0 = not queried yet
-    int &c = cache[kind & 7][top3 ? 0 : 1];
+    int &c = cache[kind & 7][top <= 3 ? 0 : 1];
     if (c == 0) {
-        switch (kind) {
-            case CPHB_EST_POINT_TO_POINT: c = iteration_occupancy<CPHB_EST_POINT_TO_POINT, ROLE>(top3); break;
-            case CPHB_EST_POINT_TO_PLANE: c = iteration_occupancy<CPHB_EST_POINT_TO_PLANE, ROLE>(top3); break;
-            case CPHB_EST_SYMMETRIC: c = iteration_occupancy<CPHB_EST_SYMMETRIC, ROLE>(top3); break;
-            case CPHB_EST_COLORED_ICP: c = iteration_occupancy<CPHB_EST_COLORED_ICP, ROLE>(top3); break;
-            case CPHB_EST_GENERALIZED_ICP: c = iteration_occupancy<CPHB_EST_GENERALIZED_ICP, ROLE>(top3); break;
-        }
+        with_kind(kind, [&](auto k) {
+            with_top(top, [&](auto t) {
+                if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&c, icp_iteration_kernel<decltype(k)::value, decltype(t)::value, ROLE>,
+                                                                  ICP_SEARCH_WARPS * 32, 0) != cudaSuccess) {
+                    cudaGetLastError();
+                    c = 0;
+                }
+            });
+        });
         if (c <= 0) c = -1;
     }
     return c;
 }
 
-#if CPHB_PDL
 // launch with stream serialisation relaxed (programmatic dependent launch): the kernel may start while its
 // predecessor drains and synchronises on it with griddepcontrol.wait
 template <class K>
@@ -148,47 +159,30 @@ static void launch_pdl(K kernel, unsigned grid, unsigned block, cudaStream_t s, 
     ++g_cphb_launches;
     if (e != cudaSuccess) cphb_set_error("PDL launch failed: %s", cudaGetErrorString(e));
 }
-#endif
 
-template <int KIND>
+// two launches per iteration: the searching-regime instance, then the certified-regime instance (which also sums and
+// solves after a searching launch); the regime is decided on the device, the instance it does not concern returns
+// at its first instructions (icp_kernels.cuh)
 static void launch_iteration(const cphb_icp *icp, const IcpArgs &a, cudaStream_t s) {
-#if CPHB_PDL
-    static const bool pdl = getenv("CPHB_NO_PDL") == nullptr;
-    // two launches per iteration: the searching-regime instance, then the certified-regime instance (which also sums and
-    // solves after a searching launch); the regime is decided on the device, the instance it does not concern returns
-    // at its first instructions (icp_kernels.cuh)
-    const bool top3 = icp->index->v.top <= 3;
-    if (pdl && !a.defer_finalize && !a.step_mode && !icp->dbg_ev) {
-        if (top3) launch_pdl(icp_iteration_kernel<KIND, 3, 0>, icp->grid_search, ICP_SEARCH_WARPS * 32, s, a);
-        else launch_pdl(icp_iteration_kernel<KIND, 5, 0>, icp->grid_search, ICP_SEARCH_WARPS * 32, s, a);
-        if (top3) launch_pdl(icp_iteration_kernel<KIND, 3, 1>, icp->grid, ICP_SEARCH_WARPS * 32, s, a);
-        else launch_pdl(icp_iteration_kernel<KIND, 5, 1>, icp->grid, ICP_SEARCH_WARPS * 32, s, a);
-        return;
-    }
-#endif
-    if (icp->index->v.top <= 3) CPHB_LAUNCH((icp_iteration_kernel<KIND, 3, 0>), icp->grid_search, ICP_SEARCH_WARPS * 32, 0, s, a);
-    else CPHB_LAUNCH((icp_iteration_kernel<KIND, 5, 0>), icp->grid_search, ICP_SEARCH_WARPS * 32, 0, s, a);
-    if (icp->dbg_ev) cudaEventRecord(icp->dbg_ev[3 * a.launch_idx + 1], s);
-    if (icp->index->v.top <= 3) CPHB_LAUNCH((icp_iteration_kernel<KIND, 3, 1>), icp->grid, ICP_SEARCH_WARPS * 32, 0, s, a);
-    else CPHB_LAUNCH((icp_iteration_kernel<KIND, 5, 1>), icp->grid, ICP_SEARCH_WARPS * 32, 0, s, a);
+    // plain stream-ordered launches where the host has work between or right after them: step mode, the NCCL
+    // all-reduce + finalize, the CPHB_DEBUG_EVENTS event between the two instances
+    const bool pdl = !a.defer_finalize && !a.step_mode && !icp->dbg_ev;
+    with_kind(icp->prm.estimation, [&](auto k) {
+        with_top(icp->index->v.top, [&](auto t) {
+            constexpr int KIND = decltype(k)::value, TOP = decltype(t)::value;
+            if (pdl) {
+                launch_pdl(icp_iteration_kernel<KIND, TOP, 0>, icp->grid_search, ICP_SEARCH_WARPS * 32, s, a);
+                launch_pdl(icp_iteration_kernel<KIND, TOP, 1>, icp->grid, ICP_SEARCH_WARPS * 32, s, a);
+                return;
+            }
+            CPHB_LAUNCH((icp_iteration_kernel<KIND, TOP, 0>), icp->grid_search, ICP_SEARCH_WARPS * 32, 0, s, a);
+            if (icp->dbg_ev) cudaEventRecord(icp->dbg_ev[3 * a.launch_idx + 1], s);
+            CPHB_LAUNCH((icp_iteration_kernel<KIND, TOP, 1>), icp->grid, ICP_SEARCH_WARPS * 32, 0, s, a);
+        });
+    });
 }
-static void launch_iteration_kind(const cphb_icp *icp, const IcpArgs &a, cudaStream_t s) {
-    switch (icp->prm.estimation) {
-        case CPHB_EST_POINT_TO_POINT: launch_iteration<CPHB_EST_POINT_TO_POINT>(icp, a, s); break;
-        case CPHB_EST_POINT_TO_PLANE: launch_iteration<CPHB_EST_POINT_TO_PLANE>(icp, a, s); break;
-        case CPHB_EST_SYMMETRIC: launch_iteration<CPHB_EST_SYMMETRIC>(icp, a, s); break;
-        case CPHB_EST_COLORED_ICP: launch_iteration<CPHB_EST_COLORED_ICP>(icp, a, s); break;
-        case CPHB_EST_GENERALIZED_ICP: launch_iteration<CPHB_EST_GENERALIZED_ICP>(icp, a, s); break;
-    }
-}
-static void launch_finalize_kind(const cphb_icp *icp, const IcpArgs &a, cudaStream_t s) {
-    switch (icp->prm.estimation) {
-        case CPHB_EST_POINT_TO_POINT: CPHB_LAUNCH(icp_finalize_kernel<CPHB_EST_POINT_TO_POINT>, 1, 32, 0, s, a); break;
-        case CPHB_EST_POINT_TO_PLANE: CPHB_LAUNCH(icp_finalize_kernel<CPHB_EST_POINT_TO_PLANE>, 1, 32, 0, s, a); break;
-        case CPHB_EST_SYMMETRIC: CPHB_LAUNCH(icp_finalize_kernel<CPHB_EST_SYMMETRIC>, 1, 32, 0, s, a); break;
-        case CPHB_EST_COLORED_ICP: CPHB_LAUNCH(icp_finalize_kernel<CPHB_EST_COLORED_ICP>, 1, 32, 0, s, a); break;
-        case CPHB_EST_GENERALIZED_ICP: CPHB_LAUNCH(icp_finalize_kernel<CPHB_EST_GENERALIZED_ICP>, 1, 32, 0, s, a); break;
-    }
+static void launch_finalize(const cphb_icp *icp, const IcpArgs &a, cudaStream_t s) {
+    with_kind(icp->prm.estimation, [&](auto k) { CPHB_LAUNCH(icp_finalize_kernel<decltype(k)::value>, 1, 32, 0, s, a); });
 }
 
 extern "C" int cphb_icp_create(const cphb_cloud *source, const cphb_cloud *target, const cphb_icp_params *params,
@@ -279,25 +273,16 @@ extern "C" int cphb_icp_create(const cphb_cloud *source, const cphb_cloud *targe
         unsigned want = (n_tiles + ICP_SEARCH_WARPS - 1) / ICP_SEARCH_WARPS;
         // every block must be resident: warps start on a static tile, and a block waiting for an SM slot
         // would hold its four tiles back until the dynamic queue has drained
-        auto grid_for = [&](int occ, const char *hook) {
+        auto grid_for = [&](int occ) {
             unsigned per_sm = 9u;
             if (occ > 0 && (unsigned)occ < per_sm) per_sm = (unsigned)occ;
-            if (const char *e = getenv(hook)) {  // tuning hook
-                int v = atoi(e);
-                if (v >= 1 && v <= 32) per_sm = (unsigned)v;
-            }
             const unsigned cap = (unsigned)sms * per_sm;
             return want < cap ? want : cap;
         };
-        icp->grid_search = grid_for(iteration_occupancy_kind<0>(params->estimation, icp->index->v.top <= 3), "CPHB_ICP_SEARCH_BLOCKS_PER_SM");
-        icp->grid = grid_for(iteration_occupancy_kind<1>(params->estimation, icp->index->v.top <= 3), "CPHB_ICP_BLOCKS_PER_SM");
-        unsigned rg = (n_tiles + 63) / 64;
-        unsigned rg_cap = (unsigned)sms;
-        if (const char *e = getenv("CPHB_REDUCE_BLOCKS_PER_SM")) {  // tuning hook: more, shorter chains of tile sums
-            int v = atoi(e);
-            if (v >= 1 && v <= 8) rg_cap = (unsigned)sms * (unsigned)v;
-        }
-        icp->reduce_grid = rg < 1 ? 1 : (rg > rg_cap ? rg_cap : rg);
+        icp->grid_search = grid_for(iteration_occupancy_kind<0>(params->estimation, icp->index->v.top));
+        icp->grid = grid_for(iteration_occupancy_kind<1>(params->estimation, icp->index->v.top));
+        const unsigned rg = (n_tiles + 63) / 64;
+        icp->reduce_grid = rg < 1 ? 1 : (rg > (unsigned)sms ? (unsigned)sms : rg);
         if (icp->reduce_grid > icp->grid) icp->reduce_grid = icp->grid;  // the sum runs on blocks of the ROLE 1 launch
     }
     const bool want_nrm = params->estimation == CPHB_EST_SYMMETRIC && source->normals;
@@ -323,10 +308,6 @@ extern "C" int cphb_icp_create(const cphb_cloud *source, const cphb_cloud *targe
     const unsigned flag_words = n_pad / 1024 + 1;
     size_t o_fb = take(sizeof(unsigned) * 2 * flag_words);
     size_t o_prev = take(sizeof(int2) * n_pad);
-    size_t o_axyz = take(sizeof(float4) * n_pad), o_aprev = take(sizeof(int2) * n_pad);
-    size_t o_anrm = want_nrm ? take(sizeof(float4) * n_pad) : 0, o_acov = want_cov ? take(sizeof(float4) * 3 * n_pad) : 0;
-    size_t o_acol = want_col ? take(sizeof(float4) * n_pad) : 0, o_ccol = want_col ? take(sizeof(float4) * n_pad) : 0;
-    size_t o_rt = take(sizeof(uint32_t) * 4 * n_pad);
     const unsigned nf_pad = (unsigned)cphb_align(n_full ? n_full : 1, ICP_BLOCK);
     size_t o_ci = take(sizeof(int32_t) * nf_pad);
     unsigned cmp_blocks = (nf_pad + CMP_BLOCK - 1) / CMP_BLOCK;
@@ -352,16 +333,6 @@ extern "C" int cphb_icp_create(const cphb_cloud *source, const cphb_cloud *targe
     icp->flag_bits = (unsigned *)(b + o_fb);
     icp->flag_words = flag_words;
     icp->prev = (int2 *)(b + o_prev);
-    icp->alt_xyz = (float4 *)(b + o_axyz);
-    icp->alt_prev = (int2 *)(b + o_aprev);
-    icp->alt_nrm = want_nrm ? (float4 *)(b + o_anrm) : nullptr;
-    icp->alt_cov = want_cov ? (float4 *)(b + o_acov) : nullptr;
-    icp->alt_col = want_col ? (float4 *)(b + o_acol) : nullptr;
-    icp->cur_col = want_col ? (float4 *)(b + o_ccol) : nullptr;
-    icp->rt_keys = (uint32_t *)(b + o_rt);
-    icp->rt_keys2 = icp->rt_keys + n_pad;
-    icp->rt_vals = icp->rt_keys + 2 * (size_t)n_pad;
-    icp->rt_order = icp->rt_keys + 3 * (size_t)n_pad;
     icp->corr_index = (int32_t *)(b + o_ci);
     icp->cmp_counts = (unsigned *)(b + o_cc);
     icp->cmp_total = (unsigned *)(b + o_ct);
@@ -439,7 +410,6 @@ static void fill_args(const cphb_icp *icp, IcpArgs &a) {
     // of them (config 2 on the H100, profiles/h100_tuning_sweep.txt: 17 / 33 / 132 helper blocks -> 6429 / 7350 / 7330 it/s, the default
     // 66 -> 7145-7381 it/s over three runs)
     a.helper_blocks = icp->grid >= 64 ? (icp->grid / 8 > 2 ? icp->grid / 8 : 2) : 0;
-    if (const char *e = getenv("CPHB_HELPER_BLOCKS")) { int v = atoi(e); if (v >= 0 && (unsigned)v < icp->grid / 2) a.helper_blocks = (unsigned)v; }
     a.prev = icp->prev;
     a.n_src = icp->n_src;
     a.n_pad = icp->n_pad;
@@ -463,14 +433,9 @@ static void fill_args(const cphb_icp *icp, IcpArgs &a) {
     a.r_up = (float)(sqrt((double)a.r2) * 1.00002);
     a.dbg = icp->dbg;
     a.claim_max = 8u;
-    if (const char *e = getenv("CPHB_CLAIM_MAX")) { int v = atoi(e); if (v >= 1 && v <= 1024) a.claim_max = (unsigned)v; }
     a.static_sched = 1;  // config 2 on the H100: 7145-7381 it/s vs 6870 with the dynamic schedule (profiles/h100_tuning_sweep.txt)
     if (const char *e = getenv("CPHB_STATIC_SCHED")) a.static_sched = atoi(e) != 0;
     a.tmax = CPHB_TRANSPOSE_MAX;
-    if (const char *e = getenv("CPHB_TRANSPOSE_MAX")) {  // tuning hook
-        int v = atoi(e);
-        if (v >= 0 && v <= 32) a.tmax = v;
-    }
 }
 
 static int reset_working_copy(cphb_icp *icp, cudaStream_t s) {
@@ -492,34 +457,6 @@ static int compact_correspondences(cphb_icp *icp, int32_t *corr_out, cudaStream_
     CPHB_LAUNCH(compact_scan_kernel, 1, 1024, 0, s, icp->cmp_counts, nb, icp->cmp_total);
     CPHB_LAUNCH(compact_write_kernel, nb, CMP_BLOCK, 0, s, icp->corr_index, n, icp->cmp_counts, corr_out);
     CPHB_CHECK_LAUNCH();
-    return CPHB_OK;
-}
-
-// permute the working arrays referenced by `a` into the alt buffers and swap
-static int retile(cphb_icp *icp, IcpArgs &a, cudaStream_t s) {
-    const unsigned n_pad = icp->n_pad, grid = n_pad / 256;
-    const uint32_t n_tgt_pad = (uint32_t)icp->index->v.n_leaves * CPHB_LEAF;
-    CPHB_LAUNCH(retile_key_kernel, grid, 256, 0, s, a.prev, icp->n_src, n_pad, n_tgt_pad, icp->rt_keys, icp->rt_vals);
-    CPHB_CHECK_LAUNCH();
-    // keys are target LEAVES (< n_tgt_pad / 32) or the two sentinels right above them: the stable radix sort only
-    // has to look at the bits that can differ (16 for 1 M points: 2 onesweep passes)
-    int bits = 1;
-    while (bits < 32 && ((uint64_t)1 << bits) < (uint64_t)(n_tgt_pad >> 5) + 2u) ++bits;
-    int rc = cphb_sort_pairs_u32(icp->rt_keys, icp->rt_keys2, icp->rt_vals, icp->rt_order, n_pad, bits, s);
-    if (rc) return rc;
-    float4 *o_xyz = (a.src == icp->work_xyz) ? icp->alt_xyz : icp->work_xyz;
-    int2 *o_prev = (a.prev == icp->prev) ? icp->alt_prev : icp->prev;
-    float4 *o_nrm = a.src_nrm ? ((a.src_nrm == icp->work_nrm) ? icp->alt_nrm : icp->work_nrm) : nullptr;
-    float4 *o_cov = a.src_cov ? ((a.src_cov == icp->work_cov) ? icp->alt_cov : icp->work_cov) : nullptr;
-    float4 *o_col = a.src_col ? ((a.src_col == icp->alt_col) ? icp->cur_col : icp->alt_col) : nullptr;
-    CPHB_LAUNCH(retile_gather_kernel, grid, 256, 0, s, icp->rt_order, n_pad, a.src, a.prev, a.src_nrm, a.src_col, a.src_cov,
-                o_xyz, o_prev, o_nrm, o_col, o_cov);
-    CPHB_CHECK_LAUNCH();
-    a.src = o_xyz;
-    a.prev = o_prev;
-    a.src_nrm = o_nrm;
-    a.src_cov = o_cov;
-    a.src_col = o_col;
     return CPHB_OK;
 }
 
@@ -600,12 +537,6 @@ extern "C" int cphb_icp_run(cphb_icp *icp, const float h_init[16], cphb_comm *co
     // j < max_iter, launch j+1 re-runs that search only to materialise its correspondences;
     // launches after "done" exit at their first instruction.
     const unsigned long long launches0 = g_cphb_launches;
-    // Re-tiling (the working copy re-ordered by the target position of every point's current match) after the launches
-    // whose bit is set.  It paid for itself while the rows were gathered through the caller's arrays; with the target
-    // attributes in index order and the certified regime's cp.async row pipeline a re-tiling is no longer earned back
-    // (config 2 on the H100: mask 0x12 / 0x4 -> 7059 / 7135 it/s, none -> 7145-7381; profiles/h100_tuning_sweep.txt), so the default is none.
-    unsigned long long retile_mask = 0ull;
-    if (const char *e = getenv("CPHB_RETILE_MASK")) retile_mask = strtoull(e, nullptr, 0);  // tuning hook
     static const bool dbg_events = getenv("CPHB_DEBUG_EVENTS") != nullptr;
     std::vector<cudaEvent_t> evs;
     if (dbg_events) {
@@ -617,16 +548,12 @@ extern "C" int cphb_icp_run(cphb_icp *icp, const float h_init[16], cphb_comm *co
     for (int it = 0; it <= a.max_iter; ++it) {
         a.launch_idx = it;
         if (dbg_events) cudaEventRecord(evs[3 * it], s);
-        launch_iteration_kind(icp, a, s);
+        launch_iteration(icp, a, s);
         if (dbg_events) cudaEventRecord(evs[3 * it + 2], s);
         if (nccl_comm) {
             rc = cphb_nccl_allreduce_f64(nccl_comm, icp->st->local, icp->st->total, 32, s);
             if (rc) return rc;
-            launch_finalize_kind(icp, a, s);
-        }
-        if (!(icp->prm.flags & CPHB_ICP_NO_RETILE) && it < a.max_iter && it < 64 && ((retile_mask >> it) & 1ull) && icp->n_src >= 4096) {
-            rc = retile(icp, a, s);
-            if (rc) return rc;
+            launch_finalize(icp, a, s);
         }
     }
     CPHB_CUDA(cudaEventRecord(icp->ev1, s));
@@ -712,7 +639,7 @@ extern "C" int cphb_icp_step(cphb_icp *icp, const float h_T[16], double h_sums[3
     a.step_mode = 1;
     a.corr_index = icp->corr_index;
     CPHB_CUDA(cudaMemsetAsync(icp->corr_index, 0xff, sizeof(int32_t) * icp->n_full, s));
-    launch_iteration_kind(icp, a, s);
+    launch_iteration(icp, a, s);
     CPHB_CHECK_LAUNCH();
     if (corr_index)
         CPHB_CUDA(cudaMemcpyAsync(corr_index, icp->corr_index, sizeof(int32_t) * icp->n_full, cudaMemcpyDeviceToDevice, s));
@@ -906,26 +833,19 @@ static int run_estimate(int estimation, const cphb_cloud *source, const cphb_clo
     a.ticket = (unsigned *)((char *)a.total + 256);
     float *Td = (float *)((char *)a.total + 512);
     CPHB_CUDA(cudaMemsetAsync(a.ticket, 0, 4, s));
-    bool have = true;
-    switch (estimation) {
-        case CPHB_EST_POINT_TO_POINT: CPHB_LAUNCH(estimate_kernel<CPHB_EST_POINT_TO_POINT>, grid, ICP_BLOCK, 0, s, a); break;
-        case CPHB_EST_POINT_TO_PLANE: have = target->normals; CPHB_LAUNCH(estimate_kernel<CPHB_EST_POINT_TO_PLANE>, grid, ICP_BLOCK, 0, s, a); break;
-        case CPHB_EST_SYMMETRIC: have = target->normals && source->normals; CPHB_LAUNCH(estimate_kernel<CPHB_EST_SYMMETRIC>, grid, ICP_BLOCK, 0, s, a); break;
-        case CPHB_EST_COLORED_ICP: have = target->normals && target->colors && source->colors; CPHB_LAUNCH(estimate_kernel<CPHB_EST_COLORED_ICP>, grid, ICP_BLOCK, 0, s, a); break;
-        case CPHB_EST_GENERALIZED_ICP: have = target->covariances && source->covariances; CPHB_LAUNCH(estimate_kernel<CPHB_EST_GENERALIZED_ICP>, grid, ICP_BLOCK, 0, s, a); break;
-    }
-    if (h_T) {
-        float dt = params ? params->det_thresh : 1e-6f;
-        unsigned long long nm = source->n;
-        switch (estimation) {
-            case CPHB_EST_POINT_TO_POINT: CPHB_LAUNCH(estimate_solve_kernel<CPHB_EST_POINT_TO_POINT>, 1, 32, 0, s, a.total, nm, dt, have, Td); break;
-            case CPHB_EST_POINT_TO_PLANE: CPHB_LAUNCH(estimate_solve_kernel<CPHB_EST_POINT_TO_PLANE>, 1, 32, 0, s, a.total, nm, dt, have, Td); break;
-            case CPHB_EST_SYMMETRIC: CPHB_LAUNCH(estimate_solve_kernel<CPHB_EST_SYMMETRIC>, 1, 32, 0, s, a.total, nm, dt, have, Td); break;
-            case CPHB_EST_COLORED_ICP: CPHB_LAUNCH(estimate_solve_kernel<CPHB_EST_COLORED_ICP>, 1, 32, 0, s, a.total, nm, dt, have, Td); break;
-            case CPHB_EST_GENERALIZED_ICP: CPHB_LAUNCH(estimate_solve_kernel<CPHB_EST_GENERALIZED_ICP>, 1, 32, 0, s, a.total, nm, dt, have, Td); break;
-        }
-        CPHB_CUDA(cudaMemcpyAsync(h_T, Td, 64, cudaMemcpyDeviceToHost, s));
-    }
+    // the inputs the estimator needs are present (otherwise the solve leaves the identity)
+    const bool have = estimation == CPHB_EST_POINT_TO_PLANE ? target->normals != nullptr
+                      : estimation == CPHB_EST_SYMMETRIC    ? target->normals && source->normals
+                      : estimation == CPHB_EST_COLORED_ICP  ? target->normals && target->colors && source->colors
+                      : estimation == CPHB_EST_GENERALIZED_ICP ? target->covariances && source->covariances
+                                                               : true;
+    const float dt = params ? params->det_thresh : 1e-6f;
+    const unsigned long long nm = source->n;
+    with_kind(estimation, [&](auto k) {
+        CPHB_LAUNCH(estimate_kernel<decltype(k)::value>, grid, ICP_BLOCK, 0, s, a);
+        if (h_T) CPHB_LAUNCH(estimate_solve_kernel<decltype(k)::value>, 1, 32, 0, s, a.total, nm, dt, have, Td);
+    });
+    if (h_T) CPHB_CUDA(cudaMemcpyAsync(h_T, Td, 64, cudaMemcpyDeviceToHost, s));
     CPHB_CHECK_LAUNCH();
     CPHB_CUDA(cudaMemcpyAsync(h_S, a.total, sizeof(double) * 32, cudaMemcpyDeviceToHost, s));
     CPHB_CUDA(cudaStreamSynchronize(s));

@@ -1,4 +1,4 @@
-// icp_aux.cuh -- working-copy kernels of the loop: source gather, re-tiling, correspondence compaction, PointCloud::Transform
+// icp_aux.cuh -- working-copy kernels of the loop: source gather, correspondence compaction, PointCloud::Transform
 // Part of the icp.cu translation unit (included there); split out for readability only.
 #pragma once
 
@@ -65,43 +65,6 @@ __global__ void __launch_bounds__(256) gather_target_kernel(const float4 *__rest
                                      : cov_col_major ? make_float4(c[r], c[3 + r], c[6 + r], 0.f)
                                                      : make_float4(c[3 * r], c[3 * r + 1], c[3 * r + 2], 0.f);
     }
-}
-
-// ---------------------------------------------------------------------------
-// Re-tiling: once the clouds are roughly aligned, re-order the working copy by the Hilbert position of
-// each point's current match, so that a warp's 32 queries fall into one or two target leaves instead
-// of straddling a dozen.  Pure permutation of the working arrays (w / prev travel with the point): the
-// result set is unchanged, only the order in which exact products are added to the float64 sums.
-// ---------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) retile_key_kernel(const int2 *__restrict__ prev, unsigned n_src, unsigned n_pad,
-                                                         uint32_t n_tgt_pad, uint32_t *keys, uint32_t *vals) {
-    unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n_pad) return;
-    uint32_t k = (n_tgt_pad >> 5) + 1u;  // padding stays last
-    if (i < n_src) {
-        const int pp = prev[i].x;  // index position of the match
-        // by LEAF of the match (the order inside a leaf does not matter for locality, and the stable sort keeps it
-        // deterministic): 5 key bits less = one radix pass less at 1 M points.  Unmatched points after the matched ones
-        k = (pp >= 0) ? ((uint32_t)pp >> 5) : (n_tgt_pad >> 5);
-    }
-    keys[i] = k;
-    vals[i] = i;
-}
-__global__ void __launch_bounds__(256) retile_gather_kernel(const uint32_t *__restrict__ order, unsigned n_pad,
-                                                            const float4 *__restrict__ xyz, const int2 *__restrict__ prev,
-                                                            const float4 *__restrict__ nrm, const float4 *__restrict__ col,
-                                                            const float4 *__restrict__ cov, float4 *o_xyz, int2 *o_prev,
-                                                            float4 *o_nrm, float4 *o_col, float4 *o_cov) {
-    unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n_pad) return;
-    const unsigned s = order[i];
-    o_xyz[i] = xyz[s];
-    o_prev[i] = prev[s];
-    if (nrm) o_nrm[i] = nrm[s];
-    if (col) o_col[i] = col[s];
-    if (cov)
-#pragma unroll
-        for (int r = 0; r < 3; ++r) o_cov[(size_t)r * n_pad + i] = cov[(size_t)r * n_pad + s];
 }
 
 // stable compaction of (i, corr_index[i]) with corr_index[i] >= 0 (registration.cu:54-69)

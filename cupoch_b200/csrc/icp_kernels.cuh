@@ -33,40 +33,17 @@ template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 // certified regime: software pipeline depth.  Tile T's target rows are requested ICP_GD tiles ahead (that needs tile T's
 // match position, i.e. its stage), the (point, match, slack) stages ICP_NS = 2 * ICP_GD tiles ahead.
-#ifndef ICP_GD
 #define ICP_GD 2
-#endif
 #define ICP_NS (2 * ICP_GD)
 // Certified regime: the normal-equation sums of a tile on the FP64 tensor cores.  The 30 products a tile contributes per
 // row are entries of the Gram matrix of the 32 x 8 matrix V = (J0..J5, r, one): eight DMMA.8x8x4 (A = V^T, B = V, four
 // points per step; for a Gram matrix both fragments hold the SAME value per lane) accumulate it in a 2-register
 // fragment per lane -- instead of 30 float64 accumulators (60 registers) per lane and a 30-column warp reduction at
 // the end.  Products of two floats are exact in float64 and every accumulation step rounds once, exactly as DFMA does;
-// only the (fixed) order of the additions differs.  -DICP_DMMA=0 restores the per-lane DFMA accumulators.
-#ifndef ICP_DMMA
-#define ICP_DMMA 1
-#endif
-// float -> double.  F2F.F64.F32 runs on the XU pipe (shared with MUFU), which nine conversions per row keep busy in a
-// certified launch; the widening is exact, so it can also be done on the integer pipes (re-bias the exponent, shift the
-// mantissa by 29 bits; zero keeps its sign; denormals / inf / NaN take the hardware path).  Measured on config 2 (H100,
-// profiles/h100_tuning_sweep.txt): 7216 it/s with the integer form vs 7069 for the same build without it, inside the +-2 % run-to-run
-// spread, so the hardware conversion stays the default; -DICP_F2D_INT=1 selects the integer form.
-#ifndef ICP_F2D_INT
-#define ICP_F2D_INT 0
-#endif
-__device__ __forceinline__ double f2d(float f) {
-#if ICP_F2D_INT
-    const unsigned u = __float_as_uint(f);
-    const unsigned a = u & 0x7fffffffu;
-    if (a - 0x00800000u >= 0x7f000000u) {  // a < 2^-126 (zero, denormal) or a >= inf
-        if (a == 0u) return __hiloint2double((int)u, 0);
-        return (double)f;
-    }
-    return __hiloint2double((int)((u & 0x80000000u) | ((a >> 3) + 0x38000000u)), (int)(u << 29));
-#else
-    return (double)f;
-#endif
-}
+// only the (fixed) order of the additions differs.
+// float -> double: the hardware conversion (F2F.F64.F32 on the XU pipe).  An exact integer-pipe form measured inside the
+// +-2 % run-to-run spread (config 2 on the H100, profiles/h100_tuning_sweep.txt: 7216 it/s vs 7069).
+__device__ __forceinline__ double f2d(float f) { return (double)f; }
 __device__ __forceinline__ void dmma_8x8x4(double &c0, double &c1, double a, double b) {
     asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};" : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
 }
@@ -80,54 +57,29 @@ __device__ __forceinline__ void prefetch_target(const IcpArgs &a, size_t p) {
     if (KIND == CPHB_EST_GENERALIZED_ICP && a.tgt_cov) prefetch_l1(a.tgt_cov + 3 * p);  // 48 B: one or two sectors
 }
 
-#ifndef ICP_DMMA
-#define ICP_DMMA 1  // certified regime: normal-equation sums on the FP64 tensor cores (see dmma_8x8x4 below)
-#endif
 #define ICP_SEARCH_WARPS 4
 // Two instances of the kernel, launched back to back every iteration (the regime is decided on the DEVICE, so each
 // instance checks the state and the one whose regime is not current leaves at once):
 //   ROLE 0  searching regime.  The traversal is bound by instruction issue at low occupancy, so it is compiled for MORE
 //           resident warps (96 registers: 5 blocks = 20 warps / SM).
-//   ROLE 1  certified regime (needs the registers: 30 float64 accumulators per lane) -- and, when the launch before it
-//           searched, the fixed-order sum of its tile sums + solve (what used to be a third kernel, icp_reduce_kernel).
-#ifndef ICP_MIN_BLOCKS
-// ROLE 1: 4 blocks = 16 warps / SM.  The tensor-core accumulation would allow 24-32 warps (80-64 registers), but more
-// resident blocks buy nothing (config 2 on the H100, profiles/h100_tuning_sweep.txt: compiled for 6 blocks 7188 it/s vs 7069 for the same
-// build at 4, a grid of 2 / 3 blocks per SM 7166 / 7395, all inside the +-2 % spread): the certified launch's SM
-// throughput saturates near 16 warps and every extra block adds launch, pipeline-fill and grid-sum work.
+//   ROLE 1  certified regime (the normal-equation sums of its tiles go into one 8 x 8 DMMA Gram fragment per warp, see
+//           dmma_8x8x4) -- and, when the launch before it searched, the fixed-order sum of its tile sums + solve (what
+//           used to be a third kernel, icp_reduce_kernel).
+// ROLE 1: 4 blocks = 16 warps / SM.  The Gram fragment is two registers per lane, so the registers would allow 24-32
+// warps (80-64 registers), but more resident blocks buy nothing (config 2 on the H100, profiles/h100_tuning_sweep.txt:
+// compiled for 6 blocks 7188 it/s vs 7069 for the same build at 4, a grid of 2 / 3 blocks per SM 7166 / 7395, all inside
+// the +-2 % spread): the certified launch's SM throughput saturates near 16 warps and every extra block adds launch,
+// pipeline-fill and grid-sum work.
 #define ICP_MIN_BLOCKS 4
-#endif
-#ifndef ICP_MIN_BLOCKS_SEARCH
 // ROLE 0: 96 registers = 20 warps / SM.  Config 2 on the H100 (profiles/h100_tuning_sweep.txt): a grid of 3 / 4 blocks per SM 6576 / 7047
 // it/s; compiled for 4 / 6 blocks 7058 / 7214 it/s against 7069 for the same build at 5.
 #define ICP_MIN_BLOCKS_SEARCH 5
-#endif
 // Programmatic dependent launch: the kernels of the loop are launched with stream serialisation relaxed, so the next
 // kernel's blocks are already resident (waiting in griddepcontrol.wait) while the last block of the current one sums and
-// solves: the launch latency of every kernel boundary is hidden (+3.5 % on config 2; -DCPHB_PDL=0 or CPHB_NO_PDL=1 disable)
-#ifndef CPHB_PDL
-#define CPHB_PDL 1
-#endif
-__device__ __forceinline__ void grid_dependency_wait() {
-#if CPHB_PDL
-    asm volatile("griddepcontrol.wait;" ::: "memory");
-#endif
-}
-__device__ __forceinline__ void grid_dependency_trigger() {
-#if CPHB_PDL
-    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-#endif
-}
+// solves: the launch latency of every kernel boundary is hidden (+3.5 % on config 2)
+__device__ __forceinline__ void grid_dependency_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
-// closed forms of c_pair_jtj / c_pair_p2p (icp_types.cuh) for compile-time unrolling
-__host__ __device__ constexpr int pair_jtj_a(int p) {
-    return p < 6 ? 0 : p < 11 ? 1 : p < 15 ? 2 : p < 18 ? 3 : p < 20 ? 4 : p < 21 ? 5 : p < 27 ? p - 21 : p == 27 ? 6 : p == 28 ? 7 : 8;
-}
-__host__ __device__ constexpr int pair_jtj_b(int p) {
-    return p < 6 ? p : p < 11 ? p - 5 : p < 15 ? p - 9 : p < 18 ? p - 12 : p < 20 ? p - 14 : p < 21 ? 5 : p < 28 ? 6 : 8;
-}
-__host__ __device__ constexpr int pair_p2p_a(int p) { return p < 6 ? p : p < 15 ? (p - 6) / 3 : p == 28 ? 7 : 8; }
-__host__ __device__ constexpr int pair_p2p_b(int p) { return p < 6 ? 8 : p < 15 ? 3 + (p - 6) % 3 : 8; }
+// the columns of the 32-double sums layout (icp_types.cuh) that an estimator fills
 __host__ __device__ constexpr bool pair_live(bool p2p, int p) { return p2p ? (p < 15 || p == 28 || p == 29) : p < 30; }
 
 // the target-side values of index position p (tp = ix.pts[p] is already in registers)
@@ -228,7 +180,7 @@ __device__ __forceinline__ void lane_writeback(const IcpArgs &a, const LaunchCtx
         for (int r = 0; r < 3; ++r) a.src_cov[(size_t)r * a.n_pad + i] = make_float4(Cs[3 * r], Cs[3 * r + 1], Cs[3 * r + 2], 0.f);
 }
 
-// Warm start + certificate (DESIGN.md 3.1.9).  prev[i].y is a lower bound (rounded down) on the distance from this point's
+// Warm start + certificate (DESIGN.md 3.1.8).  prev[i].y is a lower bound (rounded down) on the distance from this point's
 // position at the time it was last searched (minus the displacements since) to every target point other than its match.
 // If, after this iteration's displacement, the old match is still strictly closer than that bound, no other point can
 // have a smaller (d2, index) key: the search would return the same match, so the lane skips it.  All roundings go
@@ -472,7 +424,7 @@ icp_iteration_kernel(const __grid_constant__ IcpArgs a) {
 
     IcpState *st = a.st;
     const int warp = threadIdx.x >> 5, lane = lane_id();
-    grid_dependency_wait();  // (PDL builds) everything below reads state the previous launch wrote
+    grid_dependency_wait();  // everything below reads state the previous launch wrote
     // the per-launch state: ONE warp instruction per block fetches the 15 words (a few thousand warps reading the same
     // line one word at a time serialise in its L2 slice: ~20 % of a certified launch's warp time before this)
     __shared__ unsigned s_hdr[16];
@@ -534,13 +486,14 @@ icp_iteration_kernel(const __grid_constant__ IcpArgs a) {
         if (lane == 0) { dbg_time(a, 0, true); dbg_time(a, 11, false); }
         // ======================= certified regime ==================================================================
         // Every tile whose 32 lanes are certified (99.7 % of them on config 2): transform, certificate test, rows, products
-        // into this lane's float64 accumulators.  A tile with an uncertified lane goes through the searching regime's
-        // per-tile routine instead; the accumulators are folded into the warp's running row first, so they are dead while
-        // the search runs (no spills) -- the fold points depend on the data only, so the sums stay reproducible.
-        // Software pipeline, two tiles deep, without tying up registers (the 30 float64 accumulators need them): the point
-        // and the (match, slack) pair of the tile AFTER NEXT travel global -> shared memory by cp.async while the current
-        // tile is processed; at the top of a tile the next tile's match positions are read back from shared memory and
-        // the target rows they point to are pulled into L1, so those have a whole tile to arrive.
+        // into the warp's 8 x 8 Gram fragment on the FP64 tensor cores.  A tile with an uncertified lane goes through the
+        // searching regime's per-tile routine instead and its sums are added to the warp's running row; the fragment
+        // (three registers with the d2 sum) stays live across the search -- which tiles take that path depends on the data
+        // only, so the sums stay reproducible.
+        // Software pipeline, two tiles deep, without tying up registers: the point and the (match, slack) pair of the tile
+        // AFTER NEXT travel global -> shared memory by cp.async while the current tile is processed; at the top of a tile
+        // the next tile's match positions are read back from shared memory and the target rows they point to are pulled
+        // into L1, so those have a whole tile to arrive.
         // Tiles that needed a search in the LAST certified launch (a stable set: the same near-equidistant points every
         // iteration) are flagged in a bitmap.  The last `helper_blocks` blocks of the grid run exactly those tiles, bitmap
         // word by bitmap word (a fixed assignment), from the first microsecond of the launch; the other warps skip them,
@@ -577,15 +530,9 @@ icp_iteration_kernel(const __grid_constant__ IcpArgs a) {
             return;
         }
         // ---- main role ----
-#if ICP_DMMA
         double gc0 = 0.0, gc1 = 0.0;  // this lane's two elements of the warp's 8 x 8 Gram fragment: G[lane/4][2 (lane%4) + {0,1}]
         double d2acc = 0.0;           // this lane's sum of d2 (not an entry of the Gram matrix of V)
         float *stage = reinterpret_cast<float *>(s_rows[warp]);  // [32 points][8] floats (the searching code's row buffer, idle here)
-#else
-        double lacc[32];
-#pragma unroll
-        for (int p = 0; p < 32; ++p) lacc[p] = 0.0;
-#endif
         double wrow = 0.0;  // lane p: column p of what this warp has folded so far
         unsigned n_skipped = 0;
         bool searched_inline = false;
@@ -677,9 +624,8 @@ icp_iteration_kernel(const __grid_constant__ IcpArgs a) {
             if (c.materialize) continue;  // fitness / rmse / T of this pose are already in the state
             float J[NROWS][6], r[NROWS];
             lane_rows_vals<KIND, NROWS>(a, found, tv, s, sn, Cs, i, J, r);
-            // this lane's own rows, every product into its own float64 accumulator (exact products, one rounding per
-            // addition); the warp-wide reduction happens once, after the last tile
-#if ICP_DMMA
+            // the warp's rows into its Gram fragment (exact products, one rounding per addition); the fragment is read
+            // out once, after the last tile
 #pragma unroll
             for (int q = 0; q < NROWS; ++q) {
                 __syncwarp();  // every lane has read the previous row's stage
@@ -693,35 +639,11 @@ icp_iteration_kernel(const __grid_constant__ IcpArgs a) {
                 }
             }
             if (found) d2acc += f2d(d2);
-#else
-#pragma unroll
-            for (int q = 0; q < NROWS; ++q) {
-                const double v[9] = {(double)J[q][0], (double)J[q][1], (double)J[q][2], (double)J[q][3], (double)J[q][4],
-                                     (double)J[q][5], (double)r[q], (q == 0 && found) ? (double)d2 : 0.0,
-                                     (q == 0 && found) ? 1.0 : 0.0};
-#pragma unroll
-                for (int p = 0; p < 32; ++p)
-                    if (pair_live(P2P, p))
-                        lacc[p] = fma(v[P2P ? pair_p2p_a(p) : pair_jtj_a(p)], v[P2P ? pair_p2p_b(p) : pair_jtj_b(p)], lacc[p]);
-            }
-#endif
         }
         if (!cold) break;
-        // ---- cold: tile `tile` needs its search.  The accumulators are folded into the warp's running row first, so
-        // they are dead while the search runs; then the hot loop resumes with the next tile.
+        // ---- cold: tile `tile` needs its search, its sums go into the warp's running row; then the hot loop resumes
+        // with the next tile.
         if (lane == 0) atomicOr(&flag_next[tile >> 5], 1u << (tile & 31));
-#if !ICP_DMMA
-        if (!c.materialize) {
-#pragma unroll
-            for (int p = 0; p < 32; ++p) {
-                if (!pair_live(P2P, p)) continue;
-                double t = lacc[p];
-#pragma unroll
-                for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(CPHB_FULL, t, o);
-                if (lane == p) wrow += t;
-            }
-        }
-#endif
         {   // (the Gram fragment is three registers: it simply stays live across the search)
             double acc;
             __syncwarp();
@@ -730,18 +652,13 @@ icp_iteration_kernel(const __grid_constant__ IcpArgs a) {
             wrow += acc;
             __syncwarp();
         }
-#if !ICP_DMMA
-#pragma unroll
-        for (int p = 0; p < 32; ++p) lacc[p] = 0.0;
-#endif
         if (a.dbg && lane == 0) atomicAdd(&a.dbg[128 + min(a.launch_idx, 63)], 1u);
         tile += main_warps;
         }
         cp_async_wait_0();
         if (lane == 0) { dbg_time(a, 1, false); dbg_time(a, searched_inline ? 9 : 8, false); }
-        // warp reduction (xor butterfly: the same bits on every lane), lane p keeps column p
+        // lane p keeps column p
         double row = wrow;
-#if ICP_DMMA
         if (!c.materialize) {
             // the fragment IS the warp's sum: lay the 8 x 8 matrix out in shared memory and let lane p pick the entry
             // of its column pair (JTJ kinds: columns 0..6 = J0..J5, r; 7 = one.  P2P: 0..5 = s, t; 7 = one)
@@ -764,18 +681,6 @@ icp_iteration_kernel(const __grid_constant__ IcpArgs a) {
             }
             if (pair_live(P2P, lane)) row += g;
         }
-#else
-        if (!c.materialize) {
-#pragma unroll
-            for (int p = 0; p < 32; ++p) {
-                if (!pair_live(P2P, p)) continue;
-                double t = lacc[p];
-#pragma unroll
-                for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(CPHB_FULL, t, o);
-                if (lane == p) row += t;
-            }
-        }
-#endif
         icp_static_tail<KIND>(a, st, (double(*)[32])s_pipe, s_solve, &s_flag, row, c.materialize, n_skipped);
         return;
     } else {

@@ -70,7 +70,7 @@ struct IcpArgs {
     int use_p2p;         // multi-GPU over the fused peer-memory exchange
     P2pView p2p;
     int step_mode;       // debug hook: one search + sums, no solve
-    int tmax;            // transposed-scan threshold (tuning hook)
+    int tmax;            // transposed-scan threshold (CPHB_TRANSPOSE_MAX)
 };
 
 // sums layout (32 doubles): JTJ kinds: 0..20 JTJ upper | 21..26 JTr | 27 r^2 | 28 sum d2 | 29 count

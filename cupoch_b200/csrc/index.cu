@@ -494,12 +494,11 @@ int cphb_hilbert_order_n(const float *xyz, size_t n, uint32_t *perm_out, float *
     // Curve resolution by cloud size: ceil(log2(n) / 3) + 1 levels (3 bits each), i.e. >= 8 curve cells per point of a
     // volume-filling cloud; 1 M points -> 8 levels = 24-bit keys = 3 radix passes instead of 4.  The order only has to
     // cluster (every search is exact whatever the order; groups of 1024 are kd-refined afterwards), equal keys keep their
-    // original order (stable sort).  CPHB_HILBERT_LEVELS overrides (tuning hook).
+    // original order (stable sort).
     int levels = 1;
     while (levels < 10 && ((size_t)1 << (3 * levels)) < (n_ref ? n_ref : n)) ++levels;
     levels = levels + 1 > 10 ? 10 : levels + 1;
     if (levels < 4) levels = 4;
-    if (const char *e = getenv("CPHB_HILBERT_LEVELS")) { int v = atoi(e); if (v >= 1 && v <= 10) levels = v; }
     CPHB_LAUNCH(hilbert_key_kernel, (unsigned)((n + 255) / 256), 256, 0, s, xyz, n, b, 30 - 3 * levels, keys, vals);
     CPHB_CHECK_LAUNCH();
     rc = cphb_sort_pairs_u32(keys, keys2, vals, perm_out, n, 3 * levels, s);

@@ -139,10 +139,6 @@ class RegistrationResult:  # registration.h:51-67
                 % (self.fitness, self.inlier_rmse, self._n_corr if self._corr_dev is not None else len(self._corr_host)))
 
 
-ICP_NO_RETILE = 2   # CPHB_ICP_NO_RETILE
-DEFAULT_FLAGS = 0   # OR of ICP_* flags applied to every registration (ablation / debugging)
-
-
 def _params(estimation, max_distance, criteria, shard=None):
     p = _lib.IcpParams()
     p.shard_rank, p.shard_world = (int(shard[0]), int(shard[1])) if shard else (0, 0)
@@ -153,7 +149,7 @@ def _params(estimation, max_distance, criteria, shard=None):
     p.max_iteration = criteria.max_iteration
     p.det_thresh = getattr(estimation, "det_thresh", -1.0)
     p.lambda_geometric = getattr(estimation, "lambda_geometric", 0.968)
-    p.flags = DEFAULT_FLAGS
+    p.flags = 0
     return p
 
 

@@ -217,7 +217,7 @@ typedef struct cphb_icp_params {
     int max_iteration;
     float det_thresh;             /* PointToPlane / Symmetric / Colored: 1e-6; ignored for GICP */
     float lambda_geometric;       /* Colored ICP, default 0.968 */
-    int flags;                    /* CPHB_ICP_* */
+    int flags;                    /* reserved, ignored (keeps the struct layout) */
     /* Multi-GPU: with shard_world > 1 every rank passes the FULL source; the library orders it along the
      * Hilbert curve and keeps the shard_rank-th contiguous block of that order (a spatially compact
      * shard at full density).  correspondence indices stay global.  0/0 or 1 = no library-side sharding
@@ -225,8 +225,6 @@ typedef struct cphb_icp_params {
     int shard_rank;
     int shard_world;
 } cphb_icp_params;
-
-#define CPHB_ICP_NO_RETILE 2 /* keep the source in its initial Hilbert order for the whole run (debug/ablation) */
 
 typedef struct cphb_icp_result {
     float transformation[16];     /* row-major */

@@ -90,15 +90,25 @@ def _compare(res, ref, pose_tol=POSE_TOL, exact_corr=True):
     return d
 
 
-def test_icp_p2plane(orc):
-    src, sn, tgt, tn = small_pair()
-    crit = R.ICPConvergenceCriteria(0, 0, 12)
+def _check_icp_p2plane(orc, n, iterations):
+    src, sn, tgt, tn = small_pair(n=n)
+    crit = R.ICPConvergenceCriteria(0, 0, iterations)
     res = R.registration_icp(cloud(src), cloud(tgt, tn), 0.03, np.eye(4), R.TransformationEstimationPointToPlane(), crit)
-    ref = orc.registration_icp(orc.P2PLANE, src, tgt, 0.03, tgt_nrm=tn, relative_fitness=0, relative_rmse=0, max_iteration=12)
+    ref = orc.registration_icp(orc.P2PLANE, src, tgt, 0.03, tgt_nrm=tn, relative_fitness=0, relative_rmse=0,
+                               max_iteration=iterations)
     _compare(res, ref)
     gt = datagen.gt_transform((-1.0, 1.5, 2.0), (0.01, -0.005, 0.008))
     assert np.linalg.norm(res.transformation - gt) < 2e-3   # and it actually registers
     assert res.fitness > 0.99
+
+
+def test_icp_p2plane(orc):
+    _check_icp_p2plane(orc, 20000, 12)
+
+
+def test_icp_p2plane_30k(orc):
+    """A larger cloud and a longer run (30 000 points, 14 iterations) on the default path, against the same oracle."""
+    _check_icp_p2plane(orc, 30000, 14)
 
 
 def test_icp_p2plane_init_and_convergence(orc):
@@ -200,30 +210,6 @@ def test_icp_1m_properties():
     i, j = a.correspondence_set[:, 0], a.correspondence_set[:, 1]
     assert (np.diff(i) > 0).all() and j.min() >= 0 and j.max() < n          # ascending in i, valid j
     ctx.close()
-
-
-def test_retiling_does_not_change_results(orc, monkeypatch):
-    """Re-ordering the working copy by matched target position (CPHB_RETILE_MASK; round 1's schedule 0x12, off by default
-    since round 2) is a pure permutation: same pose bits, same correspondence set, with and without it (and both equal
-    the oracle)."""
-    src, sn, tgt, tn = small_pair(n=30000)
-    crit = R.ICPConvergenceCriteria(0, 0, 14)
-    monkeypatch.setenv("CPHB_RETILE_MASK", "0x12")
-    a = R.registration_icp(cloud(src), cloud(tgt, tn), 0.03, np.eye(4), R.TransformationEstimationPointToPlane(), crit)
-    monkeypatch.delenv("CPHB_RETILE_MASK")
-    b = R.registration_icp(cloud(src), cloud(tgt, tn), 0.03, np.eye(4), R.TransformationEstimationPointToPlane(), crit)
-    R.DEFAULT_FLAGS = R.ICP_NO_RETILE           # (the API flag that forbids it whatever the mask says)
-    try:
-        c = R.registration_icp(cloud(src), cloud(tgt, tn), 0.03, np.eye(4), R.TransformationEstimationPointToPlane(), crit)
-    finally:
-        R.DEFAULT_FLAGS = 0
-    np.testing.assert_array_equal(b.transformation, c.transformation)
-    # the float64 sums are added in a different order (1e-16 relative), so the float32 systems are the same
-    # except on a rounding boundary: allow one ulp-level wobble of the pose, demand identical correspondences
-    assert np.linalg.norm(a.transformation.astype(np.float64) - b.transformation) <= 1e-6
-    np.testing.assert_array_equal(a.correspondence_set, b.correspondence_set)
-    ref = orc.registration_icp(orc.P2PLANE, src, tgt, 0.03, tgt_nrm=tn, relative_fitness=0, relative_rmse=0, max_iteration=14)
-    _compare(a, ref)
 
 
 def test_kabsch_golden(golden, orc):

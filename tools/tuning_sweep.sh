@@ -1,7 +1,7 @@
 #!/bin/bash
 # Re-tuning sweep on the GPU at hand, from the repository root after build():
-#   1. config 2 (bench.py, headline leg only) with the library defaults (three times: the spread), under each tuning
-#      hook, and with each icp.cu variant found in build_variants/ (tools/build_variant.sh NAME -D...);
+#   1. config 2 (bench.py, headline leg only) with the library defaults (three times: the spread) and under each
+#      run-time hook;
 #   2. VoxelDownSample, dense-grid path vs hash path (CPHB_VOXEL_NO_DENSE), at grids below and above the L2 size;
 #   3. device-to-device copy bandwidth (what roofline.frac should be read against).
 # One line per setting on stdout; the bench lines are kept in OUTDIR.
@@ -10,9 +10,6 @@ set -u
 OUT=${1:-tuning_out}
 mkdir -p "$OUT"
 nvidia-smi --query-gpu=name,power.limit,clocks.max.sm --format=csv,noheader
-LIB=cupoch_b200/lib/libcupoch_b200.so
-cp "$LIB" "$OUT/default.so"
-trap 'cp "$OUT/default.so" "$LIB"' EXIT
 
 run() {  # label [VAR=value ...]
     local label=$1; shift
@@ -27,19 +24,8 @@ print('%-26s value %6.0f it/s  loop %6.0f it/s  T[0][3] %.7f' % (sys.argv[2], d[
 }
 
 for i in 1 2 3; do run default_$i; done
-for v in 2 3; do run icp_blocks_per_sm_$v CPHB_ICP_BLOCKS_PER_SM=$v; done
-for v in 3 4; do run search_blocks_per_sm_$v CPHB_ICP_SEARCH_BLOCKS_PER_SM=$v; done
-for v in 17 33 132; do run helper_blocks_$v CPHB_HELPER_BLOCKS=$v; done
 for v in 2 8; do run cert_gain_$v CPHB_CERT_GAIN=$v; done
 run static_sched_0 CPHB_STATIC_SCHED=0
-for v in 0x12 0x4; do run retile_mask_$v CPHB_RETILE_MASK=$v; done
-for v in 8 20; do run transpose_max_$v CPHB_TRANSPOSE_MAX=$v; done
-for so in build_variants/*.so; do
-    [ -e "$so" ] || continue
-    cp "$so" "$LIB"
-    run "variant_$(basename "$so" .so)"
-done
-cp "$OUT/default.so" "$LIB"
 
 python - <<'EOF'
 import os, time

@@ -264,6 +264,26 @@ class PointCloud:
         self.last_ransac_stats = (int(best.value), float(fr[0]), float(fr[1]))
         return np.array(h_plane, np.float32), DeviceArray((m.value,), np.int32, ptr=d_idx.ptr, base=d_idx)
 
+    def farthest_point_down_sample(self, num_samples):
+        """PointCloud::FarthestPointDownSample (pointcloud.cu:301-338; Open3D's binding name) -> new cloud of the
+        num_samples points picked by farthest-point sampling from index 0, in pick order, with their normals and
+        colours.  0 gives an empty cloud and len(self) a copy of the whole cloud in its original order.  More samples
+        than points is logged and the loop runs anyway, as in the reference: the output then repeats points."""
+        n, k = len(self), int(num_samples)
+        if k < 0:
+            raise ValueError("num_samples must be >= 0")
+        if k == 0:
+            return PointCloud()
+        if k == n:
+            return self.clone()
+        if k > n:
+            print("[cupoch_b200][error] Illegal number of samples: %d, must <= point size: %d" % (k, n), file=sys.stderr)
+            if n == 0:  # the reference would gather out of range here
+                return PointCloud()
+        d_idx = DeviceArray((k,), np.int32)
+        _lib.check(_lib.lib().cphb_farthest_point_down_sample(self._points.ptr, n, k, d_idx.ptr, None, None))
+        return self._filtered(d_idx, k)[0]
+
     def cluster_dbscan(self, eps, min_points, print_progress=False, max_edges=100):
         """PointCloud::ClusterDBSCAN (pointcloud_cluster.cu:84-179; bound as cluster_dbscan, pointcloud.cpp:228-245) ->
         device vector of n int32 labels, -1 = noise."""

@@ -409,6 +409,23 @@ public:
         inliers = std::vector<size_t>(h32.begin(), h32.end());
         return std::make_tuple(Eigen::Vector4f(h[0], h[1], h[2], h[3]), std::move(inliers));
     }
+    /// PointCloud::FarthestPointDownSample (pointcloud.cu:301-338): num_samples points by farthest-point sampling from
+    /// index 0, in pick order.  0 -> empty cloud, points_.size() -> a copy; more samples than points is logged and the
+    /// loop runs anyway (the output repeats points), except on an empty cloud, where the result is empty.
+    std::shared_ptr<PointCloud> FarthestPointDownSample(size_t num_samples) const {
+        const size_t n = points_.size();
+        if (num_samples == 0) return std::make_shared<PointCloud>();
+        if (num_samples == n) return std::make_shared<PointCloud>(*this);
+        if (num_samples > n) {
+            char msg[128];
+            std::snprintf(msg, sizeof(msg), "Illegal number of samples: %zu, must <= point size: %zu", num_samples, n);
+            utility::LogError(msg);
+            if (n == 0) return std::make_shared<PointCloud>();
+        }
+        utility::device_vector<int32_t> idx(num_samples);
+        utility::check(cphb_farthest_point_down_sample(cfp(points_), n, num_samples, idx.data(), nullptr, nullptr));
+        return gather(idx, num_samples);
+    }
     /// PointCloud::ClusterDBSCAN (pointcloud.h:195-199, pointcloud_cluster.cu:84-179): labels, -1 = noise
     std::unique_ptr<utility::device_vector<int>> ClusterDBSCAN(float eps, size_t min_points, bool print_progress = false,
                                                                size_t max_edges = 100) const {

@@ -204,6 +204,17 @@ int cphb_select_by_index(const float *points, const float *normals, const float 
 int cphb_segment_plane(const float *points, size_t n, float distance_threshold, int ransac_n, int num_iterations,
                        const int32_t *h_seeds, float h_plane[4], int32_t *inliers_out, size_t *h_n_out,
                        int32_t *h_best_iteration, float h_fitness_rmse[2], float h_phase_ms[3], void *stream);
+/* PointCloud::FarthestPointDownSample (pointcloud.cu:122-139,301-338): indices_out (device, num_samples int32)
+ * receives the farthest-point sequence: index 0 first, then at every step the point whose squared distance (dist2,
+ * DESIGN.md arithmetic contract) to the nearest point selected so far is largest, the smallest index among equal
+ * distances.  Running distances start at +inf and are updated with fminf, so a NaN distance never replaces one.  Any
+ * num_samples >= 1 runs the loop, num_samples >= n included (on a finite cloud, once every distinct point is taken the
+ * sequence repeats index 0; the front ends return an empty cloud for 0 and a copy for n).  d2_out (device, n floats, optional) receives
+ * every point's final running distance: its squared distance to the nearest selected point.  One cooperative launch
+ * for the whole loop; asynchronous on the stream (no host synchronisation).  n == 0 with num_samples > 0, or
+ * n > 2^31-1: CPHB_ERR_INVALID. */
+int cphb_farthest_point_down_sample(const float *points, size_t n, size_t num_samples, int32_t *indices_out,
+                                    float *d2_out, void *stream);
 
 /* ------------------------------------------------------------------------ *
  * registration  (registration.h:35-91, transformation_estimation.h:36-143,

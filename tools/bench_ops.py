@@ -26,9 +26,13 @@ def main():
                     help="also time the SURVEY 8f rows: RemoveRadiusOutliers / RemoveStatisticalOutliers / VoxelGrid")
     ap.add_argument("--segment-plane", action="store_true",
                     help="instead: time PointCloud::SegmentPlane per phase at N = 1 M, 10 M and T = 100, 1000")
+    ap.add_argument("--fps", action="store_true",
+                    help="instead: time PointCloud::FarthestPointDownSample at N = 100 k, 1 M, 10 M and 1024, 8192 samples")
     args = ap.parse_args()
     if args.segment_plane:
         return segment_plane(args.reps)
+    if args.fps:
+        return fps(args.reps)
     import cupoch_b200 as cph
     from cupoch_b200 import _lib
     from cupoch_b200.testing import datagen
@@ -212,6 +216,83 @@ def segment_plane(reps):
             })
     print(json.dumps({"op": "PointCloud::SegmentPlane(0.01, 3, T) on datagen.plane_scene(N, 11)", "gpu": gpu, "reps": reps,
                       "launches": int(L.cphb_launch_count()), "rows": rows}))
+
+
+def fps(reps):
+    """cphb_farthest_point_down_sample on datagen.surface(N, 11): CUDA-event time of the call (one persistent launch),
+    against a reference-shaped loop in torch on the same GPU (one step per sample: torch.minimum of the distances,
+    argmax, .item() -- launches and a host round trip per sample, as thrust::transform_reduce has in the reference),
+    timed by the host clock, which the .item() of every step synchronises.  torch rounds the squared distance
+    differently (no FMA), so its picks are counted against the product's, not asserted.  N = 100 k and 1 M keep the
+    points in shared memory, 10 M streams them (the switch is at SMs * 14336 points).  The CPU oracle runs where
+    N * samples <= 2e9 (single-threaded, a few seconds) and must agree bit for bit."""
+    import subprocess
+    import torch
+    import cupoch_b200 as cph
+    from cupoch_b200 import _lib
+    from cupoch_b200.testing import datagen
+    from cupoch_b200.utility import DeviceArray
+    from oracle import fps_py as orc
+    L = _lib.lib()
+    gpu = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                         capture_output=True, text=True).stdout.strip()
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    ev = [L.cphb_event_create() for _ in range(2)]
+    rows = []
+    for n in (100_000, 1_000_000, 10_000_000):
+        pts = datagen.surface(n, 11)[0]
+        pc = cph.geometry.PointCloud(pts)
+        P = torch.from_numpy(pts).cuda()
+        for S in (1024, 8192):
+            d_idx = DeviceArray((S,), np.int32)
+            calls = []
+            for r in range(reps + 1):  # the first call warms the allocation pool and the module
+                L.cphb_event_record(ev[0], None)
+                _lib.check(L.cphb_farthest_point_down_sample(pc.points.ptr, n, S, d_idx.ptr, None, None))
+                L.cphb_event_record(ev[1], None)
+                ms = C.c_float(0)
+                _lib.check(L.cphb_event_elapsed_ms(ev[0], ev[1], C.byref(ms)))
+                if r:
+                    calls.append(ms.value)
+            idx = d_idx.cpu()
+            med = float(np.median(calls))
+
+            def torch_loop():
+                dist = torch.full((n,), float("inf"), device="cuda")
+                far, sel = 0, []
+                for _ in range(S):
+                    sel.append(far)
+                    dist = torch.minimum(dist, ((P - P[far]) ** 2).sum(1))
+                    far = int(torch.argmax(dist).item())
+                return np.array(sel, np.int32)
+
+            torch_loop()
+            t_calls = []
+            for _ in range(max(2, reps // 2)):
+                torch.cuda.synchronize()
+                t0 = time.perf_counter()
+                t_idx = torch_loop()
+                t_calls.append((time.perf_counter() - t0) * 1e3)
+            t_med = float(np.median(t_calls))
+            agree = t_idx == idx
+            row = {"n": n, "num_samples": S, "points_in_shared_memory": bool(n <= sms * 14336),
+                   "call_ms_median": med, "call_ms_min": float(np.min(calls)), "us_per_sample": med * 1e3 / S,
+                   "torch_loop": {"ms_median": t_med, "ms_min": float(np.min(t_calls)), "us_per_sample": t_med * 1e3 / S,
+                                  "index_agreement": float(agree.mean()),
+                                  "first_disagreement": None if agree.all() else int(np.argmin(agree))},
+                   "speedup_vs_torch_loop": t_med / med}
+            if n * S <= 2e9:
+                t0 = time.perf_counter()
+                o_idx, _ = orc.farthest_point_down_sample(pts, S)
+                row["cpu_oracle"] = {"seconds": time.perf_counter() - t0, "threads": 1,
+                                     "parity": bool(np.array_equal(o_idx, idx))}
+            else:
+                row["cpu_oracle"] = None
+            rows.append(row)
+        del P
+        torch.cuda.empty_cache()
+    print(json.dumps({"op": "PointCloud::FarthestPointDownSample(S) on datagen.surface(N, 11)", "gpu": gpu, "reps": reps,
+                      "sms": sms, "launches": int(L.cphb_launch_count()), "rows": rows}))
 
 
 if __name__ == "__main__":

@@ -93,6 +93,8 @@ _SIGNATURES = {
     "cphb_segment_plane": (C.c_int, [_P, C.c_size_t, C.c_float, C.c_int, C.c_int, _I3, _F3, _P, C.POINTER(C.c_size_t),
                                      _I3, _F3, _F3, _P]),
     "cphb_farthest_point_down_sample": (C.c_int, [_P, C.c_size_t, C.c_size_t, _P, _P, _P]),
+    "cphb_compute_iss_keypoints": (C.c_int, [_P, C.c_size_t, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int, C.c_int,
+                                             _P, _P, C.POINTER(C.c_size_t), _P, _F3, _P]),
     "cphb_covariances_from_normals": (C.c_int, [_P, C.c_size_t, C.c_float, _P, C.c_int, _P]),
     "cphb_color_gradient": (C.c_int, [_P, _P, _P, C.c_size_t, C.c_float, C.c_int, _P, _P]),
     "cphb_icp_create": (C.c_int, [C.POINTER(Cloud), C.POINTER(Cloud), C.POINTER(IcpParams), _P, C.POINTER(_P)]),

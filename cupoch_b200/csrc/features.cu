@@ -11,30 +11,16 @@
 
 #include "cphb_eigen3.cuh"
 #include "cphb_internal.cuh"
+#include "fused_neighbourhood.cuh"
 #include "cphb_searchk.cuh"
 
-// compute_cumulant_functor (geometry_functor.h:35-55): one neighbour into the 9 cumulants (float64 sums of exact products)
-__device__ __forceinline__ void cumulant_add(double (&cum)[9], float x, float y, float z) {
-    cum[0] += x; cum[1] += y; cum[2] += z;
-    cum[3] = fma((double)x, (double)x, cum[3]); cum[4] = fma((double)x, (double)y, cum[4]);
-    cum[5] = fma((double)x, (double)z, cum[5]); cum[6] = fma((double)y, (double)y, cum[6]);
-    cum[7] = fma((double)y, (double)z, cum[7]); cum[8] = fma((double)z, (double)z, cum[8]);
-}
 // ComputeNormal (estimate_normals.cu:38-54): covariance E[xx^T] - E[x]E[x]^T in float32, eigenvector of the smallest
 // eigenvalue, (0,0,1) with fewer than 3 neighbours or a zero / NaN vector
 __device__ __forceinline__ void normal_from_cumulants(const double (&cum)[9], int cnt, float &nx, float &ny, float &nz) {
     nx = 0.f; ny = 0.f; nz = 1.f;
     if (cnt < 3) return;
-    float c[9];
-#pragma unroll
-    for (int a = 0; a < 9; ++a) c[a] = (float)cum[a] / (float)cnt;
     float cov[9];
-    cov[0] = __fmaf_rn(-c[0], c[0], c[3]);
-    cov[4] = __fmaf_rn(-c[1], c[1], c[6]);
-    cov[8] = __fmaf_rn(-c[2], c[2], c[8]);
-    cov[1] = cov[3] = __fmaf_rn(-c[0], c[1], c[4]);
-    cov[2] = cov[6] = __fmaf_rn(-c[0], c[2], c[5]);
-    cov[5] = cov[7] = __fmaf_rn(-c[1], c[2], c[7]);
+    covariance_from_cumulants(cum, cnt, cov);
     float e[3], V[9];
     fast_eigen3x3(cov, e, V);
     int mi = 0;
@@ -72,58 +58,19 @@ __global__ void __launch_bounds__(128) normals_kernel(const float *__restrict__ 
 // EstimateNormals in ONE kernel (SURVEY 8f rank 1; estimate_normals.cu:82-127 + geometry_functor.h:35-55): the warp's
 // k-best search (lists in shared memory) is followed, in the same kernel, by the 9 cumulants over each lane's list in
 // list order and the 3x3 eigen-solve -- the [n][k] index / distance table (8 k bytes per point written and read back,
-// 2.4 GB at 10 M x k = 30) never exists.
-//   self_order: the queries are the indexed cloud itself, taken in INDEX order (lane = one point of a leaf, so a warp's
-//               queries are exactly one leaf and need no ordering pass); original position = ix.pts[i].w
-//   otherwise : query i is pts[first + perm[i]] (perm = Hilbert order of the block, or NULL), output row perm[i]
+// 2.4 GB at 10 M x k = 30) never exists.  Query order: fused_query_setup (fused_neighbourhood.cuh).
 template <int TOP>
 __global__ void normals_fused_kernel(IndexView ix, const float *__restrict__ pts, size_t first, size_t count,
                                      const uint32_t *__restrict__ perm, int self_order, float r2, int k, float *__restrict__ out) {
     extern __shared__ __align__(16) unsigned char smem[];
-    const int nwarp = blockDim.x >> 5;
-    const int warp = threadIdx.x >> 5;
-    float4 *tiles = (float4 *)smem;
-    uint64_t *bars = (uint64_t *)(tiles + (size_t)nwarp * 2 * CPHB_LEAF);
-    unsigned long long *lists = (unsigned long long *)(bars + 2 * nwarp);
     WarpSearchK w;
-    warp_search_setup(w, tiles + (size_t)warp * 2 * CPHB_LEAF, bars + 2 * warp);
-    w.k = k;
-    w.list = lists + (size_t)warp * k * 32 + lane_id();
-    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    size_t pos = 0;
-    w.qx = w.qy = w.qz = 0.f;
-    if (self_order) {
-        w.valid = i < (size_t)ix.n_leaves * CPHB_LEAF;
-        if (w.valid) {
-            const float4 q = ix.pts[i];
-            w.valid = __float_as_uint(q.w) != 0xffffffffu;  // padded tail of the index
-            pos = __float_as_uint(q.w);
-            w.qx = q.x; w.qy = q.y; w.qz = q.z;
-        }
-    } else {
-        w.valid = i < count;
-        if (w.valid) {
-            pos = perm ? perm[i] : i;
-            const float *q = pts + 3 * (first + pos);
-            w.qx = q[0]; w.qy = q[1]; w.qz = q[2];
-        }
-    }
-    const unsigned long long init = (r2 > 0.f) ? init_key(r2) : 0ull;
-    for (int j = 0; j < k; ++j) w.list[j * 32] = init;
-    w.worst = init;
-    w.bound = (unsigned)(init >> 32);
-    warp_query_box(w);
-    if (__any_sync(CPHB_FULL, w.valid)) warp_nn_search<TOP>(ix, w);
+    size_t pos;
+    const unsigned long long init = fused_query_setup(w, smem, ix, pts, first, count, perm, self_order, r2, k, pos);
+    fused_query_search<TOP>(ix, w);
     if (!w.valid) return;
-    double cum[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
-    int cnt = 0;
-    for (int j = 0; j < k; ++j) {
-        const unsigned long long key = w.list[j * 32];
-        if (!(key < init)) break;  // ascending: the unfilled slots are at the end
-        const size_t id = (unsigned)(key & 0xffffffffull);
-        cumulant_add(cum, pts[3 * id], pts[3 * id + 1], pts[3 * id + 2]);
-        ++cnt;
-    }
+    double cum[9];
+    int cnt;
+    list_cumulants(w, k, init, pts, cum, cnt);
     float nx, ny, nz;
     normal_from_cumulants(cum, cnt, nx, ny, nz);
     out[3 * pos] = nx; out[3 * pos + 1] = ny; out[3 * pos + 2] = nz;
@@ -142,7 +89,7 @@ static int launch_normals_fused(const cphb_index *ix, const float *points, size_
         rc = cphb_hilbert_order_n(points + 3 * first, count, perm, ix->bounds, 1, count < n ? count : n, s);
         if (rc) { cphb_free_async(perm, s); return rc; }
     }
-    const size_t per_warp = 2 * CPHB_LEAF * sizeof(float4) + 2 * sizeof(uint64_t) + (size_t)k * 32 * sizeof(unsigned long long);
+    const size_t per_warp = fused_smem_per_warp(k);
     int warps = (int)((96 * 1024) / per_warp);
     if (warps > 8) warps = 8;
     if (warps < 1) warps = 1;

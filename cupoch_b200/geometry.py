@@ -642,3 +642,6 @@ class KDTreeFlann:
         if k < 0:
             raise RuntimeError("search_radius_vector_3f() error!")
         return k, idx.cpu().reshape(-1), d2.cpu().reshape(-1)
+
+
+from . import keypoint  # noqa: E402,F401  (cph.geometry.keypoint: the reference's submodule, keypoint.cpp:76-79)

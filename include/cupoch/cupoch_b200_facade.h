@@ -693,6 +693,48 @@ private:
     }
     cphb_occgrid *h_ = nullptr;
 };
+
+namespace keypoint {
+/// geometry::keypoint::ComputeISSKeypoints (keypoint.h:54-60, iss_keypoints.cu:108-172) -> (the keypoints in ascending
+/// index order with their normals and colours, the per-point mask).  salient_radius == 0 or non_max_radius == 0 replaces
+/// both from the cloud's resolution.  An empty input, or max_neighbors outside [0, 256], is logged and gives empty results.
+inline std::tuple<std::shared_ptr<PointCloud>, std::shared_ptr<utility::device_vector<bool>>> ComputeISSKeypoints(
+        const PointCloud &input, float salient_radius = 0.0, float non_max_radius = 0.0, float gamma_21 = 0.975,
+        float gamma_32 = 0.975, int min_neighbors = 5, int max_neighbors = knn::NUM_MAX_NN) {
+    static_assert(sizeof(bool) == 1, "the mask is written as bytes");
+    auto out = std::make_shared<PointCloud>();
+    auto mask = std::make_shared<utility::device_vector<bool>>();
+    const size_t n = input.points_.size();
+    if (n == 0) {
+        utility::LogWarning("[ComputeISSKeypoints] Input PointCloud is empty!");
+        return std::make_tuple(out, mask);
+    }
+    if (max_neighbors < 0 || max_neighbors > 256) {
+        utility::LogError("[ComputeISSKeypoints] max_neighbors must lie in [0, 256].");
+        return std::make_tuple(out, mask);
+    }
+    mask->resize(n);
+    utility::device_vector<int32_t> idx(n);
+    size_t m = 0;
+    utility::check(cphb_compute_iss_keypoints(reinterpret_cast<const float *>(input.points_.data()), n, salient_radius,
+                                              non_max_radius, gamma_21, gamma_32, min_neighbors, max_neighbors,
+                                              reinterpret_cast<uint8_t *>(mask->data()), idx.data(), &m, nullptr, nullptr,
+                                              nullptr));
+    if (m) {  // SelectByMask (down_sample.cu:131-167): points, normals and colours of the masked rows
+        const bool hn = input.HasNormals(), hc = input.HasColors();
+        out->points_.resize(m);
+        if (hn) out->normals_.resize(m);
+        if (hc) out->colors_.resize(m);
+        utility::check(cphb_select_by_index(
+            reinterpret_cast<const float *>(input.points_.data()), hn ? reinterpret_cast<const float *>(input.normals_.data()) : nullptr,
+            hc ? reinterpret_cast<const float *>(input.colors_.data()) : nullptr, n, idx.data(), m,
+            reinterpret_cast<float *>(out->points_.data()), hn ? reinterpret_cast<float *>(out->normals_.data()) : nullptr,
+            hc ? reinterpret_cast<float *>(out->colors_.data()) : nullptr, nullptr));
+        utility::check(cphb_stream_synchronize(nullptr));
+    }
+    return std::make_tuple(out, mask);
+}
+}  // namespace keypoint
 }  // namespace geometry
 
 // --------------------------------------------------------------------------- registration

@@ -215,6 +215,22 @@ int cphb_segment_plane(const float *points, size_t n, float distance_threshold, 
  * n > 2^31-1: CPHB_ERR_INVALID. */
 int cphb_farthest_point_down_sample(const float *points, size_t n, size_t num_samples, int32_t *indices_out,
                                     float *d2_out, void *stream);
+/* geometry::keypoint::ComputeISSKeypoints (keypoint.h:54-60, iss_keypoints.cu:108-172): Intrinsic Shape Signature
+ * keypoints.  salient_radius == 0 or non_max_radius == 0 replaces BOTH by 6 and 4 times the resolution sqrtf(sum of
+ * the cloud's 2-NN squared distances / (float)n), the sum taken in DESIGN.md's tiled order.  A point's saliency is the
+ * smallest eigenvalue of its neighbourhood covariance (radius search (salient_radius, max_neighbors), the point
+ * itself included), as FastEigen3x3 returns it (normalised by the covariance's largest coefficient); it is -1 when
+ * fewer than min_neighbors points are listed, when every covariance coefficient is within 1e-5 of 0 (absolute), or
+ * unless lambda2 / lambda3 < gamma_21 and lambda1 / lambda2 < gamma_32.  A point is a keypoint (mask_out[i] = 1) iff
+ * its saliency is >= 0 and no point of its (non_max_radius, max_neighbors) list has a strictly larger one.
+ * mask_out: device, n bytes.  Optional (NULL to skip): indices_out (device, n int32) gets the ascending keypoint
+ * indices, saliency_out (device, n floats) every saliency, h_radii the two radii used.  *h_n_out = keypoint count.
+ * max_neighbors in [0, 256] (0: no keypoints), else CPHB_ERR_INVALID; a negative radius acts as its absolute value;
+ * n == 0 gives 0 keypoints.  One index serves every search; no [n][max_neighbors] table is built.  Synchronises. */
+int cphb_compute_iss_keypoints(const float *points, size_t n, float salient_radius, float non_max_radius,
+                               float gamma_21, float gamma_32, int min_neighbors, int max_neighbors, uint8_t *mask_out,
+                               int32_t *indices_out, size_t *h_n_out, float *saliency_out, float h_radii[2],
+                               void *stream);
 
 /* ------------------------------------------------------------------------ *
  * registration  (registration.h:35-91, transformation_estimation.h:36-143,

@@ -28,11 +28,15 @@ def main():
                     help="instead: time PointCloud::SegmentPlane per phase at N = 1 M, 10 M and T = 100, 1000")
     ap.add_argument("--fps", action="store_true",
                     help="instead: time PointCloud::FarthestPointDownSample at N = 100 k, 1 M, 10 M and 1024, 8192 samples")
+    ap.add_argument("--iss", action="store_true",
+                    help="instead: time geometry::keypoint::ComputeISSKeypoints (defaults, automatic radii) at N = 1 M, 10 M")
     args = ap.parse_args()
     if args.segment_plane:
         return segment_plane(args.reps)
     if args.fps:
         return fps(args.reps)
+    if args.iss:
+        return iss(args.reps)
     import cupoch_b200 as cph
     from cupoch_b200 import _lib
     from cupoch_b200.testing import datagen
@@ -293,6 +297,125 @@ def fps(reps):
         torch.cuda.empty_cache()
     print(json.dumps({"op": "PointCloud::FarthestPointDownSample(S) on datagen.surface(N, 11)", "gpu": gpu, "reps": reps,
                       "sms": sms, "launches": int(L.cphb_launch_count()), "rows": rows}))
+
+
+ISS_PHASES = (("radii", ("iss_knn2", "iss_tile_sum", "iss_radii")), ("saliency", ("iss_saliency",)),
+              ("suppression", ("iss_suppress",)), ("compaction_gather", ("keep_", "select_rows")))
+
+
+def eigvals3(A):
+    """ascending eigenvalues of a batch of symmetric 3x3 float32 matrices, closed form (trigonometric), in torch.
+    torch.linalg.eigvalsh raised CUSOLVER_STATUS_INVALID_VALUE on these batches on the H100 (torch 2.11, CUDA 12.8)."""
+    import torch
+    q = A.diagonal(dim1=1, dim2=2).sum(1) / 3
+    B = A - q[:, None, None] * torch.eye(3, device=A.device)
+    p = torch.sqrt((B * B).sum((1, 2)) / 6).clamp(min=1e-30)
+    r = (torch.linalg.det(B / p[:, None, None]) / 2).clamp(-1, 1)
+    phi = torch.acos(r) / 3
+    e3 = q + 2 * p * torch.cos(phi)
+    e1 = q + 2 * p * torch.cos(phi + 2 * np.pi / 3)
+    return torch.stack([e1, 3 * q - e1 - e3, e3], 1)
+
+
+def iss(reps):
+    """compute_iss_keypoints(pc) with the defaults (automatic radii, max_neighbors 100) on datagen.surface(N, 11) over a
+    sqrt(N / 1e5)-wide square:
+    CUDA-event time of the whole Python call (index build, the fused kernels, compaction, gather), and per-phase kernel
+    times from torch.profiler in a separate profiled call (radii = kNN-2 + tiled sum; saliency; suppression; compaction
+    + gather; the rest is the index build).  Comparison arm shaped like the reference (iss_keypoints.cu:108-172) on the
+    same GPU, timed by the host clock around a synchronised run: cphb_search_knn(k = 2) + a torch sum for the radii,
+    cphb_search_radius into [n][100] tables twice, torch for the cumulants (float32 sums over the table rows),
+    closed-form 3x3 eigenvalues in torch (eigvals3, float32) and the suppression gather.  Its eigen-solver is not FastEigen3x3, so its keypoints
+    are compared as a set (Jaccard overlap), not asserted."""
+    import subprocess
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    import cupoch_b200 as cph
+    from cupoch_b200 import _lib
+    from cupoch_b200.testing import datagen
+    from cupoch_b200.utility import DeviceArray
+    L = _lib.lib()
+    gpu = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                         capture_output=True, text=True).stdout.strip()
+    ev = [L.cphb_event_create() for _ in range(2)]
+    kp_fn = cph.geometry.keypoint.compute_iss_keypoints
+    rows = []
+    for n in (1_000_000, 10_000_000):
+        # extent sqrt(N / 1e5): 1e5 points per unit square.  On the unit square at 1 M every neighbourhood covariance is
+        # within 1e-5 of zero, and the reference's absolute isZero test leaves no salient point at all
+        pts = datagen.surface(n, 11, extent=float(np.sqrt(n / 1e5)))[0]
+        pc = cph.geometry.PointCloud(pts)
+        calls = []
+        for r in range(reps + 1):  # the first call warms the allocation pool and the modules
+            L.cphb_event_record(ev[0], None)
+            out, mask = kp_fn(pc)
+            L.cphb_event_record(ev[1], None)
+            ms = C.c_float(0)
+            _lib.check(L.cphb_event_elapsed_ms(ev[0], ev[1], C.byref(ms)))
+            if r:
+                calls.append(ms.value)
+        radii = pc.last_iss_radii
+        keep = mask.cpu()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            kp_fn(pc)
+            torch.cuda.synchronize()
+        phase_ms = {name: 0.0 for name, _ in ISS_PHASES}
+        phase_ms["index_build"] = 0.0
+        for e in prof.key_averages():
+            t = getattr(e, "device_time_total", getattr(e, "cuda_time_total", 0.0)) * 1e-3
+            if t <= 0 or "Memset" in e.key or "Memcpy" in e.key:
+                continue
+            name = next((p for p, keys in ISS_PHASES if any(k in e.key for k in keys)), "index_build")
+            phase_ms[name] += t
+
+        def reference_shaped():
+            P = torch.as_tensor(pc.points, device="cuda")
+            tree = cph.geometry.KDTreeFlann(pc)
+            _, i2, d2 = tree.search_knn(pc.points, 2)
+            res = torch.sqrt(torch.as_tensor(d2, device="cuda")[:, 1].sum() / n)
+            rs, rn = float(6 * res), float(4 * res)
+            _, idx, _ = tree.search_radius(pc.points, rs, 100)
+            I = torch.as_tensor(idx, device="cuda")
+            sal = torch.empty(n, device="cuda")
+            for lo in range(0, n, 1 << 20):  # the cumulants per table row, chunked only to bound torch's temporaries
+                J = I[lo:lo + (1 << 20)]
+                ok = (J >= 0).unsqueeze(-1)
+                X = P[J.clamp(min=0).long()] * ok
+                cnt = ok.sum(1).float()
+                mu = X.sum(1) / cnt
+                cov = torch.einsum("nki,nkj->nij", X, X) / cnt.unsqueeze(-1) - mu.unsqueeze(-1) * mu.unsqueeze(-2)
+                e = eigvals3(cov / cov.flatten(1).amax(1).clamp(min=1e-30)[:, None, None])
+                nonzero = (cov.flatten(1).abs() > 1e-5).any(1)
+                s = torch.where((cnt[:, 0] >= 5) & nonzero & (e[:, 2] > 0) & (e[:, 1] / e[:, 2] < 0.975) & (e[:, 0] / e[:, 1] < 0.975),
+                                e[:, 0], torch.full_like(e[:, 0], -1.0))
+                sal[lo:lo + len(J)] = s
+            del I, X
+            _, idx, _ = tree.search_radius(pc.points, rn, 100)
+            I = torch.as_tensor(idx, device="cuda")
+            nb = torch.where(I >= 0, sal[I.clamp(min=0).long()], torch.full_like(sal[:1], -2.0).expand_as(I))
+            m = (sal >= 0) & ~(nb > sal[:, None]).any(1)
+            return m.cpu().numpy()
+
+        reference_shaped()
+        t_calls = []
+        for _ in range(max(2, reps // 2)):
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            t_mask = reference_shaped()
+            torch.cuda.synchronize()
+            t_calls.append((time.perf_counter() - t0) * 1e3)
+        torch.cuda.empty_cache()
+        t_med = float(np.median(t_calls))
+        med = float(np.median(calls))
+        inter, union = int((keep & t_mask).sum()), int((keep | t_mask).sum())
+        rows.append({"n": n, "radii": list(radii), "keypoints": int(keep.sum()), "call_ms_median": med,
+                     "call_ms_min": float(np.min(calls)), "phase_ms_profiled": phase_ms,
+                     "tables_not_written_bytes": int(2 * 100 * 8 * n + 2 * 8 * n),
+                     "reference_shaped": {"ms_median": t_med, "ms_min": float(np.min(t_calls)), "keypoints": int(t_mask.sum()),
+                                          "jaccard_overlap": inter / union if union else 1.0},
+                     "speedup_vs_reference_shaped": t_med / med})
+    print(json.dumps({"op": "geometry::keypoint::ComputeISSKeypoints(defaults) on datagen.surface(N, 11)", "gpu": gpu,
+                      "reps": reps, "launches": int(L.cphb_launch_count()), "rows": rows}))
 
 
 if __name__ == "__main__":

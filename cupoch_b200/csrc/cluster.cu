@@ -94,25 +94,20 @@ extern "C" int cphb_cluster_dbscan(const float *points, size_t n, float eps, int
         return CPHB_ERR_INVALID;
     }
     const int K = max_edges + 1;
-    cphb_index *ix = nullptr;
-    int rc = cphb_index_create(points, n, stream, &ix);
-    if (rc) return rc;
-    int32_t *idx = nullptr, *queue = nullptr;
-    float *d2 = nullptr;
+    cphb_nbr_table t;
+    int32_t *queue = nullptr;
     int *degree = nullptr, *visited = nullptr, *ncl = nullptr;
     unsigned *stamp = nullptr;
-    rc = cphb_alloc_async((void **)&idx, sizeof(int32_t) * n * K, s);
-    if (!rc) rc = cphb_alloc_async((void **)&d2, sizeof(float) * n * K, s);
+    int rc = cphb_nbr_table_create(points, n, 0, n, 0, eps, K, &t, s);
     if (!rc) rc = cphb_alloc_async((void **)&degree, sizeof(int) * n, s);
     if (!rc) rc = cphb_alloc_async((void **)&visited, sizeof(int) * n, s);
     if (!rc) rc = cphb_alloc_async((void **)&stamp, sizeof(unsigned) * n, s);
     if (!rc) rc = cphb_alloc_async((void **)&queue, sizeof(int32_t) * n, s);
     if (!rc) rc = cphb_alloc_async((void **)&ncl, sizeof(int), s);
-    if (!rc) rc = cphb_search_radius(ix, points, n, eps, K, idx, d2, nullptr, stream);
     if (!rc) {
-        CPHB_LAUNCH(dbscan_degree_kernel, (unsigned)((n + 255) / 256), 256, 0, s, idx, n, K, min_points, degree);
-        CPHB_LAUNCH(dbscan_bfs_kernel, 1, DB_THREADS, 0, s, idx, degree, (unsigned)n, K, min_points, labels_out, stamp, visited, queue,
-                    ncl);
+        CPHB_LAUNCH(dbscan_degree_kernel, (unsigned)((n + 255) / 256), 256, 0, s, t.idx, n, K, min_points, degree);
+        CPHB_LAUNCH(dbscan_bfs_kernel, 1, DB_THREADS, 0, s, t.idx, degree, (unsigned)n, K, min_points, labels_out, stamp, visited,
+                    queue, ncl);
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) { cphb_set_error("dbscan kernels: %s", cudaGetErrorString(e)); rc = CPHB_ERR_CUDA; }
     }
@@ -123,9 +118,7 @@ extern "C" int cphb_cluster_dbscan(const float *points, size_t n, float eps, int
         if (e != cudaSuccess) { cphb_set_error("cphb_cluster_dbscan: %s", cudaGetErrorString(e)); rc = CPHB_ERR_CUDA; }
     }
     if (h_n_clusters) *h_n_clusters = h;
-    cphb_free_async(idx, s); cphb_free_async(d2, s); cphb_free_async(degree, s); cphb_free_async(visited, s);
-    cphb_free_async(stamp, s); cphb_free_async(queue, s); cphb_free_async(ncl, s);
-    cudaStreamSynchronize(s);
-    cphb_index_destroy(ix);
-    return rc;
+    cphb_free_async(degree, s); cphb_free_async(visited, s); cphb_free_async(stamp, s); cphb_free_async(queue, s);
+    cphb_free_async(ncl, s);
+    return cphb_nbr_table_release(&t, rc, s);
 }

@@ -96,6 +96,19 @@ int cphb_sort_pairs_u64(const uint64_t *keys_in, uint64_t *keys_out, const uint3
 // *h_n_out (synchronises the stream)
 int cphb_compact_flags(const uint8_t *keep, size_t n, int32_t *indices_out, size_t *h_n_out, cudaStream_t s);
 
+// neighbour table of an index client (search.cu): create builds an index of points[n] and searches the rows
+// [first, first + count) against it into idx / d2 [count][k] -- KNN(knn) when knn > 0, else Radius(radius, max_nn),
+// k = knn or max_nn.  Release (also after a failed create) frees the tables, synchronises the stream and destroys the
+// index; it returns rc, or CPHB_ERR_CUDA when rc was CPHB_OK and the synchronise failed.
+struct cphb_nbr_table {
+    cphb_index *ix = nullptr;
+    int32_t *idx = nullptr;
+    float *d2 = nullptr;
+};
+int cphb_nbr_table_create(const float *points, size_t n, size_t first, size_t count, int knn, float radius, int max_nn,
+                          cphb_nbr_table *t, cudaStream_t s);
+int cphb_nbr_table_release(cphb_nbr_table *t, int rc, cudaStream_t s);
+
 // index.cu internals reused by icp.cu (Hilbert-ordering of the source)
 // perm_out[pos] = original index of the pos-th point along the Hilbert curve.
 // bounds_dev6: device buffer of 6 ordered-uint floats; computed here unless

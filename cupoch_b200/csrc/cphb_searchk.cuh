@@ -1,5 +1,6 @@
-// cphb_searchk.cuh -- the k-best result set of the warp-cooperative traversal (k > 1), shared by search.cu (SearchKNN /
-// SearchRadius) and features.cu (the fused EstimateNormals kernel).
+// cphb_searchk.cuh -- the k-best result set of the warp-cooperative traversal (k > 1), used by every k-list kernel
+// through fused_neighbourhood.cuh: search.cu (SearchKNN / SearchRadius), features.cu (the fused EstimateNormals kernel)
+// and iss.cu (ComputeISSKeypoints).
 #pragma once
 #include "cphb_internal.cuh"
 

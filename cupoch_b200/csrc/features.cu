@@ -76,61 +76,6 @@ __global__ void normals_fused_kernel(IndexView ix, const float *__restrict__ pts
     out[3 * pos] = nx; out[3 * pos + 1] = ny; out[3 * pos + 2] = nz;
 }
 
-// launch of the fused kernel for the queries [first, first + count) of `points` against the index of the whole cloud
-static int launch_normals_fused(const cphb_index *ix, const float *points, size_t n, size_t first, size_t count, int knn,
-                                float radius, int k, float *out, cudaStream_t s) {
-    const float r2 = (knn > 0) ? INFINITY : radius * radius;  // kdtree_flann.inl:120
-    const bool self_order = (first == 0 && count == n);
-    uint32_t *perm = nullptr;
-    int rc = CPHB_OK;
-    if (!self_order && count > 32) {
-        rc = cphb_alloc_async((void **)&perm, sizeof(uint32_t) * count, s);
-        if (rc) return rc;
-        rc = cphb_hilbert_order_n(points + 3 * first, count, perm, ix->bounds, 1, count < n ? count : n, s);
-        if (rc) { cphb_free_async(perm, s); return rc; }
-    }
-    const size_t per_warp = fused_smem_per_warp(k);
-    int warps = (int)((96 * 1024) / per_warp);
-    if (warps > 8) warps = 8;
-    if (warps < 1) warps = 1;
-    const size_t smem = per_warp * warps;
-    const unsigned block = warps * 32;
-    const size_t lanes = self_order ? (size_t)ix->v.n_leaves * CPHB_LEAF : count;
-    const unsigned grid = (unsigned)((lanes + block - 1) / block);
-    if (ix->v.top <= 3) {
-        CPHB_CUDA(cudaFuncSetAttribute(normals_fused_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-        CPHB_LAUNCH(normals_fused_kernel<3>, grid, block, smem, s, ix->v, points, first, count, perm, self_order ? 1 : 0, r2, k, out);
-    } else {
-        CPHB_CUDA(cudaFuncSetAttribute(normals_fused_kernel<5>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-        CPHB_LAUNCH(normals_fused_kernel<5>, grid, block, smem, s, ix->v, points, first, count, perm, self_order ? 1 : 0, r2, k, out);
-    }
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { cphb_set_error("normals_fused_kernel: %s", cudaGetErrorString(e)); rc = CPHB_ERR_CUDA; }
-    cphb_free_async(perm, s);
-    return rc;
-}
-
-static int normals_two_pass(cphb_index *ix, const float *points, size_t first, size_t count, int knn, float radius, int k,
-                            float *out, cudaStream_t s) {
-    int32_t *idx = nullptr;
-    float *d2 = nullptr;
-    int rc = cphb_alloc_async((void **)&idx, sizeof(int32_t) * count * k, s);
-    if (!rc) rc = cphb_alloc_async((void **)&d2, sizeof(float) * count * k, s);
-    if (!rc) {
-        const float *q = points + 3 * first;
-        if (knn > 0) rc = cphb_search_knn(ix, q, count, k, idx, d2, nullptr, s);
-        else rc = cphb_search_radius(ix, q, count, radius, k, idx, d2, nullptr, s);
-    }
-    if (!rc) {
-        CPHB_LAUNCH(normals_kernel, (unsigned)((count + 127) / 128), 128, 0, s, points, count, idx, k, out);
-        cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess) { cphb_set_error("normals_kernel: %s", cudaGetErrorString(e)); rc = CPHB_ERR_CUDA; }
-    }
-    cphb_free_async(idx, s);
-    cphb_free_async(d2, s);
-    return rc;
-}
-
 // k limits as the search entry points have them: SearchKNN rejects knn > NUM_MAX_NN = 100 (kdtree_flann.cu:52-54),
 // SearchRadius is bounded by what one warp's lists can hold in shared memory (search.cu)
 static int normals_impl(const float *points, size_t n, int knn, float radius, int max_nn, size_t first, size_t count,
@@ -145,14 +90,37 @@ static int normals_impl(const float *points, size_t n, int knn, float radius, in
         cphb_set_error("search: k=%d outside [0,%d]", k, knn > 0 ? 100 : 256);
         return CPHB_ERR_INVALID;
     }
+    // either form builds one fresh index of the whole cloud, as the reference builds a fresh tree (:86-87)
+    if (getenv("CPHB_NORMALS_UNFUSED")) {  // A/B hook (read per call): the two-pass form, identical results
+        cphb_nbr_table t;
+        int rc = cphb_nbr_table_create(points, n, first, count, knn, radius, max_nn, &t, s);
+        if (!rc) {
+            CPHB_LAUNCH(normals_kernel, (unsigned)((count + 127) / 128), 128, 0, s, points, count, t.idx, k, out_normals);
+            const cudaError_t e = cudaGetLastError();
+            if (e != cudaSuccess) { cphb_set_error("normals_kernel: %s", cudaGetErrorString(e)); rc = CPHB_ERR_CUDA; }
+        }
+        return cphb_nbr_table_release(&t, rc, s);
+    }
+    // fused: the queries [first, first + count) against the index of the whole cloud -- the whole cloud in index order,
+    // a block in its own Hilbert order
+    const float r2 = (knn > 0) ? INFINITY : radius * radius;  // kdtree_flann.inl:120
+    const bool self_order = (first == 0 && count == n);
     cphb_index *ix = nullptr;
-    int rc = cphb_index_create(points, n, s, &ix);  // the reference also builds a fresh tree (:86-87)
-    if (rc) return rc;
-    const bool unfused = getenv("CPHB_NORMALS_UNFUSED") != nullptr;  // A/B hook (read per call): identical results
-    if (unfused) rc = normals_two_pass(ix, points, first, count, knn, radius, k, out_normals, s);
-    else rc = launch_normals_fused(ix, points, n, first, count, knn, radius, k, out_normals, s);
-    cudaStreamSynchronize(s);
+    uint32_t *perm = nullptr;
+    int rc = cphb_index_create(points, n, s, &ix);
+    if (!rc && !self_order && count > 32) {
+        rc = cphb_alloc_async((void **)&perm, sizeof(uint32_t) * count, s);
+        if (!rc) rc = cphb_hilbert_order_n(points + 3 * first, count, perm, ix->bounds, 1, count < n ? count : n, s);
+    }
+    if (!rc) {
+        const size_t lanes = self_order ? (size_t)ix->v.n_leaves * CPHB_LEAF : count;
+        rc = launch_fused(ix, normals_fused_kernel<3>, normals_fused_kernel<5>, lanes, k, s, points, first, count, perm,
+                          self_order ? 1 : 0, r2, k, out_normals);
+    }
+    cphb_free_async(perm, s);
+    const cudaError_t e = cudaStreamSynchronize(s);
     cphb_index_destroy(ix);
+    if (!rc && e != cudaSuccess) { cphb_set_error("normals_fused_kernel: %s", cudaGetErrorString(e)); rc = CPHB_ERR_CUDA; }
     return rc;
 }
 
@@ -286,23 +254,13 @@ extern "C" int cphb_color_gradient(const float *points, const float *normals, co
         cphb_set_error("cphb_color_gradient: invalid argument");
         return CPHB_ERR_INVALID;
     }
-    cphb_index *ix = nullptr;
-    int rc = cphb_index_create(points, n, stream, &ix);
-    if (rc) return rc;
-    int32_t *idx = nullptr;
-    float *d2 = nullptr;
-    rc = cphb_alloc_async((void **)&idx, sizeof(int32_t) * n * max_nn, s);
-    if (!rc) rc = cphb_alloc_async((void **)&d2, sizeof(float) * n * max_nn, s);
-    if (!rc) rc = cphb_search_radius(ix, points, n, radius, max_nn, idx, d2, nullptr, stream);
+    cphb_nbr_table t;
+    int rc = cphb_nbr_table_create(points, n, 0, n, 0, radius, max_nn, &t, s);
     if (!rc) {
-        CPHB_LAUNCH(color_gradient_kernel, (unsigned)((n + 127) / 128), 128, 0, s, points, normals, colors, n, idx, max_nn,
+        CPHB_LAUNCH(color_gradient_kernel, (unsigned)((n + 127) / 128), 128, 0, s, points, normals, colors, n, t.idx, max_nn,
                     out_gradient);
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) { cphb_set_error("color_gradient_kernel: %s", cudaGetErrorString(e)); rc = CPHB_ERR_CUDA; }
     }
-    cphb_free_async(idx, s);
-    cphb_free_async(d2, s);
-    cudaStreamSynchronize(s);
-    cphb_index_destroy(ix);
-    return rc;
+    return cphb_nbr_table_release(&t, rc, s);
 }

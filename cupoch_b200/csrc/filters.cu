@@ -247,26 +247,16 @@ extern "C" int cphb_remove_radius_outliers(const float *points, size_t n, int nb
         return CPHB_ERR_INVALID;
     }
     const int k = nb_points + 1;
-    cphb_index *ix = nullptr;
-    int rc = cphb_index_create(points, n, stream, &ix);  // the reference builds a fresh tree too (:324-325)
-    if (rc) return rc;
-    int32_t *idx = nullptr;
-    float *d2 = nullptr;
+    cphb_nbr_table t;
     uint8_t *keep = nullptr;
-    rc = cphb_alloc_async((void **)&idx, sizeof(int32_t) * n * k, s);
-    if (!rc) rc = cphb_alloc_async((void **)&d2, sizeof(float) * n * k, s);
+    int rc = cphb_nbr_table_create(points, n, 0, n, 0, radius, k, &t, s);  // the reference builds a fresh tree too (:324-325)
     if (!rc) rc = cphb_alloc_async((void **)&keep, n, s);
-    if (!rc) rc = cphb_search_radius(ix, points, n, radius, k, idx, d2, nullptr, stream);
     if (!rc) {
-        CPHB_LAUNCH(radius_keep_kernel, (unsigned)((n + 255) / 256), 256, 0, s, idx, n, k, nb_points, keep);
+        CPHB_LAUNCH(radius_keep_kernel, (unsigned)((n + 255) / 256), 256, 0, s, t.idx, n, k, nb_points, keep);
         rc = cphb_compact_flags(keep, n, indices_out, h_n_out, s);
     }
-    cphb_free_async(idx, s);
-    cphb_free_async(d2, s);
     cphb_free_async(keep, s);
-    cudaStreamSynchronize(s);
-    cphb_index_destroy(ix);
-    return rc;
+    return cphb_nbr_table_release(&t, rc, s);
 }
 
 extern "C" int cphb_remove_statistical_outliers(const float *points, size_t n, int nb_neighbors, float std_ratio,
@@ -288,24 +278,19 @@ extern "C" int cphb_remove_statistical_outliers(const float *points, size_t n, i
         return CPHB_ERR_INVALID;
     }
     const int k = nb_neighbors;
-    cphb_index *ix = nullptr;
-    int rc = cphb_index_create(points, n, stream, &ix);
-    if (rc) return rc;
     const unsigned nb = (unsigned)((n + FLT_BLOCK - 1) / FLT_BLOCK);
-    int32_t *idx = nullptr;
-    float *d2 = nullptr, *avg = nullptr, *scalars = nullptr;
+    cphb_nbr_table t;
+    float *avg = nullptr, *scalars = nullptr;
     double *partial = nullptr;
     uint8_t *keep = nullptr;
-    rc = cphb_alloc_async((void **)&idx, sizeof(int32_t) * n * k, s);
-    if (!rc) rc = cphb_alloc_async((void **)&d2, sizeof(float) * n * k, s);
+    int rc = cphb_nbr_table_create(points, n, 0, n, k, 0.f, 0, &t, s);
     if (!rc) rc = cphb_alloc_async((void **)&avg, sizeof(float) * n, s);
     if (!rc) rc = cphb_alloc_async((void **)&scalars, sizeof(float) * 4, s);
     if (!rc) rc = cphb_alloc_async((void **)&partial, sizeof(double) * 2 * (size_t)nb, s);
     if (!rc) rc = cphb_alloc_async((void **)&keep, n, s);
-    if (!rc) rc = cphb_search_knn(ix, points, n, k, idx, d2, nullptr, stream);
     if (!rc) {
         const unsigned g256 = (unsigned)((n + 255) / 256);
-        CPHB_LAUNCH(row_mean_kernel, g256, 256, 0, s, d2, n, k, avg);
+        CPHB_LAUNCH(row_mean_kernel, g256, 256, 0, s, t.d2, n, k, avg);
         CPHB_LAUNCH(stat_partial_kernel, nb, FLT_BLOCK, 0, s, avg, n, 0, scalars, partial);
         CPHB_LAUNCH(stat_final_kernel, 1, FLT_BLOCK, 0, s, partial, nb, 0, std_ratio, scalars);
         CPHB_LAUNCH(stat_partial_kernel, nb, FLT_BLOCK, 0, s, avg, n, 1, scalars, partial);
@@ -318,15 +303,11 @@ extern "C" int cphb_remove_statistical_outliers(const float *points, size_t n, i
             if (e != cudaSuccess) { cphb_set_error("cphb_remove_statistical_outliers: %s", cudaGetErrorString(e)); rc = CPHB_ERR_CUDA; }
         }
     }
-    cphb_free_async(idx, s);
-    cphb_free_async(d2, s);
     cphb_free_async(avg, s);
     cphb_free_async(scalars, s);
     cphb_free_async(partial, s);
     cphb_free_async(keep, s);
-    cudaStreamSynchronize(s);
-    cphb_index_destroy(ix);
-    return rc;
+    return cphb_nbr_table_release(&t, rc, s);
 }
 
 // PointCloud::GaussianFilter (pointcloud.cu:56-106,387-433): weighted mean of the neighbours found by a radius search
@@ -379,24 +360,15 @@ extern "C" int cphb_gaussian_filter(const float *points, const float *normals, c
         return CPHB_ERR_INVALID;
     }
     const int k = num_max_search_points;
-    cphb_index *ix = nullptr;
-    int rc = cphb_index_create(points, n, stream, &ix);
-    if (rc) return rc;
-    int32_t *idx = nullptr;
-    float *d2 = nullptr;
-    rc = cphb_alloc_async((void **)&idx, sizeof(int32_t) * n * k, s);
-    if (!rc) rc = cphb_alloc_async((void **)&d2, sizeof(float) * n * k, s);
-    if (!rc) rc = cphb_search_radius(ix, points, n, search_radius, k, idx, d2, nullptr, stream);
+    cphb_nbr_table t;
+    int rc = cphb_nbr_table_create(points, n, 0, n, 0, search_radius, k, &t, s);
     if (!rc) {
-        CPHB_LAUNCH(gaussian_filter_kernel, (unsigned)((n + 127) / 128), 128, 0, s, points, normals, colors, n, idx, d2, k, sigma2,
-                    out_points, out_normals, out_colors);
+        CPHB_LAUNCH(gaussian_filter_kernel, (unsigned)((n + 127) / 128), 128, 0, s, points, normals, colors, n, t.idx, t.d2, k,
+                    sigma2, out_points, out_normals, out_colors);
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) { cphb_set_error("gaussian_filter_kernel: %s", cudaGetErrorString(e)); rc = CPHB_ERR_CUDA; }
     }
-    cphb_free_async(idx, s);
-    cphb_free_async(d2, s);
-    cudaStreamSynchronize(s);
-    cphb_index_destroy(ix);
+    rc = cphb_nbr_table_release(&t, rc, s);
     if (!rc) *h_n_out = n;
     return rc;
 }

@@ -137,28 +137,16 @@ extern "C" int cphb_compute_fpfh_feature(const float *points, const float *norma
         cphb_set_error("cphb_compute_fpfh_feature: neighbour count %d outside [1, 100]", k);
         return CPHB_ERR_INVALID;
     }
-    cphb_index *ix = nullptr;
-    int rc = cphb_index_create(points, n, stream, &ix);
-    if (rc) return rc;
-    int32_t *idx = nullptr;
-    float *d2 = nullptr, *spfh = nullptr;
-    rc = cphb_alloc_async((void **)&idx, sizeof(int32_t) * n * k, s);
-    if (!rc) rc = cphb_alloc_async((void **)&d2, sizeof(float) * n * k, s);
+    cphb_nbr_table t;
+    float *spfh = nullptr;
+    int rc = cphb_nbr_table_create(points, n, 0, n, knn, radius, max_nn, &t, s);
     if (!rc) rc = cphb_alloc_async((void **)&spfh, sizeof(float) * n * 33, s);
     if (!rc) {
-        if (knn > 0) rc = cphb_search_knn(ix, points, n, k, idx, d2, nullptr, stream);
-        else rc = cphb_search_radius(ix, points, n, radius, k, idx, d2, nullptr, stream);
-    }
-    if (!rc) {
-        CPHB_LAUNCH(spfh_kernel, (unsigned)((n + 127) / 128), 128, 0, s, points, normals, n, idx, k, spfh);
-        CPHB_LAUNCH(fpfh_kernel, (unsigned)((n + 127) / 128), 128, 0, s, spfh, n, idx, d2, k, out_features);
+        CPHB_LAUNCH(spfh_kernel, (unsigned)((n + 127) / 128), 128, 0, s, points, normals, n, t.idx, k, spfh);
+        CPHB_LAUNCH(fpfh_kernel, (unsigned)((n + 127) / 128), 128, 0, s, spfh, n, t.idx, t.d2, k, out_features);
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) { cphb_set_error("fpfh kernels: %s", cudaGetErrorString(e)); rc = CPHB_ERR_CUDA; }
     }
-    cphb_free_async(idx, s);
-    cphb_free_async(d2, s);
     cphb_free_async(spfh, s);
-    cudaStreamSynchronize(s);
-    cphb_index_destroy(ix);
-    return rc;
+    return cphb_nbr_table_release(&t, rc, s);
 }

@@ -1,7 +1,8 @@
-// fused_neighbourhood.cuh -- the fused "k-best search, then a per-point epilogue over the list" form shared by
-// features.cu (EstimateNormals) and iss.cu (ComputeISSKeypoints): the warp's k-best search with its lists in shared
-// memory, the 9 cumulants over a lane's list in list order (geometry_functor.h:35-55) and the covariance
-// E[xx^T] - E[x]E[x]^T formed from them.  No [n][k] table is ever written.
+// fused_neighbourhood.cuh -- the "k-best search, then a per-point epilogue over the list" form shared by every k-list
+// kernel: search.cu (searchk_kernel, whose epilogue writes the [n][k] table), features.cu (EstimateNormals) and iss.cu
+// (ComputeISSKeypoints).  The warp's k-best search with its lists in shared memory, its one launch rule
+// (launch_fused), the 9 cumulants over a lane's list in list order (geometry_functor.h:35-55) and the covariance
+// E[xx^T] - E[x]E[x]^T formed from them; the fused epilogues write no [n][k] table.
 // Translation units including this must be compiled with -fmad=false.
 #pragma once
 #include "cphb_internal.cuh"
@@ -98,4 +99,25 @@ __device__ __forceinline__ void list_cumulants(const WarpSearchK &w, int k, unsi
 // dynamic shared memory of one warp of a fused kernel with k-slot lists
 static inline size_t fused_smem_per_warp(int k) {
     return 2 * CPHB_LEAF * sizeof(float4) + 2 * sizeof(uint64_t) + (size_t)k * 32 * sizeof(unsigned long long);
+}
+
+// launch of one k-list kernel over `lanes` query lanes (one thread each): as many warps per block as fit in 96 KB of
+// lists and tiles, 1 to 8; the <3> or <5> instance by the index's depth.  The kernel's first argument is the index view.
+template <class K3, class K5, class... Args>
+static int launch_fused(const cphb_index *ix, K3 k3, K5 k5, size_t lanes, int k, cudaStream_t s, Args... args) {
+    int warps = (int)((96 * 1024) / fused_smem_per_warp(k));
+    if (warps > 8) warps = 8;
+    if (warps < 1) warps = 1;
+    const size_t smem = fused_smem_per_warp(k) * warps;
+    const unsigned block = warps * 32;
+    const unsigned grid = (unsigned)((lanes + block - 1) / block);
+    if (ix->v.top <= 3) {
+        CPHB_CUDA(cudaFuncSetAttribute(k3, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
+        CPHB_LAUNCH(k3, grid, block, smem, s, ix->v, args...);
+    } else {
+        CPHB_CUDA(cudaFuncSetAttribute(k5, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
+        CPHB_LAUNCH(k5, grid, block, smem, s, ix->v, args...);
+    }
+    CPHB_CHECK_LAUNCH();
+    return CPHB_OK;
 }

@@ -134,26 +134,6 @@ __global__ void __launch_bounds__(256) iss_fill_kernel(float *__restrict__ salie
     mask[i] = 0;
 }
 
-// launch of one fused kernel over the index's lanes with k-slot lists
-template <class K3, class K5, class... Args>
-static int launch_fused(const cphb_index *ix, K3 k3, K5 k5, int k, cudaStream_t s, Args... args) {
-    int warps = (int)((96 * 1024) / fused_smem_per_warp(k));
-    if (warps > 8) warps = 8;
-    if (warps < 1) warps = 1;
-    const size_t smem = fused_smem_per_warp(k) * warps;
-    const unsigned block = warps * 32;
-    const unsigned grid = (unsigned)(((size_t)ix->v.n_leaves * CPHB_LEAF + block - 1) / block);
-    if (ix->v.top <= 3) {
-        CPHB_CUDA(cudaFuncSetAttribute(k3, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-        CPHB_LAUNCH(k3, grid, block, smem, s, ix->v, args...);
-    } else {
-        CPHB_CUDA(cudaFuncSetAttribute(k5, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-        CPHB_LAUNCH(k5, grid, block, smem, s, ix->v, args...);
-    }
-    CPHB_CHECK_LAUNCH();
-    return CPHB_OK;
-}
-
 extern "C" int cphb_compute_iss_keypoints(const float *points, size_t n, float salient_radius, float non_max_radius,
                                           float gamma_21, float gamma_32, int min_neighbors, int max_neighbors,
                                           uint8_t *mask_out, int32_t *indices_out, size_t *h_n_out, float *saliency_out,
@@ -186,13 +166,14 @@ extern "C" int cphb_compute_iss_keypoints(const float *points, size_t n, float s
     double *partial = nullptr;
     int32_t *idx = indices_out;
     int rc = cphb_index_create(points, n, s, &ix);
+    const size_t lanes = rc ? 0 : (size_t)ix->v.n_leaves * CPHB_LEAF;  // every search: the indexed points in index order
     if (!rc) rc = cphb_alloc_async((void **)&radii, 2 * sizeof(float), s);
     if (!rc && !sal) rc = cphb_alloc_async((void **)&sal, n * sizeof(float), s);
     if (!rc && !idx) rc = cphb_alloc_async((void **)&idx, n * sizeof(int32_t), s);
     if (!rc && automatic) {
         rc = cphb_alloc_async((void **)&d2_1, n * sizeof(float), s);
         if (!rc) rc = cphb_alloc_async((void **)&partial, n_tiles * sizeof(double), s);
-        if (!rc) rc = launch_fused(ix, iss_knn2_kernel<3>, iss_knn2_kernel<5>, 2, s, points, d2_1);
+        if (!rc) rc = launch_fused(ix, iss_knn2_kernel<3>, iss_knn2_kernel<5>, lanes, 2, s, points, d2_1);
         if (!rc) {
             CPHB_LAUNCH(iss_tile_sum_kernel, (unsigned)((n_tiles + 127) / 128), 128, 0, s, d2_1, n, partial);
             CPHB_LAUNCH(iss_radii_kernel, 1, 32, 0, s, partial, n_tiles, n, radii);
@@ -210,11 +191,11 @@ extern "C" int cphb_compute_iss_keypoints(const float *points, size_t n, float s
         CPHB_LAUNCH(iss_fill_kernel, (unsigned)((n + 255) / 256), 256, 0, s, sal, mask_out, n);
         CPHB_CHECK_LAUNCH();
     } else if (!rc) {
-        rc = launch_fused(ix, iss_saliency_kernel<3>, iss_saliency_kernel<5>, k, s, points, (const float *)radii, k,
+        rc = launch_fused(ix, iss_saliency_kernel<3>, iss_saliency_kernel<5>, lanes, k, s, points, (const float *)radii, k,
                           min_neighbors, gamma_21, gamma_32, sal);
         if (!rc)
-            rc = launch_fused(ix, iss_suppress_kernel<3>, iss_suppress_kernel<5>, k, s, points, (const float *)radii, k,
-                              (const float *)sal, mask_out);
+            rc = launch_fused(ix, iss_suppress_kernel<3>, iss_suppress_kernel<5>, lanes, k, s, points, (const float *)radii,
+                              k, (const float *)sal, mask_out);
     }
     if (!rc) rc = cphb_compact_flags(mask_out, n, idx, h_n_out, s);  // synchronises
     if (!rc && h_radii && automatic) {

@@ -11,6 +11,7 @@
 
 #include "cphb_internal.cuh"
 #include "cphb_searchk.cuh"
+#include "fused_neighbourhood.cuh"
 
 template <int TOP>
 __global__ void __launch_bounds__(256) search1_kernel(IndexView ix, const float *__restrict__ qxyz,
@@ -51,31 +52,10 @@ __global__ void searchk_kernel(IndexView ix, const float *__restrict__ qxyz, con
                                size_t nq, float r2, int k, int32_t *__restrict__ out_idx,
                                float *__restrict__ out_d2, unsigned long long *count) {
     extern __shared__ __align__(16) unsigned char smem[];
-    const int nwarp = blockDim.x >> 5;
-    const int warp = threadIdx.x >> 5;
-    float4 *tiles = (float4 *)smem;
-    uint64_t *bars = (uint64_t *)(tiles + (size_t)nwarp * 2 * CPHB_LEAF);
-    unsigned long long *lists = (unsigned long long *)(bars + 2 * nwarp);
     WarpSearchK w;
-    warp_search_setup(w, tiles + (size_t)warp * 2 * CPHB_LEAF, bars + 2 * warp);
-    w.k = k;
-    w.list = lists + (size_t)warp * k * 32 + lane_id();
-    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    w.valid = i < nq;
-    size_t pos = 0;
-    w.qx = w.qy = w.qz = 0.f;
-    if (w.valid) {
-        pos = perm ? perm[i] : i;
-        w.qx = qxyz[3 * pos];
-        w.qy = qxyz[3 * pos + 1];
-        w.qz = qxyz[3 * pos + 2];
-    }
-    const unsigned long long init = (r2 > 0.f) ? init_key(r2) : 0ull;  // r2==0: d2 < 0 never holds
-    for (int j = 0; j < k; ++j) w.list[j * 32] = init;
-    w.worst = init;
-    w.bound = (unsigned)(init >> 32);
-    warp_query_box(w);
-    if (__any_sync(CPHB_FULL, w.valid)) warp_nn_search<TOP>(ix, w);
+    size_t pos;
+    const unsigned long long init = fused_query_setup(w, smem, ix, qxyz, 0, nq, perm, 0, r2, k, pos);
+    fused_query_search<TOP>(ix, w);
     int filled = 0;
     if (w.valid) {
         for (int j = 0; j < k; ++j) {
@@ -97,6 +77,31 @@ __global__ void searchk_kernel(IndexView ix, const float *__restrict__ qxyz, con
 // k_limit: SearchKNN rejects knn > NUM_MAX_NN (kdtree_flann.cu:52-54); SearchRadius has no such check (:70-72) -- DBSCAN's
 // default asks for max_nn = 101 -- so there the limit is what one warp's lists can hold in shared memory
 #define CPHB_RADIUS_MAX_NN 256
+
+// the search kernel's launch, and the read-back of the found count into *h_count when it is given
+static int search_launch(const cphb_index *index, const float *query, const uint32_t *perm, size_t nq, float r2, int k,
+                         int32_t *idx, float *d2, unsigned long long *count, int64_t *h_count, cudaStream_t s) {
+    if (count) CPHB_CUDA(cudaMemsetAsync(count, 0, 8, s));
+    if (k == 1) {
+        const unsigned grid = (unsigned)((nq + 255) / 256);
+        if (index->v.top <= 3)
+            CPHB_LAUNCH(search1_kernel<3>, grid, 256, 0, s, index->v, query, perm, nq, r2, idx, d2, count);
+        else
+            CPHB_LAUNCH(search1_kernel<5>, grid, 256, 0, s, index->v, query, perm, nq, r2, idx, d2, count);
+        CPHB_CHECK_LAUNCH();
+    } else {
+        const int rc = launch_fused(index, searchk_kernel<3>, searchk_kernel<5>, nq, k, s, query, perm, nq, r2, k, idx, d2, count);
+        if (rc) return rc;
+    }
+    if (h_count) {
+        unsigned long long h = 0;
+        CPHB_CUDA(cudaMemcpyAsync(&h, count, 8, cudaMemcpyDeviceToHost, s));
+        CPHB_CUDA(cudaStreamSynchronize(s));
+        *h_count = (int64_t)h;
+    }
+    return CPHB_OK;
+}
+
 static int search_impl(const cphb_index *index, const float *query, size_t nq, float r2, int k, int k_limit, int32_t *idx,
                        float *d2, int64_t *h_count, cudaStream_t s) {
     if (!index || !query || !idx || !d2) {
@@ -116,51 +121,16 @@ static int search_impl(const cphb_index *index, const float *query, size_t nq, f
     if (k == 0) return CPHB_OK;
     uint32_t *perm = nullptr;
     unsigned long long *count = nullptr;
-    int rc;
+    int rc = CPHB_OK;
     if (nq > 32) {
         rc = cphb_alloc_async((void **)&perm, sizeof(uint32_t) * nq, s);
-        if (rc) return rc;
-        rc = cphb_hilbert_order_n(query, nq, perm, index->bounds, 1, nq < index->v.n ? nq : (size_t)index->v.n, s);
-        if (rc) { cphb_free_async(perm, s); return rc; }
+        if (!rc) rc = cphb_hilbert_order_n(query, nq, perm, index->bounds, 1, nq < index->v.n ? nq : (size_t)index->v.n, s);
     }
-    if (h_count) {
-        rc = cphb_alloc_async((void **)&count, 16, s);
-        if (rc) { cphb_free_async(perm, s); return rc; }
-        CPHB_CUDA(cudaMemsetAsync(count, 0, 8, s));
-    }
-    const int top = index->v.top;
-    if (k == 1) {
-        unsigned grid = (unsigned)((nq + 255) / 256);
-        if (top <= 3)
-            CPHB_LAUNCH(search1_kernel<3>, grid, 256, 0, s, index->v, query, perm, nq, r2, idx, d2, count);
-        else
-            CPHB_LAUNCH(search1_kernel<5>, grid, 256, 0, s, index->v, query, perm, nq, r2, idx, d2, count);
-    } else {
-        size_t per_warp = 2 * CPHB_LEAF * sizeof(float4) + 2 * sizeof(uint64_t) + (size_t)k * 32 * sizeof(unsigned long long);
-        int warps = (int)((96 * 1024) / per_warp);
-        if (warps > 8) warps = 8;
-        if (warps < 1) warps = 1;
-        size_t smem = per_warp * warps;
-        unsigned block = warps * 32;
-        unsigned grid = (unsigned)((nq + block - 1) / block);
-        if (top <= 3) {
-            CPHB_CUDA(cudaFuncSetAttribute(searchk_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-            CPHB_LAUNCH(searchk_kernel<3>, grid, block, smem, s, index->v, query, perm, nq, r2, k, idx, d2, count);
-        } else {
-            CPHB_CUDA(cudaFuncSetAttribute(searchk_kernel<5>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-            CPHB_LAUNCH(searchk_kernel<5>, grid, block, smem, s, index->v, query, perm, nq, r2, k, idx, d2, count);
-        }
-    }
-    CPHB_CHECK_LAUNCH();
+    if (!rc && h_count) rc = cphb_alloc_async((void **)&count, 16, s);
+    if (!rc) rc = search_launch(index, query, perm, nq, r2, k, idx, d2, count, h_count, s);
     cphb_free_async(perm, s);
-    if (h_count) {
-        unsigned long long h = 0;
-        CPHB_CUDA(cudaMemcpyAsync(&h, count, 8, cudaMemcpyDeviceToHost, s));
-        CPHB_CUDA(cudaStreamSynchronize(s));
-        *h_count = (int64_t)h;
-        cphb_free_async(count, s);
-    }
-    return CPHB_OK;
+    cphb_free_async(count, s);
+    return rc;
 }
 
 extern "C" int cphb_search_radius(const cphb_index *index, const float *query, size_t n_query, float radius,
@@ -175,4 +145,30 @@ extern "C" int cphb_search_hybrid(const cphb_index *index, const float *query, s
 extern "C" int cphb_search_knn(const cphb_index *index, const float *query, size_t n_query, int knn, int32_t *idx,
                                float *d2, int64_t *h_count, void *stream) {
     return search_impl(index, query, n_query, INFINITY, knn, 100, idx, d2, h_count, (cudaStream_t)stream);
+}
+
+int cphb_nbr_table_create(const float *points, size_t n, size_t first, size_t count, int knn, float radius, int max_nn,
+                          cphb_nbr_table *t, cudaStream_t s) {
+    const int k = (knn > 0) ? knn : max_nn;
+    int rc = cphb_index_create(points, n, s, &t->ix);
+    if (!rc) rc = cphb_alloc_async((void **)&t->idx, sizeof(int32_t) * count * k, s);
+    if (!rc) rc = cphb_alloc_async((void **)&t->d2, sizeof(float) * count * k, s);
+    if (!rc) {
+        const float *q = points + 3 * first;
+        if (knn > 0) rc = cphb_search_knn(t->ix, q, count, k, t->idx, t->d2, nullptr, s);
+        else rc = cphb_search_radius(t->ix, q, count, radius, k, t->idx, t->d2, nullptr, s);
+    }
+    return rc;
+}
+
+int cphb_nbr_table_release(cphb_nbr_table *t, int rc, cudaStream_t s) {
+    cphb_free_async(t->idx, s);
+    cphb_free_async(t->d2, s);
+    const cudaError_t e = cudaStreamSynchronize(s);
+    cphb_index_destroy(t->ix);
+    if (!rc && e != cudaSuccess) {
+        cphb_set_error("neighbour-table client: %s", cudaGetErrorString(e));
+        return CPHB_ERR_CUDA;
+    }
+    return rc;
 }

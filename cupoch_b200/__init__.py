@@ -5,7 +5,8 @@
             cph.registration.TransformationEstimationPointToPlane())
 
 Mirrors `import cupoch as cph` for: cph.geometry.{PointCloud, KDTreeFlann, KDTreeSearchParamKNN,
-KDTreeSearchParamRadius, VoxelGrid, OccupancyGrid, OccupancyVoxel, keypoint.compute_iss_keypoints},
+KDTreeSearchParamRadius, VoxelGrid, OccupancyGrid, OccupancyVoxel, DistanceTransform, DistanceVoxel,
+keypoint.compute_iss_keypoints},
 cph.registration.{registration_icp,
 registration_generalized_icp, registration_colored_icp, ICPConvergenceCriteria, TransformationEstimation*
 (user subclasses run the generic loop), RegistrationResult, compute_fpfh_feature, kabsch, kabsch_weighted},

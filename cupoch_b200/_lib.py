@@ -11,6 +11,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libcupoch_b200.so")
 
 OK = 0
+CPHB_ERR_INVALID = -1
 EST_UNSPECIFIED, EST_POINT_TO_POINT, EST_POINT_TO_PLANE, EST_SYMMETRIC, EST_COLORED_ICP, EST_GENERALIZED_ICP = range(6)
 
 
@@ -62,6 +63,18 @@ _SIGNATURES = {
     "cphb_occgrid_bounds": (C.c_int, [_P, _I3, _I3, _P]),
     "cphb_occgrid_extract": (C.c_int, [_P, C.c_int, _P, _P, C.c_size_t, C.POINTER(C.c_size_t), _P]),
     "cphb_occgrid_get_voxel": (C.c_int, [_P, _F3, C.POINTER(C.c_int), C.POINTER(C.c_float), _I3, _P]),
+    "cphb_occgrid_get_params": (C.c_int, [_P, C.POINTER(OccGridParams)]),
+    "cphb_dt_create": (C.c_int, [C.c_float, C.c_int, _F3, _P, C.POINTER(_P)]),
+    "cphb_dt_destroy": (None, [_P]),
+    "cphb_dt_reconstruct": (C.c_int, [_P, C.c_float, C.c_int, _P]),
+    "cphb_dt_set_geometry": (C.c_int, [_P, C.c_float, _F3]),
+    "cphb_dt_compute_sites": (C.c_int, [_P, _P, C.c_size_t, C.c_int, _P]),
+    "cphb_dt_compute_voxel_grid": (C.c_int, [_P, _P, C.c_size_t, C.c_float, _F3, C.c_int, _P]),
+    "cphb_dt_from_occgrid": (C.c_int, [_P, _P, C.POINTER(_P)]),
+    "cphb_dt_get_distances": (C.c_int, [_P, _P, C.c_size_t, _P, _P]),
+    "cphb_dt_get_voxel": (C.c_int, [_P, _F3, C.POINTER(C.c_int), _I3, C.POINTER(C.c_int), C.POINTER(C.c_float), _P]),
+    "cphb_dt_distance_data": (_P, [_P]),
+    "cphb_dt_nearest_data": (_P, [_P]),
     # name: (restype, argtypes)
     "cphb_version": (C.c_int, []),
     "cphb_last_error": (C.c_char_p, []),

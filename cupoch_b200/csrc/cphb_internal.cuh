@@ -109,6 +109,9 @@ int cphb_nbr_table_create(const float *points, size_t n, size_t first, size_t co
                           cphb_nbr_table *t, cudaStream_t s);
 int cphb_nbr_table_release(cphb_nbr_table *t, int rc, cudaStream_t s);
 
+// the grid's voxel size and origin (occgrid.cu), for the DistanceTransform built from it (edt.cu)
+void cphb_occgrid_geometry(const cphb_occgrid *g, float *voxel_size, float origin[3]);
+
 // index.cu internals reused by icp.cu (Hilbert-ordering of the source)
 // perm_out[pos] = original index of the pos-th point along the Hilbert curve.
 // bounds_dev6: device buffer of 6 ordered-uint floats; computed here unless

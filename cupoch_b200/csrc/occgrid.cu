@@ -311,6 +311,15 @@ extern "C" int cphb_occgrid_set_params(cphb_occgrid *g, const cphb_occgrid_param
     g->prm = *p;
     return CPHB_OK;
 }
+extern "C" int cphb_occgrid_get_params(const cphb_occgrid *g, cphb_occgrid_params *p) {
+    if (!g || !p) { cphb_set_error("cphb_occgrid_get_params: null argument"); return CPHB_ERR_INVALID; }
+    *p = g->prm;
+    return CPHB_OK;
+}
+void cphb_occgrid_geometry(const cphb_occgrid *g, float *voxel_size, float origin[3]) {
+    *voxel_size = g->voxel_size;
+    for (int a = 0; a < 3; ++a) origin[a] = g->origin[a];
+}
 extern "C" int cphb_occgrid_set_geometry(cphb_occgrid *g, float voxel_size, const float origin[3]) {
     if (!g) { cphb_set_error("cphb_occgrid_set_geometry: null grid"); return CPHB_ERR_INVALID; }
     g->voxel_size = voxel_size;  // the reference exposes voxel_size_ / origin_ as plain members (its tests assign them)

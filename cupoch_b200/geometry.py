@@ -566,6 +566,122 @@ class OccupancyGrid:
             pass
 
 
+class DistanceVoxel:
+    """geometry::DistanceVoxel (distancetransform.h:30-49; pybind distancetransform.cpp:34-53): nearest_index (3 uint16,
+    the nearest site's grid cell) and distance (float32)."""
+
+    def __init__(self, nearest_index=(0, 0, 0), distance=0.0):
+        self.nearest_index = np.asarray(nearest_index, np.uint16)
+        self.distance = float(np.float32(distance))
+
+    def __repr__(self):
+        return "geometry::DistanceVoxel with nearest_index: (%d, %d, %d), distance: %f)" % (*self.nearest_index.tolist(), self.distance)
+
+
+class DistanceTransform:
+    """geometry::DistanceTransform (distancetransform.h:51-78; pybind distancetransform.cpp:55-93): a dense res^3 grid of
+    nearest sites and the Euclidean distances to them, on the device.  `voxel_size` and `origin` are plain attributes as
+    in the reference; `resolution` is read-only (reconstruct changes it)."""
+
+    def __init__(self, voxel_size=0.05, resolution=512, origin=(0.0, 0.0, 0.0), _handle=None):
+        _lib.require_gpu()
+        self._voxel_size, self._resolution = float(np.float32(voxel_size)), int(resolution)
+        self._origin = np.asarray(origin, np.float32).reshape(3).copy()
+        if _handle is not None:
+            self._h = _handle
+            return
+        self._h = C.c_void_p()
+        _lib.check(_lib.lib().cphb_dt_create(self._voxel_size, self._resolution, OccupancyGrid._f3(self._origin), None,
+                                             C.byref(self._h)))
+
+    voxel_size = property(lambda s: s._voxel_size, lambda s, v: s._set_geometry(voxel_size=v))
+    origin = property(lambda s: s._origin, lambda s, v: s._set_geometry(origin=v))
+    resolution = property(lambda s: s._resolution)
+
+    def _set_geometry(self, voxel_size=None, origin=None):
+        if voxel_size is not None:
+            self._voxel_size = float(np.float32(voxel_size))
+        if origin is not None:
+            self._origin = np.asarray(origin, np.float32).reshape(3).copy()
+        _lib.check(_lib.lib().cphb_dt_set_geometry(self._h, self._voxel_size, OccupancyGrid._f3(self._origin)))
+
+    def reconstruct(self, voxel_size, resolution):
+        """Reconstruct (densegrid.inl:128-134): the linear prefix of the old cells is kept, the rest are defaults"""
+        _lib.check(_lib.lib().cphb_dt_reconstruct(self._h, float(voxel_size), int(resolution), None))
+        self._voxel_size, self._resolution = float(np.float32(voxel_size)), int(resolution)
+        return self
+
+    def _compute(self, sites, with_distance):
+        if isinstance(sites, VoxelGrid):
+            keys = sites.voxels_keys
+            rc = _lib.lib().cphb_dt_compute_voxel_grid(self._h, keys.ptr if keys is not None else None, len(sites),
+                                                       float(sites.voxel_size), OccupancyGrid._f3(sites.origin),
+                                                       int(with_distance), None)
+            if rc == _lib.CPHB_ERR_INVALID:  # distancetransform.cu:331-337: logged, the grid is unchanged
+                print("[cupoch_b200][error] %s" % _lib.lib().cphb_last_error().decode(errors="replace"), file=sys.stderr)
+                return self
+            _lib.check(rc)
+            return self
+        if not isinstance(sites, DeviceArray) and not hasattr(sites, "is_cuda"):
+            sites = np.asarray(sites, np.int32).reshape(-1, 3)
+        d = DeviceArray.wrap(sites, np.int32)
+        _lib.check(_lib.lib().cphb_dt_compute_sites(self._h, d.ptr if len(d) else None, len(d), int(with_distance), None))
+        return self
+
+    def compute_edt(self, voxel_grid):
+        """ComputeEDT(VoxelGrid | [n, 3] int32 grid cells) (distancetransform.cu:320-345)"""
+        return self._compute(voxel_grid, True)
+
+    def compute_voronoi_diagram(self, voxel_grid):
+        """ComputeVoronoiDiagram(VoxelGrid | [n, 3] int32 grid cells): nearest sites only, every distance 0"""
+        return self._compute(voxel_grid, False)
+
+    def get_distances(self, points):
+        """GetDistances (:421-435): host or device [n, 3] points -> device float32 [n]; 0 outside the grid or for NaN"""
+        q = Vector3fVector(points)
+        n = 0 if q is None else len(q)
+        out = DeviceArray((n,), np.float32)
+        if n:
+            _lib.check(_lib.lib().cphb_dt_get_distances(self._h, q.ptr, n, out.ptr, None))
+        return out
+
+    def get_distance(self, point):
+        """GetDistance (:411-419)"""
+        return float(self.get_distances(np.asarray(point, np.float32).reshape(1, 3)).cpu()[0])
+
+    def get_voxel(self, point):
+        """-> (found, DistanceVoxel)  (DenseGrid::GetVoxel, densegrid.inl:148-155)"""
+        f, nb, st, d = C.c_int(0), (C.c_int32 * 3)(), C.c_int(0), C.c_float(0)
+        _lib.check(_lib.lib().cphb_dt_get_voxel(self._h, OccupancyGrid._f3(point), C.byref(f), nb, C.byref(st), C.byref(d), None))
+        return bool(f.value), DistanceVoxel(list(nb), d.value)
+
+    @staticmethod
+    def create_from_occupancy_grid(occupancy_grid):
+        """CreateFromOccupancyGrid (distancetransform_factory.cu:40-62), with the EDT of the occupied cells computed"""
+        occupancy_grid._sync_params()
+        h = C.c_void_p()
+        _lib.check(_lib.lib().cphb_dt_from_occgrid(occupancy_grid._h, None, C.byref(h)))
+        return DistanceTransform(occupancy_grid.voxel_size, occupancy_grid.resolution, occupancy_grid.origin, _handle=h)
+
+    def to_torch(self):
+        """zero-copy [res, res, res] float32 CUDA tensor of the distances"""
+        import torch
+        r = self._resolution
+        return torch.as_tensor(DeviceArray((r, r, r), np.float32, ptr=_lib.lib().cphb_dt_distance_data(self._h), base=self), device="cuda")
+
+    def __repr__(self):
+        return "geometry::DistanceTransform with %d resolution." % self._resolution
+
+    def __del__(self):
+        try:
+            if self._h:
+                _lib.lib().cphb_stream_synchronize(None)
+                _lib.lib().cphb_dt_destroy(self._h)
+                self._h = None
+        except Exception:
+            pass
+
+
 class KDTreeFlann:
     """knn::KDTreeFlann (kdtree_flann.h:43-124), exposed as cupoch.geometry.KDTreeFlann
     (kdtree_flann.cpp:93-95)."""

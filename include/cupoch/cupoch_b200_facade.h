@@ -671,6 +671,7 @@ public:
     bool visualize_free_area_ = true;
 
 private:
+    friend class DistanceTransform;  // CreateFromOccupancyGrid reads the dense grid
     void sync() const {  // the public members are the source of truth, like the reference's
         const float o[3] = {origin_[0], origin_[1], origin_[2]};
         utility::check(cphb_occgrid_set_geometry(h_, voxel_size_, o));
@@ -692,6 +693,105 @@ private:
         return out;
     }
     cphb_occgrid *h_ = nullptr;
+};
+
+/// geometry::DistanceVoxel (distancetransform.h:30-49)
+class DistanceVoxel {
+public:
+    enum State { HasNext = 1, NotSite = 1 << 1 };
+    DistanceVoxel() {}
+    DistanceVoxel(const Eigen::Vector3i &nearest_index, unsigned char state) : nearest_index_(nearest_index), state_(state) {}
+    bool IsNotSite() const { return state_ & NotSite; }
+    bool CheckHasNext() const { return state_ & HasNext; }
+    Eigen::Vector3i nearest_index_ = Eigen::Vector3i(0, 0, 0);  // (Vector3ui16 in the reference)
+    unsigned char state_ = NotSite;
+    float distance_ = 0;
+};
+
+/// geometry::DistanceTransform (distancetransform.h:51-78): a dense resolution^3 grid of nearest sites and Euclidean
+/// distances.  voxel_size_ and origin_ are public as in the reference and handed to the engine at every call;
+/// resolution_ changes only through Reconstruct.  A voxel-size mismatch with the VoxelGrid is logged and leaves the grid
+/// unchanged.  Among equidistant sites the lexicographically smallest is the nearest one.
+class DistanceTransform {
+public:
+    DistanceTransform() : DistanceTransform(0.05f, 512) {}
+    DistanceTransform(float voxel_size, size_t resolution, const Eigen::Vector3f &origin = Eigen::Vector3f(0.f, 0.f, 0.f))
+        : voxel_size_(voxel_size), resolution_(resolution), origin_(origin) {
+        const float o[3] = {origin[0], origin[1], origin[2]};
+        utility::check(cphb_dt_create(voxel_size, (int)resolution, o, nullptr, &h_));
+    }
+    ~DistanceTransform() { cphb_stream_synchronize(nullptr); cphb_dt_destroy(h_); }
+    DistanceTransform(const DistanceTransform &) = delete;
+    DistanceTransform &operator=(const DistanceTransform &) = delete;
+
+    DistanceTransform &Reconstruct(float voxel_size, size_t resolution) {
+        utility::check(cphb_dt_reconstruct(h_, voxel_size, (int)resolution, nullptr));
+        voxel_size_ = voxel_size;
+        resolution_ = resolution;
+        return *this;
+    }
+    DistanceTransform &ComputeEDT(const utility::device_vector<Eigen::Vector3i> &points) { return compute(points, 1); }
+    DistanceTransform &ComputeEDT(const VoxelGrid &voxelgrid) { return compute(voxelgrid, 1); }
+    DistanceTransform &ComputeVoronoiDiagram(const utility::device_vector<Eigen::Vector3i> &points) { return compute(points, 0); }
+    DistanceTransform &ComputeVoronoiDiagram(const VoxelGrid &voxelgrid) { return compute(voxelgrid, 0); }
+
+    float GetDistance(const Eigen::Vector3f &query) const {
+        utility::device_vector<Eigen::Vector3f> q(std::vector<Eigen::Vector3f>(1, query));
+        return GetDistances(q)->to_host()[0];
+    }
+    std::unique_ptr<utility::device_vector<float>> GetDistances(const utility::device_vector<Eigen::Vector3f> &queries) const {
+        sync();
+        auto out = std::make_unique<utility::device_vector<float>>(queries.size());
+        if (queries.size())
+            utility::check(cphb_dt_get_distances(h_, reinterpret_cast<const float *>(queries.data()), queries.size(), out->data(), nullptr));
+        return out;
+    }
+    std::tuple<bool, DistanceVoxel> GetVoxel(const Eigen::Vector3f &point) const {  // densegrid.inl:148-155
+        sync();
+        const float p[3] = {point[0], point[1], point[2]};
+        int found = 0, state = 0, nb[3];
+        float d = 0.f;
+        utility::check(cphb_dt_get_voxel(h_, p, &found, nb, &state, &d, nullptr));
+        DistanceVoxel v(Eigen::Vector3i(nb[0], nb[1], nb[2]), (unsigned char)state);
+        v.distance_ = d;
+        return std::make_tuple(found != 0, v);
+    }
+    /// the reference stamps only the occupied cells; here the EDT of the occupied cells is computed
+    static std::shared_ptr<DistanceTransform> CreateFromOccupancyGrid(const OccupancyGrid &input) {
+        if (input.voxel_size_ <= 0.0) utility::LogError("[CreateOccupancyGrid] occupancy grid  voxel_size <= 0.");
+        input.sync();
+        cphb_dt *h = nullptr;
+        utility::check(cphb_dt_from_occgrid(input.h_, nullptr, &h));
+        return std::shared_ptr<DistanceTransform>(new DistanceTransform(h, input.voxel_size_, input.resolution_, input.origin_));
+    }
+
+public:
+    float voxel_size_ = 0.05f;
+    size_t resolution_ = 512;
+    Eigen::Vector3f origin_ = Eigen::Vector3f(0.f, 0.f, 0.f);
+
+private:
+    DistanceTransform(cphb_dt *h, float voxel_size, size_t resolution, const Eigen::Vector3f &origin)
+        : voxel_size_(voxel_size), resolution_(resolution), origin_(origin), h_(h) {}
+    void sync() const {
+        const float o[3] = {origin_[0], origin_[1], origin_[2]};
+        utility::check(cphb_dt_set_geometry(h_, voxel_size_, o));
+    }
+    DistanceTransform &compute(const utility::device_vector<Eigen::Vector3i> &points, int with_distance) {
+        sync();
+        utility::check(cphb_dt_compute_sites(h_, reinterpret_cast<const int32_t *>(points.data()), points.size(), with_distance, nullptr));
+        return *this;
+    }
+    DistanceTransform &compute(const VoxelGrid &vg, int with_distance) {
+        sync();
+        const float o[3] = {vg.origin_[0], vg.origin_[1], vg.origin_[2]};
+        const int rc = cphb_dt_compute_voxel_grid(h_, reinterpret_cast<const int32_t *>(vg.voxels_keys_.data()), vg.voxels_keys_.size(),
+                                                  vg.voxel_size_, o, with_distance, nullptr);
+        if (rc == CPHB_ERR_INVALID) utility::LogError("Unsupport computing Voronoi diagrams from different voxel size.");
+        else utility::check(rc);
+        return *this;
+    }
+    cphb_dt *h_ = nullptr;
 };
 
 namespace keypoint {

@@ -394,6 +394,49 @@ int cphb_occgrid_extract(const cphb_occgrid *grid, int which, int32_t *out_index
 /* GetVoxel(point) (:351-356, densegrid.inl:137-146): *h_known = inside the grid and not NaN */
 int cphb_occgrid_get_voxel(const cphb_occgrid *grid, const float point[3], int *h_known, float *h_prob_log,
                            int32_t h_grid_index[3], void *stream);
+/* the five probability parameters cphb_occgrid_set_params last set (the defaults before that) */
+int cphb_occgrid_get_params(const cphb_occgrid *grid, cphb_occgrid_params *p);
+
+/* ------------------------------------------------------------------------ *
+ * geometry::DistanceTransform (distancetransform.h, distancetransform.cu): a
+ * dense resolution^3 grid, cell (x, y, z) at linear index (x * res + y) * res + z
+ * and centred on origin like the OccupancyGrid.  Each cell holds its nearest
+ * site and the distance to it: nearest is u32 x << 20 | y << 10 | z with bit 30
+ * = DistanceVoxel::NotSite, distance is float32 |nearest - cell| * voxel_size.
+ * Among equidistant sites the lexicographically smallest (x, y, z) is taken.  A
+ * fresh grid, and every cell Reconstruct adds, is nearest (0,0,0), NotSite,
+ * distance 0.  1 <= resolution <= 1024, else CPHB_ERR_INVALID.  The compute
+ * calls are stream-ordered (no host synchronisation) and start from an empty
+ * site set: a clear, a stamp and three sweeps, whatever the resolution.
+ * ------------------------------------------------------------------------ */
+typedef struct cphb_dt cphb_dt;
+/* DistanceTransform(voxel_size, resolution = 512, origin = 0) (distancetransform.cu:293-301) */
+int cphb_dt_create(float voxel_size, int resolution, const float origin[3], void *stream, cphb_dt **out);
+void cphb_dt_destroy(cphb_dt *dt);
+/* Reconstruct (densegrid.inl:128-134): the linear prefix of the old cells is kept, distances are not rescaled */
+int cphb_dt_reconstruct(cphb_dt *dt, float voxel_size, int resolution, void *stream);
+int cphb_dt_set_geometry(cphb_dt *dt, float voxel_size, const float origin[3]); /* voxel_size_ / origin_ */
+/* ComputeEDT (with_distance = 1) / ComputeVoronoiDiagram (0, every distance 0) of device [n][3] int32 grid indices;
+ * indices outside the grid are ignored.  No site at all: every nearest is (0,0,0) with NotSite, its distance
+ * |cell| * voxel_size (0 for the Voronoi diagram). */
+int cphb_dt_compute_sites(cphb_dt *dt, const int32_t *cells, size_t n, int with_distance, void *stream);
+/* the same from VoxelGrid keys (device [n][3] int32): cell = floor(((key * vs + vg_origin) - origin) / vs) + res / 2
+ * with vs the transform's voxel size, each operation rounded on its own (distancetransform.cu:254-260).
+ * |voxel_size - vg_voxel_size| > FLT_EPSILON: CPHB_ERR_INVALID and the grid is left unchanged. */
+int cphb_dt_compute_voxel_grid(cphb_dt *dt, const int32_t *keys, size_t n, float vg_voxel_size, const float vg_origin[3],
+                               int with_distance, void *stream);
+/* CreateFromOccupancyGrid (distancetransform_factory.cu:40-62): a new transform with the grid's voxel size,
+ * resolution and origin, and the EDT of its occupied cells (!isnan(p) && p > occ_prob_thres_log) */
+int cphb_dt_from_occgrid(const cphb_occgrid *grid, void *stream, cphb_dt **out);
+/* GetDistances (:421-435): out[i] = distance of cell floor(((q - origin) + (0.5 * vs) * res) / vs); 0 for a query
+ * outside the grid or with a NaN coordinate.  points, out: device. */
+int cphb_dt_get_distances(const cphb_dt *dt, const float *points, size_t n, float *out, void *stream);
+/* GetVoxel (densegrid.inl:137-155): cell floor((point - origin) / vs) + res / 2.  Outside the grid or NaN:
+ * *h_found = 0 and the default voxel.  h_state: 0, or 2 (NotSite).  Synchronises. */
+int cphb_dt_get_voxel(const cphb_dt *dt, const float point[3], int *h_found, int32_t h_nearest[3], int *h_state,
+                      float *h_distance, void *stream);
+const float *cphb_dt_distance_data(const cphb_dt *dt);   /* device distance[res^3], borrowed */
+const uint32_t *cphb_dt_nearest_data(const cphb_dt *dt); /* device nearest[res^3] (packed as above), borrowed */
 
 /* registration::EvaluateRegistration (registration.cu:106-119). */
 int cphb_evaluate_registration(const cphb_cloud *source, const cphb_cloud *target,

@@ -30,7 +30,11 @@ def main():
                     help="instead: time PointCloud::FarthestPointDownSample at N = 100 k, 1 M, 10 M and 1024, 8192 samples")
     ap.add_argument("--iss", action="store_true",
                     help="instead: time geometry::keypoint::ComputeISSKeypoints (defaults, automatic radii) at N = 1 M, 10 M")
+    ap.add_argument("--edt", action="store_true",
+                    help="instead: time geometry::DistanceTransform::ComputeEDT at 256^3 and 512^3 and GetDistances of 10 M points")
     args = ap.parse_args()
+    if args.edt:
+        return edt(args.reps)
     if args.segment_plane:
         return segment_plane(args.reps)
     if args.fps:
@@ -416,6 +420,102 @@ def iss(reps):
                      "speedup_vs_reference_shaped": t_med / med})
     print(json.dumps({"op": "geometry::keypoint::ComputeISSKeypoints(defaults) on datagen.surface(N, 11)", "gpu": gpu,
                       "reps": reps, "launches": int(L.cphb_launch_count()), "rows": rows}))
+
+
+HBM_BYTES_PER_S = 3.35e12  # H100 SXM data sheet
+
+
+def edt_bytes_model(r):
+    """HBM bytes of one ComputeEDT at res r (a model, not a measurement).  Per cell: the bitmap clear, stamp and read
+    (3 / 8 B); sweep z writes nearest (4 B); sweeps y and x each read nearest, write and read back their stack and write
+    nearest (16 B), and sweep x also writes the distance (4 B).  A stack entry is written only for a candidate that is
+    not dominated when it arrives and read back only where the envelope moves, so the stack terms lie between 0 and 8 B
+    per sweep: 24.4 B per cell at least, 40.4 B at most."""
+    cells = r ** 3
+    return {"min": int(cells * (3 / 8 + 4 + 8 + 12)), "max": int(cells * (3 / 8 + 4 + 16 + 20))}
+
+
+def edt(reps):
+    """DistanceTransform(1 / r, r).compute_edt(voxel grid) at r = 256 and 512: CUDA-event time of the whole call (clear,
+    stamp, three sweeps), median of `reps` calls after one warm-up call, and the same for compute_voronoi_diagram.  The
+    sites are datagen.surface sheets (z = 0.1 sin(4 pi x) cos(4 pi y)) stacked along z and voxelised at the grid's own
+    voxel size, about 1 % of the cells.  The device result is checked against the CPU oracle at 256^3.  Then
+    get_distances of 10 M uniform points in the grid's box.  CPU arm: scipy.ndimage.distance_transform_edt of the same
+    site mask on the host (single-threaded: scipy's EDT has no thread option), one call."""
+    import subprocess
+    from scipy import ndimage
+    import cupoch_b200 as cph
+    from cupoch_b200 import _lib
+    from cupoch_b200.testing import datagen
+    from cupoch_b200.utility import DeviceArray
+    from oracle import edt_py
+    L = _lib.lib()
+    G = cph.geometry
+    gpu = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                         capture_output=True, text=True).stdout.strip()
+    ev = [L.cphb_event_create() for _ in range(2)]
+
+    def timed(fn):
+        calls = []
+        for k in range(reps + 1):
+            L.cphb_event_record(ev[0], None)
+            fn()
+            L.cphb_event_record(ev[1], None)
+            ms = C.c_float(0)
+            _lib.check(L.cphb_event_elapsed_ms(ev[0], ev[1], C.byref(ms)))
+            if k:
+                calls.append(ms.value)
+        return float(np.median(calls)), float(np.min(calls))
+
+    rows = []
+    for r in (256, 512):
+        vs = 1.0 / r
+        layers = r // 100 + 1
+        sheets = []
+        for i in range(layers):
+            p = datagen.surface(4 * r * r, 70 + i)[0]
+            p[:, 2] += np.float32(-0.35 + 0.7 * (i + 0.5) / layers)
+            sheets.append(p)
+        pts = np.concatenate(sheets)
+        vg = G.VoxelGrid.create_from_point_cloud_within_bounds(G.PointCloud(pts), vs, (0, 0, -0.5), (1, 1, 0.5))
+        dt = G.DistanceTransform(vs, r, (0.5, 0.5, 0.0))
+        edt_ms, edt_min = timed(lambda: dt.compute_edt(vg))
+        vor_ms, vor_min = timed(lambda: dt.compute_voronoi_diagram(vg))
+        dt.compute_edt(vg)
+        dist = dt.to_torch().cpu().numpy()
+        near = DeviceArray((r, r, r), np.uint32, ptr=L.cphb_dt_nearest_data(dt._h), base=dt).cpu()
+        sites = (near & ((1 << 30) - 1)) == edt_cell_codes(r)
+        occupancy = float(sites.mean())
+        row = {"res": r, "voxel_grid_keys": len(vg), "site_occupancy": occupancy, "compute_edt_ms_median": edt_ms,
+               "compute_edt_ms_min": edt_min, "compute_voronoi_ms_median": vor_ms, "compute_voronoi_ms_min": vor_min}
+        model = edt_bytes_model(r)
+        row["bytes_model"] = model
+        row["bytes_model_share_of_hbm_peak"] = {k: v / HBM_BYTES_PER_S / (edt_ms * 1e-3) for k, v in model.items()}
+        if r == 256:
+            o = edt_py.compute_voxel_grid(r, vs, (0.5, 0.5, 0.0), vg.voxels_keys.cpu(), vg.voxel_size, vg.origin)
+            row["oracle_parity"] = bool(np.array_equal(o[2].view(np.uint32), dist.view(np.uint32)) and
+                                        np.array_equal(o[1] == 2, (near >> 30) & 1 == 1))
+        t0 = time.perf_counter()
+        ref = ndimage.distance_transform_edt(~sites)
+        row["scipy_edt_cpu"] = {"seconds": time.perf_counter() - t0, "threads": 1,
+                                "max_abs_diff_in_voxels": float(np.abs(ref * vs - dist).max() / vs)}
+        rows.append(row)
+        if r == 512:
+            n = 10_000_000
+            q = DeviceArray.from_numpy(datagen.uniform_cube(n, 5, lo=(0, 0, -0.5), hi=(1, 1, 0.5)))
+            q_ms, q_min = timed(lambda: dt.get_distances(q))
+            query = {"res": r, "queries": n, "ms_median": q_ms, "ms_min": q_min,
+                     "bytes_model": n * (12 + 4 + 4), "note": "12 B point + 4 B result + one 4 B distance gather per query"}
+        del dt
+    print(json.dumps({"op": "geometry::DistanceTransform::ComputeEDT(VoxelGrid) and GetDistances", "gpu": gpu, "reps": reps,
+                      "hbm_peak_bytes_per_s": HBM_BYTES_PER_S, "launches": int(L.cphb_launch_count()), "rows": rows,
+                      "get_distances": query}))
+
+
+def edt_cell_codes(r):
+    """x << 20 | y << 10 | z of every cell of an r^3 grid (a site is its own nearest site)"""
+    g = np.arange(r, dtype=np.uint32)
+    return (g[:, None, None] << 20) | (g[None, :, None] << 10) | g[None, None, :]
 
 
 if __name__ == "__main__":

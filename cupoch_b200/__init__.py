@@ -9,7 +9,7 @@ KDTreeSearchParamRadius, VoxelGrid, OccupancyGrid, OccupancyVoxel, DistanceTrans
 keypoint.compute_iss_keypoints},
 cph.registration.{registration_icp,
 registration_generalized_icp, registration_colored_icp, ICPConvergenceCriteria, TransformationEstimation*
-(user subclasses run the generic loop), RegistrationResult, compute_fpfh_feature, kabsch, kabsch_weighted},
+(user subclasses run the generic loop), RegistrationResult, compute_fpfh_feature, compute_shot_feature, FeatureSHOT, kabsch, kabsch_weighted},
 cph.utility.{Vector3fVector, compute_jtj_jtr, compute_weighted_jtj_jtr}; cupoch_b200.distributed holds the
 multi-GPU orchestration (torch.distributed).  All computation runs in libcupoch_b200.so (hand-written sm_90a CUDA);
 there is no CPU fallback.

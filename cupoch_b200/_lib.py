@@ -130,6 +130,7 @@ _SIGNATURES = {
     "cphb_compute_weighted_jtj_jtr": (C.c_int, [_P, _P, C.c_size_t, C.c_int, C.c_float, C.c_float, C.POINTER(C.c_double),
                                                  C.POINTER(C.c_float), _P]),
     "cphb_compute_fpfh_feature": (C.c_int, [_P, _P, C.c_size_t, C.c_int, C.c_float, C.c_int, _P, _P]),
+    "cphb_compute_shot_feature": (C.c_int, [_P, _P, C.c_size_t, C.c_float, C.c_int, C.c_float, C.c_int, _P, _P]),
     "cphb_cluster_dbscan": (C.c_int, [_P, C.c_size_t, C.c_float, C.c_int, C.c_int, _P, C.POINTER(C.c_int), _P]),
     "cphb_reserve_pool": (C.c_int, [C.c_size_t]),
     "cphb_malloc": (_P, [C.c_size_t]),

@@ -1,6 +1,7 @@
 // cphb_eigen3.cuh -- small fixed-size float32 linear algebra shared by icp.cu and
 // features.cu: cross products, the analytic symmetric 3x3 eigen-solver
-// (eigenvalue.inl:30-178), SqrtMatrix3x3 and Eigen's cofactor 3x3 inverse.
+// (eigenvalue.inl:30-178), SqrtMatrix3x3 and Eigen's cofactor 3x3 inverse; the deterministic acos / cos / atan2
+// (det_acosf, det_cosf, det_atan2f) that iss.cu, fpfh.cu and shot.cu use as well.
 // Translation units including this must be compiled with -fmad=false.
 #pragma once
 #include "cphb_internal.cuh"
@@ -157,6 +158,35 @@ static __device__ float det_acosf(float xf) {  // xf in [-1, 1]
     else if (x < -0.5) r = __dsub_rn(dt::PI, __dmul_rn(2.0, dt::asin_p(sqrt(__dmul_rn(__dadd_rn(1.0, x), 0.5)))));
     else r = __dsub_rn(dt::PI_2, dt::asin_p(x));
     return (float)r;
+}
+// deterministic atan2f (fpfh.cu, shot.cu): float64, IEEE add / mul / div / sqrt only.  atan(t), t >= 0: two half-angle
+// reductions t <- t / (1 + sqrt(1 + t^2)) (atan t = 2 atan of that) bring t below 0.2, then 13 Taylor terms (error < 1e-17).
+__device__ __forceinline__ double dt_atan_pos(double t) {
+    int doubled = 0;
+    for (int k = 0; k < 3; ++k) {
+        if (t > 0.2) {
+            t = __ddiv_rn(t, __dadd_rn(1.0, sqrt(__dadd_rn(1.0, __dmul_rn(t, t)))));
+            ++doubled;
+        }
+    }
+    const double t2 = __dmul_rn(t, t);
+    double p = 1.0 / 25.0;
+#pragma unroll
+    for (int k = 11; k >= 0; --k) p = __dsub_rn(1.0 / (double)(2 * k + 1), __dmul_rn(t2, p));
+    double a = __dmul_rn(t, p);
+    for (int k = 0; k < doubled; ++k) a = __dmul_rn(2.0, a);
+    return a;
+}
+static __device__ float det_atan2f(float yf, float xf) {
+    const double y = (double)yf, x = (double)xf;
+    const double PI = 0x1.921fb54442d18p+1, PI_2 = 0x1.921fb54442d18p+0;
+    if (x == 0.0 && y == 0.0) return copysignf((signbit(xf) ? (float)PI : 0.f), yf);
+    const double ay = fabs(y), ax = fabs(x);
+    double a;  // angle of (ax, ay) in [0, pi/2]
+    if (ay <= ax) a = dt_atan_pos(__ddiv_rn(ay, ax));
+    else a = __dsub_rn(PI_2, dt_atan_pos(__ddiv_rn(ax, ay)));
+    if (x < 0.0) a = __dsub_rn(PI, a);
+    return (float)(signbit(y) ? -a : a);  // atan2(-0, x < 0) = -pi, not +pi
 }
 static __device__ float det_cosf(float yf) {  // yf in [0, 2 pi]
     double y = (double)yf;

@@ -2,43 +2,13 @@
 //   k-NN / radius neighbours of every point (the library's own search) -> SPFH (11 + 11 + 11 bin histogram of the pair
 //   features of a point with each neighbour) -> FPFH (distance-weighted sum of the neighbours' SPFH + the point's own).
 // Arithmetic contract: float32 pair features in the reference's operation order; the three transcendental calls
-// (acos for the frame choice, atan2 for the first angle) are the deterministic float64 routines of cphb_eigen3.cuh /
-// below, rounded once to float32 -- the oracle uses the same specification, so histograms are bit-exact; histogram
+// (acos for the frame choice, atan2 for the first angle) are the deterministic float64 routines of cphb_eigen3.cuh,
+// rounded once to float32 -- the oracle uses the same specification, so histograms are bit-exact; histogram
 // increments are float32 additions in neighbour order (nearest first), exactly as the reference's sequential loops.
 #include <math.h>
 
 #include "cphb_internal.cuh"
 #include "cphb_eigen3.cuh"
-
-// deterministic atan2f: float64, IEEE add / mul / div / sqrt only.  atan(t), t >= 0: two half-angle reductions
-// t <- t / (1 + sqrt(1 + t^2)) (atan t = 2 atan of that) bring t below 0.2, then 13 Taylor terms (error < 1e-17).
-__device__ __forceinline__ double dt_atan_pos(double t) {
-    int doubled = 0;
-    for (int k = 0; k < 3; ++k) {
-        if (t > 0.2) {
-            t = __ddiv_rn(t, __dadd_rn(1.0, sqrt(__dadd_rn(1.0, __dmul_rn(t, t)))));
-            ++doubled;
-        }
-    }
-    const double t2 = __dmul_rn(t, t);
-    double p = 1.0 / 25.0;
-#pragma unroll
-    for (int k = 11; k >= 0; --k) p = __dsub_rn(1.0 / (double)(2 * k + 1), __dmul_rn(t2, p));
-    double a = __dmul_rn(t, p);
-    for (int k = 0; k < doubled; ++k) a = __dmul_rn(2.0, a);
-    return a;
-}
-__device__ float det_atan2f(float yf, float xf) {
-    const double y = (double)yf, x = (double)xf;
-    const double PI = 0x1.921fb54442d18p+1, PI_2 = 0x1.921fb54442d18p+0;
-    if (x == 0.0 && y == 0.0) return copysignf((signbit(xf) ? (float)PI : 0.f), yf);
-    const double ay = fabs(y), ax = fabs(x);
-    double a;  // angle of (ax, ay) in [0, pi/2]
-    if (ay <= ax) a = dt_atan_pos(__ddiv_rn(ay, ax));
-    else a = __dsub_rn(PI_2, dt_atan_pos(__ddiv_rn(ax, ay)));
-    if (x < 0.0) a = __dsub_rn(PI, a);
-    return (float)(signbit(y) ? -a : a);  // atan2(-0, x < 0) = -pi, not +pi
-}
 
 // ComputePairFeatures (fpfh.cu:34-69)
 __device__ void pair_features(const float *p1, const float *n1, const float *p2, const float *n2, float (&f)[4]) {

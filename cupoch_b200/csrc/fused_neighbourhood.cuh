@@ -1,6 +1,6 @@
 // fused_neighbourhood.cuh -- the "k-best search, then a per-point epilogue over the list" form shared by every k-list
-// kernel: search.cu (searchk_kernel, whose epilogue writes the [n][k] table), features.cu (EstimateNormals) and iss.cu
-// (ComputeISSKeypoints).  The warp's k-best search with its lists in shared memory, its one launch rule
+// kernel: search.cu (searchk_kernel, whose epilogue writes the [n][k] table), features.cu (EstimateNormals), iss.cu
+// (ComputeISSKeypoints) and shot.cu (ComputeSHOTFeature, with shared memory of its own per warp: launch_fused_extra).  The warp's k-best search with its lists in shared memory, its one launch rule
 // (launch_fused), the 9 cumulants over a lane's list in list order (geometry_functor.h:35-55) and the covariance
 // E[xx^T] - E[x]E[x]^T formed from them; the fused epilogues write no [n][k] table.
 // Translation units including this must be compiled with -fmad=false.
@@ -96,19 +96,30 @@ __device__ __forceinline__ void list_cumulants(const WarpSearchK &w, int k, unsi
     }
 }
 
-// dynamic shared memory of one warp of a fused kernel with k-slot lists
-static inline size_t fused_smem_per_warp(int k) {
-    return 2 * CPHB_LEAF * sizeof(float4) + 2 * sizeof(uint64_t) + (size_t)k * 32 * sizeof(unsigned long long);
+// dynamic shared memory of one warp of a fused kernel with k-slot lists, plus `extra` bytes of the kernel's own per warp
+// (placed after every warp's lists: fused_warp_extra)
+static inline size_t fused_smem_per_warp(int k, size_t extra = 0) {
+    return 2 * CPHB_LEAF * sizeof(float4) + 2 * sizeof(uint64_t) + (size_t)k * 32 * sizeof(unsigned long long) + extra;
+}
+
+// this warp's `extra` bytes of a kernel launched with launch_fused_extra (16-byte aligned when `extra` is a multiple of 16)
+__device__ __forceinline__ unsigned char *fused_warp_extra(unsigned char *smem, int k, size_t extra) {
+    const size_t nwarp = blockDim.x >> 5;
+    unsigned char *lists_end =
+        smem + nwarp * (2 * CPHB_LEAF * sizeof(float4) + 2 * sizeof(uint64_t) + (size_t)k * 32 * sizeof(unsigned long long));
+    return lists_end + (size_t)(threadIdx.x >> 5) * extra;
 }
 
 // launch of one k-list kernel over `lanes` query lanes (one thread each): as many warps per block as fit in 96 KB of
-// lists and tiles, 1 to 8; the <3> or <5> instance by the index's depth.  The kernel's first argument is the index view.
+// lists, tiles and `extra` bytes per warp, 1 to 8; the <3> or <5> instance by the index's depth.  The kernel's first
+// argument is the index view.
 template <class K3, class K5, class... Args>
-static int launch_fused(const cphb_index *ix, K3 k3, K5 k5, size_t lanes, int k, cudaStream_t s, Args... args) {
-    int warps = (int)((96 * 1024) / fused_smem_per_warp(k));
+static int launch_fused_extra(const cphb_index *ix, K3 k3, K5 k5, size_t lanes, int k, size_t extra, cudaStream_t s,
+                              Args... args) {
+    int warps = (int)((96 * 1024) / fused_smem_per_warp(k, extra));
     if (warps > 8) warps = 8;
     if (warps < 1) warps = 1;
-    const size_t smem = fused_smem_per_warp(k) * warps;
+    const size_t smem = fused_smem_per_warp(k, extra) * warps;
     const unsigned block = warps * 32;
     const unsigned grid = (unsigned)((lanes + block - 1) / block);
     if (ix->v.top <= 3) {
@@ -120,4 +131,8 @@ static int launch_fused(const cphb_index *ix, K3 k3, K5 k5, size_t lanes, int k,
     }
     CPHB_CHECK_LAUNCH();
     return CPHB_OK;
+}
+template <class K3, class K5, class... Args>
+static int launch_fused(const cphb_index *ix, K3 k3, K5 k5, size_t lanes, int k, cudaStream_t s, Args... args) {
+    return launch_fused_extra(ix, k3, k5, lanes, k, 0, s, args...);
 }

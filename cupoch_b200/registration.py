@@ -405,6 +405,34 @@ def compute_fpfh_feature(input, search_param):
     return Feature(out)
 
 
+class FeatureSHOT(Feature):
+    """registration::Feature<352> (feature.h:62-66), the reference binding's FeatureSHOT: `data` is [n, 352] float32 on
+    the device, one row per point."""
+
+
+def compute_shot_feature(input, radius, search_param):
+    """registration::ComputeSHOTFeature (shot.cu:222-255).  `radius` is the descriptor's support; `search_param`
+    (KDTreeSearchParamKNN(knn <= 100) or KDTreeSearchParamRadius(r, max_nn <= 256)) chooses the neighbours, and
+    neighbours beyond `radius` are used as the reference uses them."""
+    from .geometry import KDTreeSearchParamKNN, KDTreeSearchParamRadius
+    _lib.require_gpu()
+    n = len(input)
+    out = DeviceArray((n, 352), np.float32)
+    if isinstance(search_param, KDTreeSearchParamKNN):
+        knn, search_radius, max_nn = int(search_param.knn), 0.0, 0
+    elif isinstance(search_param, KDTreeSearchParamRadius):
+        knn, search_radius, max_nn = 0, float(search_param.radius), int(search_param.max_nn)
+    else:
+        raise RuntimeError("Unsupport search param type.")
+    if n == 0:
+        return FeatureSHOT(out)
+    if not input.has_normals():
+        raise RuntimeError("[ComputeSHOTFeature] Failed because input point cloud has no normal.")
+    _lib.check(_lib.lib().cphb_compute_shot_feature(input._points.ptr, input._normals.ptr, n, float(radius), knn,
+                                                    search_radius, max_nn, out.ptr, None))
+    return FeatureSHOT(out)
+
+
 class IcpContext:
     """Reusable RegistrationICP state (index + Hilbert-ordered source), for repeated runs and
     the per-step test hook.  Thin wrapper over cphb_icp_create / _run / _step."""

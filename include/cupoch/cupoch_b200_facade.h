@@ -1097,5 +1097,36 @@ inline std::shared_ptr<Feature<33>> ComputeFPFHFeature(const geometry::PointClou
                                                  max_nn, feature->data_.data(), nullptr));
     return feature;
 }
+/// registration::ComputeSHOTFeature (feature.h:62-66, shot.cu:222-255): one row of 352 floats per point.  `radius` is
+/// the descriptor's support, independent of the search.  Missing normals, knn > 100 or max_nn outside [0, 256] are
+/// logged and leave the rows unset.
+inline std::shared_ptr<Feature<352>> ComputeSHOTFeature(const geometry::PointCloud &input, float radius,
+                                                        const knn::KDTreeSearchParam &search_param) {
+    auto feature = std::make_shared<Feature<352>>();
+    feature->Resize((int)input.points_.size());
+    int knn = 0, max_nn = 0;
+    float search_radius = 0.f;
+    switch (search_param.GetSearchType()) {
+        case knn::KDTreeSearchParam::SearchType::Knn: knn = ((const knn::KDTreeSearchParamKNN &)search_param).knn_; break;
+        case knn::KDTreeSearchParam::SearchType::Radius:
+            search_radius = ((const knn::KDTreeSearchParamRadius &)search_param).radius_;
+            max_nn = ((const knn::KDTreeSearchParamRadius &)search_param).max_nn_;
+            break;
+        default: utility::LogError("Unsupport search param type."); return feature;
+    }
+    if (input.points_.empty()) return feature;
+    if (!input.HasNormals()) {
+        utility::LogError("[ComputeSHOTFeature] Failed because input point cloud has no normal.");
+        return feature;
+    }
+    if (knn > knn::NUM_MAX_NN || (knn <= 0 && (max_nn < 0 || max_nn > 256))) {
+        utility::LogError("[ComputeSHOTFeature] knn must be <= 100 and max_nn must lie in [0, 256].");
+        return feature;
+    }
+    utility::check(cphb_compute_shot_feature(reinterpret_cast<const float *>(input.points_.data()),
+                                             reinterpret_cast<const float *>(input.normals_.data()), input.points_.size(),
+                                             radius, knn, search_radius, max_nn, feature->data_.data(), nullptr));
+    return feature;
+}
 }  // namespace registration
 }  // namespace cupoch

@@ -348,6 +348,15 @@ int cphb_compute_weighted_jtj_jtr(const float *J, const float *r, size_t n, int 
 int cphb_compute_fpfh_feature(const float *points, const float *normals, size_t n, int knn, float radius,
                               int max_nn, float *out_features, void *stream);
 
+/* registration::ComputeSHOTFeature(input, radius, search_param) (feature.h:62-66, shot.cu:222-255):
+   knn > 0 -> KDTreeSearchParamKNN(knn), else KDTreeSearchParamRadius(search_radius, max_nn).
+   out_features [n][352] float32, one row per point.  `radius` is the descriptor's support (frame weights radius - d,
+   shells at radius / 4, / 2, * 3 / 4), independent of the search.  Normals are required; a point's row is all zero
+   when fewer than 5 other points are listed.  knn <= 100 and 0 <= max_nn <= 256, else CPHB_ERR_INVALID; n == 0 is a
+   no-op.  One index serves one fused kernel; no [n][k] table is built.  Synchronises. */
+int cphb_compute_shot_feature(const float *points, const float *normals, size_t n, float radius,
+                              int knn, float search_radius, int max_nn, float *out_features, void *stream);
+
 /* geometry::PointCloud::ClusterDBSCAN(eps, min_points, print_progress, max_edges) (pointcloud.h:195-199,
  * pointcloud_cluster.cu:84-179): labels_out (device, n int32), -1 = noise; *h_n_clusters (optional) = cluster ids
  * handed out.  max_edges in [1, 255] (reference default NUM_MAX_NN = 100). */

@@ -30,6 +30,9 @@ def main():
                     help="instead: time PointCloud::FarthestPointDownSample at N = 100 k, 1 M, 10 M and 1024, 8192 samples")
     ap.add_argument("--iss", action="store_true",
                     help="instead: time geometry::keypoint::ComputeISSKeypoints (defaults, automatic radii) at N = 1 M, 10 M")
+    ap.add_argument("--shot", action="store_true",
+                    help="instead: time registration::ComputeSHOTFeature (Radius(r, 100), r = 5 spacings) at N = 100 k, 1 M")
+    ap.add_argument("--out", default=None, help="--shot: also write the JSON object to this file")
     ap.add_argument("--edt", action="store_true",
                     help="instead: time geometry::DistanceTransform::ComputeEDT at 256^3 and 512^3 and GetDistances of 10 M points")
     args = ap.parse_args()
@@ -41,6 +44,8 @@ def main():
         return fps(args.reps)
     if args.iss:
         return iss(args.reps)
+    if args.shot:
+        return shot(args.reps, args.out)
     import cupoch_b200 as cph
     from cupoch_b200 import _lib
     from cupoch_b200.testing import datagen
@@ -420,6 +425,83 @@ def iss(reps):
                      "speedup_vs_reference_shaped": t_med / med})
     print(json.dumps({"op": "geometry::keypoint::ComputeISSKeypoints(defaults) on datagen.surface(N, 11)", "gpu": gpu,
                       "reps": reps, "launches": int(L.cphb_launch_count()), "rows": rows}))
+
+
+SHOT_PHASES = (("shot_kernel", ("shot_kernel",)),)
+
+
+def shot(reps, out=None):
+    """compute_shot_feature(pc, r, KDTreeSearchParamRadius(r, 100)) with r = 5 x the point spacing on datagen.surface(N,
+    11) over a sqrt(N / 1e5)-wide square (1e5 points per unit square); normals from EstimateNormals(KNN 30), not timed.
+    CUDA-event time of the whole Python call after a warm-up call, and per-kernel times from torch.profiler in a separate
+    profiled call (shot_kernel; the rest is the index build).  Comparison arm: the library's own search_radius writing
+    the [n][100] index and distance tables the reference materialises before its descriptor pass (shot.cu:229-245),
+    index build included, timed by CUDA events -- a lower bound on the reference's first stage only.  The reference
+    binary itself is not run here."""
+    import subprocess
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    import cupoch_b200 as cph
+    from cupoch_b200 import _lib
+    from cupoch_b200.testing import datagen
+    L = _lib.lib()
+    gpu = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                         capture_output=True, text=True).stdout.strip()
+    ev = [L.cphb_event_create() for _ in range(2)]
+
+    def timed(fn):
+        times = []
+        for r in range(reps + 1):  # the first call warms the allocation pool and the modules
+            L.cphb_event_record(ev[0], None)
+            fn()
+            L.cphb_event_record(ev[1], None)
+            ms = C.c_float(0)
+            _lib.check(L.cphb_event_elapsed_ms(ev[0], ev[1], C.byref(ms)))
+            if r:
+                times.append(ms.value)
+        return times
+
+    rows = []
+    for n in (100_000, 1_000_000):
+        pts = datagen.surface(n, 11, extent=float(np.sqrt(n / 1e5)))[0]
+        pc = cph.geometry.PointCloud(pts)
+        pc.estimate_normals(cph.geometry.KDTreeSearchParamKNN(30))
+        r = float(np.float32(5.0 / np.sqrt(1e5)))
+        param = cph.geometry.KDTreeSearchParamRadius(r, 100)
+        calls = timed(lambda: cph.registration.compute_shot_feature(pc, r, param))
+        f = cph.registration.compute_shot_feature(pc, r, param).cpu()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            cph.registration.compute_shot_feature(pc, r, param)
+            torch.cuda.synchronize()
+        phase_ms = {"shot_kernel": 0.0, "index_build": 0.0}
+        for e in prof.key_averages():
+            t = getattr(e, "device_time_total", getattr(e, "cuda_time_total", 0.0)) * 1e-3
+            if t <= 0 or "Memset" in e.key or "Memcpy" in e.key:
+                continue
+            phase_ms["shot_kernel" if "shot_kernel" in e.key else "index_build"] += t
+
+        def tables():
+            tree = cph.geometry.KDTreeFlann(pc)
+            return tree.search_radius(pc.points, r, 100)
+
+        table_calls = timed(tables)
+        listed = int(tables()[0])  # the number of (point, neighbour) slots filled
+        med = float(np.median(calls))
+        rows.append({"n": n, "radius": r, "mean_listed_neighbours": listed / n,
+                     "nonzero_rows": int((np.abs(f).sum(1) > 0).sum()),
+                     "call_ms_median": med, "call_ms_min": float(np.min(calls)), "phase_ms_profiled": phase_ms,
+                     "descriptor_bytes_written": int(n * 352 * 4),
+                     "tables_not_written_bytes": int(n * 100 * (4 + 4)),
+                     "reference_first_stage_tables": {"ms_median": float(np.median(table_calls)),
+                                                      "ms_min": float(np.min(table_calls))},
+                     "speedup_vs_cupoch": "not measured"})
+        torch.cuda.empty_cache()
+    res = {"op": "registration::ComputeSHOTFeature(pc, r, KDTreeSearchParamRadius(r, 100)), r = 5 spacings, on "
+                 "datagen.surface(N, 11) at 1e5 points per unit square", "gpu": gpu, "reps": reps, "rows": rows}
+    print(json.dumps(res))
+    if out:
+        with open(out, "w") as fh:
+            json.dump(res, fh)
 
 
 HBM_BYTES_PER_S = 3.35e12  # H100 SXM data sheet

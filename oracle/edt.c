@@ -1,7 +1,7 @@
 /*
  * edt.c -- CPU restatement of cupoch's geometry::DistanceTransform (geometry/distancetransform.cu) as the product
  * defines it (DESIGN.md section 4, parity hazard 13).  TEST INFRASTRUCTURE ONLY, like oracle.c: loaded by tests/ and
- * tools/bench_ops.py through edt_py.py, never by the product.  Built by edt_py.build() with oracle/Makefile's flags
+ * tools/bench_ops.py through edt_py.py, never by the product.  Built by oracle.build() (oracle/__init__.py)
  * (-ffp-contract=off, no -ffast-math, OpenMP).
  *
  * The transform is separable: along z the nearest site of each row, along y then x the lower envelope of the

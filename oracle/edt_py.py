@@ -1,35 +1,19 @@
 """ctypes loader for the DistanceTransform restatement (oracle/edt.c).
 
 TEST INFRASTRUCTURE ONLY, like oracle_py: imported by tests/ and tools/bench_ops.py --edt, never by the product package
-cupoch_b200/.  The library is compiled on first use with oracle/Makefile's flags into oracle/_build/ (or a per-user
-temporary directory when the tree is read-only).
+cupoch_b200/.  The library is built by oracle.build() (oracle/__init__.py).
 """
 import ctypes as C
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SRC = os.path.join(_HERE, "edt.c")
-CFLAGS = ["-O2", "-fPIC", "-ffp-contract=off", "-fno-fast-math", "-mfma", "-Wall", "-Wextra", "-Wno-unused-parameter",
-          "-Wno-unknown-pragmas"]
+from . import build as _build, load, ptr as _p
+
 NOT_SITE = 2  # DistanceVoxel::NotSite
 
 
 def build(force=False):
-    out_dir = os.path.join(_HERE, "_build")
-    if not os.access(_HERE, os.W_OK) and not os.access(out_dir, os.W_OK):
-        out_dir = os.path.join(tempfile.gettempdir(), "cphb_oracle_%d" % os.getuid())
-    so = os.path.join(out_dir, "libedt.so")
-    if force or not os.path.exists(so) or os.path.getmtime(so) < os.path.getmtime(_SRC):
-        os.makedirs(out_dir, exist_ok=True)
-        cmd = [os.environ.get("CC", "gcc")] + CFLAGS + ["-shared", "-o", so, _SRC, "-lm"]
-        # OpenMP only parallelises over lines (each line's result is computed alone): single-threaded if unavailable
-        if subprocess.run(cmd[:1] + ["-fopenmp"] + cmd[1:], capture_output=True).returncode != 0:
-            subprocess.check_call(cmd)
-    return so
+    return _build("edt", force)
 
 
 _lib = None
@@ -38,16 +22,12 @@ _lib = None
 def lib():
     global _lib
     if _lib is None:
-        _lib = C.CDLL(build())
+        _lib = load("edt")
         _lib.orc_dt_voxel_size_ok.restype = C.c_int
         _lib.orc_dt_voxel_size_ok.argtypes = [C.c_float, C.c_float]
         for f in ("orc_dt_key_cells", "orc_dt_compute", "orc_dt_distance_index", "orc_dt_voxel_index"):
             getattr(_lib, f).restype = None
     return _lib
-
-
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p)
 
 
 def _f3(v):

@@ -1,7 +1,7 @@
 /*
  * fps.c -- CPU restatement of cupoch's PointCloud::FarthestPointDownSample (geometry/pointcloud.cu:122-139,301-338).
  * TEST INFRASTRUCTURE ONLY, like oracle.c: loaded by tests/ and tools/bench_ops.py through fps_py.py, never by the
- * product.  Built by fps_py.build() with oracle/Makefile's flags: -ffp-contract=off (no implicit FMA; the squared
+ * product.  Built by oracle.build() (oracle/__init__.py): -ffp-contract=off (no implicit FMA; the squared
  * distance's fused multiply-adds are explicit) and no -ffast-math.
  */
 #include <math.h>

@@ -1,7 +1,7 @@
 /*
  * iss.c -- CPU restatement of cupoch's geometry::keypoint::ComputeISSKeypoints (geometry/iss_keypoints.cu:37-172).
  * TEST INFRASTRUCTURE ONLY, like oracle.c: loaded by tests/ and tools/bench_ops.py through iss_py.py, never by the
- * product.  Built by iss_py.build() with oracle/Makefile's flags (-ffp-contract=off, no -ffast-math, OpenMP).
+ * product.  Built by oracle.build() (oracle/__init__.py): -ffp-contract=off, no -ffast-math, OpenMP.
  *
  * oracle.c is compiled into this translation unit (the #include below), so the kd-tree search with its result set and
  * tie rule (kd_search_rec, rset_*) and the FastEigen3x3 restatement (fast_eigen3x3, static there) are the oracle's

@@ -1,8 +1,8 @@
 /*
  * oracle.c -- CPU restatement of cupoch's ICP / kNN / voxel-grid hot path.
- * TEST INFRASTRUCTURE ONLY (see oracle.h).  Build: make -C oracle
- * Compile flags matter: -ffp-contract=off (no implicit FMA; every fused
- * multiply-add below is an explicit fmaf) and no -ffast-math.
+ * TEST INFRASTRUCTURE ONLY (see oracle.h).  Built by oracle.build()
+ * (oracle/__init__.py).  Compile flags matter: -ffp-contract=off (no implicit
+ * FMA; every fused multiply-add below is an explicit fmaf) and no -ffast-math.
  *
  * Arithmetic conventions (shared with the CUDA product by specification, not
  * by code):

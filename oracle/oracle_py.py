@@ -2,24 +2,20 @@
 
 TEST INFRASTRUCTURE ONLY: imported by tests/, __graft_entry__.smoke() and
 bench.py's cpu_baseline / --impl reference legs.  The product package
-cupoch_b200/ must never import this module.
+cupoch_b200/ must never import this module.  The library is built by
+oracle.build() (oracle/__init__.py).
 """
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SO = os.path.join(_HERE, "_build", "liboracle.so")
+from . import build as _build, load, ptr as _p
 
 P2P, P2PLANE, SYMMETRIC, COLORED, GICP = 1, 2, 3, 4, 5
 
 
 def build(force=False):
-    if force or not os.path.exists(_SO) or os.path.getmtime(_SO) < os.path.getmtime(os.path.join(_HERE, "oracle.c")):
-        subprocess.check_call(["make", "-C", _HERE, "-s"])
-    return _SO
+    return _build("oracle", force)
 
 
 class IcpResult(C.Structure):
@@ -39,9 +35,7 @@ _lib = None
 def lib():
     global _lib
     if _lib is None:
-        if not os.path.exists(_SO):
-            build()
-        _lib = C.CDLL(_SO)
+        _lib = load("oracle")
         _lib.orc_search_bruteforce.restype = C.c_long
         _lib.orc_kdtree_build.restype = C.c_void_p
         _lib.orc_kdtree_search.restype = C.c_long
@@ -52,10 +46,6 @@ def lib():
 
 def _f(a):
     return None if a is None else np.ascontiguousarray(a, dtype=np.float32)
-
-
-def _p(a):
-    return None if a is None else a.ctypes.data_as(C.c_void_p)
 
 
 def search(tgt, qry, k, radius=-1.0, kdtree=False):

@@ -1,7 +1,7 @@
 /*
  * segment_plane.c -- CPU restatement of cupoch's PointCloud::SegmentPlane (geometry/segmentation.cu:36-267).
  * TEST INFRASTRUCTURE ONLY, like oracle.c: loaded by tests/ and tools/bench_ops.py through segment_plane_py.py,
- * never by the product.  Built by segment_plane_py.build() with oracle/Makefile's flags: -ffp-contract=off (no
+ * never by the product.  Built by oracle.build() (oracle/__init__.py): -ffp-contract=off (no
  * implicit FMA; the one fused multiply-add, dot3f, is explicit) and no -ffast-math.
  */
 #include <math.h>

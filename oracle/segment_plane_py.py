@@ -1,44 +1,21 @@
 """ctypes loader for the SegmentPlane restatement (oracle/segment_plane.c).
 
 TEST INFRASTRUCTURE ONLY, like oracle_py: imported by tests/ and tools/bench_ops.py --segment-plane, never by the
-product package cupoch_b200/.  The library is compiled on first use with oracle/Makefile's flags into oracle/_build/
-(or a per-user temporary directory when the tree is read-only).
+product package cupoch_b200/.  The library is built by oracle.build() (oracle/__init__.py).
 """
 import ctypes as C
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SRC = os.path.join(_HERE, "segment_plane.c")
-CFLAGS = ["-O2", "-fPIC", "-ffp-contract=off", "-fno-fast-math", "-mfma", "-Wall", "-Wextra"]
+from . import build as _build, load, ptr as _p
 
 
 def build(force=False):
-    out_dir = os.path.join(_HERE, "_build")
-    if not os.access(_HERE, os.W_OK) and not os.access(out_dir, os.W_OK):
-        out_dir = os.path.join(tempfile.gettempdir(), "cphb_oracle_%d" % os.getuid())
-    so = os.path.join(out_dir, "libsegment_plane.so")
-    if force or not os.path.exists(so) or os.path.getmtime(so) < os.path.getmtime(_SRC):
-        os.makedirs(out_dir, exist_ok=True)
-        subprocess.check_call([os.environ.get("CC", "gcc")] + CFLAGS + ["-shared", "-o", so, _SRC, "-lm"])
-    return so
-
-
-_lib = None
+    return _build("segment_plane", force)
 
 
 def lib():
-    global _lib
-    if _lib is None:
-        _lib = C.CDLL(build())
-    return _lib
-
-
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p)
+    return load("segment_plane")
 
 
 def segment_plane(pts, distance_threshold, ransac_n, seeds):

@@ -1,7 +1,7 @@
 /*
  * shot.c -- CPU restatement of cupoch's registration::ComputeSHOTFeature (registration/shot.cu:33-255).
  * TEST INFRASTRUCTURE ONLY, like oracle.c: loaded by tests/ and tools/bench_ops.py through shot_py.py, never by the
- * product.  Built by shot_py.build() with oracle/Makefile's flags (-ffp-contract=off, no -ffast-math, OpenMP).
+ * product.  Built by oracle.build() (oracle/__init__.py): -ffp-contract=off, no -ffast-math, OpenMP.
  *
  * oracle.c is compiled into this translation unit (the #include below), so the kd-tree search with its result set and
  * tie rule (kd_search_rec, rset_*), the FastEigen3x3 restatement (fast_eigen3x3) and the deterministic det_acosf /

@@ -12,31 +12,9 @@
 
 #include "cupoch/geometry/distancetransform.h"
 #include "cupoch/geometry/voxelgrid.h"
+#include "facade_check.h"
 
 using namespace cupoch;
-
-static int fails = 0;
-#define EXPECT(cond)                                                          \
-    do {                                                                      \
-        if (!(cond)) { std::printf("FAILED %s:%d: %s\n", __FILE__, __LINE__, #cond); ++fails; } \
-    } while (0)
-
-template <class T>
-static std::vector<T> read_all(const std::string &path) {
-    std::vector<T> v;
-    std::FILE *f = std::fopen(path.c_str(), "rb");
-    if (!f) return v;
-    T x;
-    while (std::fread(&x, sizeof(T), 1, f) == 1) v.push_back(x);
-    std::fclose(f);
-    return v;
-}
-
-static void write_bytes(const std::string &path, const void *p, size_t bytes) {
-    std::FILE *f = std::fopen(path.c_str(), "wb");
-    std::fwrite(p, 1, bytes, f);
-    std::fclose(f);
-}
 
 static bool throws_for(size_t res) {
     try {
@@ -50,9 +28,9 @@ static bool throws_for(size_t res) {
 int main(int argc, char **argv) {
     if (argc != 2) return 0;  // compile-and-link check only
     const std::string dir = argv[1];
-    const std::vector<float> prm = read_all<float>(dir + "/params.f32");
-    const std::vector<int32_t> c = read_all<int32_t>(dir + "/cells.i32");
-    const std::vector<float> q = read_all<float>(dir + "/queries.f32");
+    const std::vector<float> prm = read_file<float>(dir + "/params.f32");
+    const std::vector<int32_t> c = read_file<int32_t>(dir + "/cells.i32");
+    const std::vector<Eigen::Vector3f> queries = rows3(read_file<float>(dir + "/queries.f32"));
     if (prm.size() != 5) return 2;
     EXPECT(throws_for(0) && throws_for(1025));
 
@@ -66,12 +44,10 @@ int main(int argc, char **argv) {
     other.voxels_keys_ = std::vector<Eigen::Vector3i>(1, Eigen::Vector3i(0, 0, 0));
     dt.ComputeEDT(other);
 
-    std::vector<Eigen::Vector3f> queries;
-    for (size_t i = 0; i + 2 < q.size(); i += 3) queries.push_back(Eigen::Vector3f(q[i], q[i + 1], q[i + 2]));
     const std::vector<float> d = dt.GetDistances(utility::device_vector<Eigen::Vector3f>(queries))->to_host();
     EXPECT(d.size() == queries.size());
     if (!queries.empty()) EXPECT(dt.GetDistance(queries[0]) == d[0]);
-    write_bytes(dir + "/out_dist.f32", d.data(), d.size() * sizeof(float));
+    write_file(dir + "/out_dist.f32", d.data(), d.size() * sizeof(float));
 
     std::vector<int32_t> vox;
     for (const auto &p : queries) {
@@ -82,7 +58,7 @@ int main(int argc, char **argv) {
         std::memcpy(&bits, &v.distance_, 4);
         vox.insert(vox.end(), {std::get<0>(r) ? 1 : 0, v.nearest_index_[0], v.nearest_index_[1], v.nearest_index_[2], (int32_t)v.state_, bits});
     }
-    write_bytes(dir + "/out_voxel.i32", vox.data(), vox.size() * sizeof(int32_t));
+    write_file(dir + "/out_voxel.i32", vox.data(), vox.size() * sizeof(int32_t));
     if (fails) return 1;
     std::printf("facade DistanceTransform: all expectations met\n");
     return 0;

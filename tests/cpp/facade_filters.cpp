@@ -12,14 +12,9 @@
 
 #include "cupoch/geometry/pointcloud.h"
 #include "cupoch/geometry/voxelgrid.h"
+#include "facade_check.h"
 
 using namespace cupoch;
-
-static int fails = 0;
-#define EXPECT(cond)                                                          \
-    do {                                                                      \
-        if (!(cond)) { std::printf("FAILED %s:%d: %s\n", __FILE__, __LINE__, #cond); ++fails; } \
-    } while (0)
 
 int main() {
     {   // RemoveRadiusOutliers

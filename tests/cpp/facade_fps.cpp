@@ -10,35 +10,11 @@
 #include <vector>
 
 #include "cupoch/geometry/pointcloud.h"
+#include "facade_check.h"
 
 using namespace cupoch;
 
-static int fails = 0;
-#define EXPECT(cond)                                                          \
-    do {                                                                      \
-        if (!(cond)) { std::printf("FAILED %s:%d: %s\n", __FILE__, __LINE__, #cond); ++fails; } \
-    } while (0)
-
-static std::vector<Eigen::Vector3f> read_rows(const std::string &path) {
-    std::vector<Eigen::Vector3f> rows;
-    std::FILE *f = std::fopen(path.c_str(), "rb");
-    if (!f) return rows;
-    float v[3];
-    while (std::fread(v, sizeof(float), 3, f) == 3) rows.push_back(Eigen::Vector3f(v[0], v[1], v[2]));
-    std::fclose(f);
-    return rows;
-}
-
 static bool same(const Eigen::Vector3f &a, const Eigen::Vector3f &b) { return a[0] == b[0] && a[1] == b[1] && a[2] == b[2]; }
-
-static void write_rows(const std::string &path, const std::vector<Eigen::Vector3f> &rows) {
-    std::FILE *f = std::fopen(path.c_str(), "wb");
-    for (const auto &r : rows) {
-        const float v[3] = {r[0], r[1], r[2]};
-        std::fwrite(v, sizeof(float), 3, f);
-    }
-    std::fclose(f);
-}
 
 int main(int argc, char **argv) {
     {
@@ -58,12 +34,13 @@ int main(int argc, char **argv) {
     }
     if (argc == 3) {
         const std::string dir = argv[1];
-        geometry::PointCloud pcd(read_rows(dir + "/points.f32"));
-        pcd.SetNormals(read_rows(dir + "/normals.f32"));
+        geometry::PointCloud pcd(rows3(read_file<float>(dir + "/points.f32")));
+        pcd.SetNormals(rows3(read_file<float>(dir + "/normals.f32")));
         if (pcd.IsEmpty() || !pcd.HasNormals()) return 2;
         auto out = pcd.FarthestPointDownSample((size_t)std::atol(argv[2]));
-        write_rows(dir + "/out_points.f32", out->GetPoints());
-        write_rows(dir + "/out_normals.f32", out->GetNormals());
+        const std::vector<float> p = rows3(out->GetPoints()), n = rows3(out->GetNormals());
+        write_file(dir + "/out_points.f32", p.data(), p.size() * sizeof(float));
+        write_file(dir + "/out_normals.f32", n.data(), n.size() * sizeof(float));
     }
     if (fails) return 1;
     std::printf("facade FarthestPointDownSample: all expectations met\n");

@@ -9,36 +9,9 @@
 
 #include "cupoch/geometry/keypoint.h"
 #include "cupoch/geometry/pointcloud.h"
+#include "facade_check.h"
 
 using namespace cupoch;
-
-static int fails = 0;
-#define EXPECT(cond)                                                          \
-    do {                                                                      \
-        if (!(cond)) { std::printf("FAILED %s:%d: %s\n", __FILE__, __LINE__, #cond); ++fails; } \
-    } while (0)
-
-static std::vector<Eigen::Vector3f> read_rows(const std::string &path) {
-    std::vector<Eigen::Vector3f> rows;
-    std::FILE *f = std::fopen(path.c_str(), "rb");
-    if (!f) return rows;
-    float v[3];
-    while (std::fread(v, sizeof(float), 3, f) == 3) rows.push_back(Eigen::Vector3f(v[0], v[1], v[2]));
-    std::fclose(f);
-    return rows;
-}
-
-static void write_bytes(const std::string &path, const void *p, size_t bytes) {
-    std::FILE *f = std::fopen(path.c_str(), "wb");
-    std::fwrite(p, 1, bytes, f);
-    std::fclose(f);
-}
-
-static void write_rows(const std::string &path, const std::vector<Eigen::Vector3f> &rows) {
-    std::vector<float> flat;
-    for (const auto &r : rows) flat.insert(flat.end(), {r[0], r[1], r[2]});
-    write_bytes(path, flat.data(), flat.size() * sizeof(float));
-}
 
 int main(int argc, char **argv) {
     {
@@ -48,8 +21,8 @@ int main(int argc, char **argv) {
     }
     if (argc == 2) {
         const std::string dir = argv[1];
-        geometry::PointCloud pcd(read_rows(dir + "/points.f32"));
-        pcd.SetNormals(read_rows(dir + "/normals.f32"));
+        geometry::PointCloud pcd(rows3(read_file<float>(dir + "/points.f32")));
+        pcd.SetNormals(rows3(read_file<float>(dir + "/normals.f32")));
         if (pcd.IsEmpty() || !pcd.HasNormals()) return 2;
         auto bad = geometry::keypoint::ComputeISSKeypoints(pcd, 0.f, 0.f, 0.975f, 0.975f, 5, 257);
         EXPECT(std::get<0>(bad)->IsEmpty() && std::get<1>(bad)->empty());
@@ -62,9 +35,10 @@ int main(int argc, char **argv) {
         size_t m = 0;
         for (unsigned char b : h) m += b;
         EXPECT(m == out.points_.size() && out.HasNormals());
-        write_rows(dir + "/out_points.f32", out.GetPoints());
-        write_rows(dir + "/out_normals.f32", out.GetNormals());
-        write_bytes(dir + "/out_mask.u8", h.data(), h.size());
+        const std::vector<float> p = rows3(out.GetPoints()), n = rows3(out.GetNormals());
+        write_file(dir + "/out_points.f32", p.data(), p.size() * sizeof(float));
+        write_file(dir + "/out_normals.f32", n.data(), n.size() * sizeof(float));
+        write_file(dir + "/out_mask.u8", h.data(), h.size());
     }
     if (fails) return 1;
     std::printf("facade ComputeISSKeypoints: all expectations met\n");

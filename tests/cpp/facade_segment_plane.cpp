@@ -10,14 +10,9 @@
 #include <vector>
 
 #include "cupoch/geometry/pointcloud.h"
+#include "facade_check.h"
 
 using namespace cupoch;
-
-static int fails = 0;
-#define EXPECT(cond)                                                          \
-    do {                                                                      \
-        if (!(cond)) { std::printf("FAILED %s:%d: %s\n", __FILE__, __LINE__, #cond); ++fails; } \
-    } while (0)
 
 int main(int argc, char **argv) {
     {   // SegmentPlaneKnownPlane
@@ -44,12 +39,8 @@ int main(int argc, char **argv) {
     }
     if (argc == 5) {
         const std::string dir = argv[1];
-        std::FILE *f = std::fopen((dir + "/points.f32").c_str(), "rb");
-        if (!f) return 2;
-        std::vector<Eigen::Vector3f> pts;
-        float v[3];
-        while (std::fread(v, sizeof(float), 3, f) == 3) pts.push_back(Eigen::Vector3f(v[0], v[1], v[2]));
-        std::fclose(f);
+        const std::vector<Eigen::Vector3f> pts = rows3(read_file<float>(dir + "/points.f32"));
+        if (pts.empty()) return 2;
         geometry::PointCloud pcd(pts);
         std::srand((unsigned)std::atoi(argv[2]));
         Eigen::Vector4f plane;
@@ -58,12 +49,8 @@ int main(int argc, char **argv) {
         float h[4] = {plane[0], plane[1], plane[2], plane[3]};
         std::vector<size_t> idx = inliers.to_host();
         std::vector<long long> out(idx.begin(), idx.end());
-        f = std::fopen((dir + "/plane.f32").c_str(), "wb");
-        std::fwrite(h, sizeof(float), 4, f);
-        std::fclose(f);
-        f = std::fopen((dir + "/inliers.i64").c_str(), "wb");
-        if (!out.empty()) std::fwrite(out.data(), sizeof(long long), out.size(), f);
-        std::fclose(f);
+        write_file(dir + "/plane.f32", h, sizeof(h));
+        write_file(dir + "/inliers.i64", out.data(), out.size() * sizeof(long long));
     }
     if (fails) return 1;
     std::printf("facade SegmentPlane: all expectations met\n");

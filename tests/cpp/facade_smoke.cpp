@@ -2,33 +2,15 @@
 // cupoch's own examples/tests do (examples/cpp/registration.cpp:42-47, tests/knn/kdtree_flann.cpp).
 // usage: facade_smoke <dir>   reads src.f32 tgt.f32 tgt_nrm.f32 (n x 3 float32), writes results.
 #include <cstdio>
-#include <cstdlib>
 #include <string>
 #include <vector>
 
 #include "cupoch/geometry/pointcloud.h"
 #include "cupoch/knn/kdtree_flann.h"
 #include "cupoch/registration/registration.h"
+#include "facade_check.h"
 
 using namespace cupoch;
-
-static std::vector<Eigen::Vector3f> load(const std::string &path) {
-    FILE *f = fopen(path.c_str(), "rb");
-    if (!f) { fprintf(stderr, "cannot open %s\n", path.c_str()); exit(2); }
-    fseek(f, 0, SEEK_END);
-    long bytes = ftell(f);
-    fseek(f, 0, SEEK_SET);
-    std::vector<Eigen::Vector3f> v(bytes / 12);
-    if (fread(v.data(), 12, v.size(), f) != v.size()) exit(2);
-    fclose(f);
-    return v;
-}
-template <class T>
-static void save(const std::string &path, const T *p, size_t bytes) {
-    FILE *f = fopen(path.c_str(), "wb");
-    fwrite(p, 1, bytes, f);
-    fclose(f);
-}
 
 // a user-defined estimator: forces the generic (virtual-dispatch) loop, delegating to point-to-plane
 class MyEstimation : public registration::TransformationEstimation {
@@ -52,8 +34,14 @@ private:
 int main(int argc, char **argv) {
     if (argc < 2) return 2;
     const std::string dir = argv[1];
-    geometry::PointCloud source(load(dir + "/src.f32")), target(load(dir + "/tgt.f32"));
-    target.SetNormals(load(dir + "/tgt_nrm.f32"));
+    const auto src = rows3(read_file<float>(dir + "/src.f32")), tgt = rows3(read_file<float>(dir + "/tgt.f32")),
+               tgt_nrm = rows3(read_file<float>(dir + "/tgt_nrm.f32"));
+    if (src.empty() || tgt.empty() || tgt_nrm.empty()) {
+        fprintf(stderr, "missing or empty input in %s\n", dir.c_str());
+        return 2;
+    }
+    geometry::PointCloud source(src), target(tgt);
+    target.SetNormals(tgt_nrm);
 
     // KDTreeFlann::SearchRadius / SearchKNN on device vectors
     knn::KDTreeFlann tree(target.points_);
@@ -61,7 +49,7 @@ int main(int argc, char **argv) {
     utility::device_vector<float> d2;
     int k = tree.SearchRadius(source.points_, 0.03f, 1, idx, d2);
     auto hidx = idx.to_host();
-    save(dir + "/radius_idx.i32", hidx.data(), hidx.size() * 4);
+    write_file(dir + "/radius_idx.i32", hidx.data(), hidx.size() * 4);
     std::vector<int> hi;
     std::vector<float> hd;
     int k1 = tree.SearchKNN(source.GetPoints()[0], 5, hi, hd);
@@ -76,11 +64,11 @@ int main(int argc, char **argv) {
     float T[32];
     utility::to_row_major(fused.transformation_, T);
     utility::to_row_major(generic.transformation_, T + 16);
-    save(dir + "/T.f32", T, sizeof(T));
+    write_file(dir + "/T.f32", T, sizeof(T));
     auto corr = fused.GetCorrespondenceSet();
-    save(dir + "/corr.i32", corr.data(), corr.size() * 8);
+    write_file(dir + "/corr.i32", corr.data(), corr.size() * 8);
     float fr[4] = {fused.fitness_, fused.inlier_rmse_, generic.fitness_, generic.inlier_rmse_};
-    save(dir + "/fit.f32", fr, sizeof(fr));
+    write_file(dir + "/fit.f32", fr, sizeof(fr));
     printf("icp: fitness %.4f rmse %.6f corr %zu | generic calls %d fitness %.4f\n", fused.fitness_, fused.inlier_rmse_,
            corr.size(), mine.calls, generic.fitness_);
 

@@ -8,23 +8,11 @@ import tempfile
 import numpy as np
 import pytest
 
-from conftest import ROOT
-
-
-def build_facade():
-    import __graft_entry__
-    __graft_entry__.build()
-    from test_facade_cpp import build_dir
-    exe = os.path.join(build_dir(), "facade_edt")
-    lib = os.path.join(ROOT, "cupoch_b200", "lib")
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-Wall", "-I" + os.path.join(ROOT, "include"),
-                           os.path.join(ROOT, "tests", "cpp", "facade_edt.cpp"), "-o", exe, "-L" + lib,
-                           "-lcupoch_b200", "-Wl,-rpath," + lib])
-    return exe
+from test_facade_cpp import build_facade
 
 
 def test_facade_edt_compiles_and_links():
-    exe = build_facade()
+    exe = build_facade("facade_edt")
     out = subprocess.run(["ldd", exe], capture_output=True, text=True).stdout
     assert "libcupoch_b200.so" in out and "not found" not in out
 
@@ -32,7 +20,7 @@ def test_facade_edt_compiles_and_links():
 @pytest.mark.gpu
 def test_facade_edt_matches_oracle():
     from oracle import edt_py
-    exe = build_facade()
+    exe = build_facade("facade_edt")
     r, vs, origin = 40, 0.25, np.array([0.5, -1.0, 2.0], np.float32)
     rng = np.random.default_rng(5)
     cells = rng.integers(-3, r + 3, (300, 3)).astype(np.int32)  # some outside the grid

@@ -7,8 +7,8 @@ import tempfile
 import numpy as np
 import pytest
 
-from conftest import ROOT
 from cupoch_b200.testing import datagen
+from test_facade_cpp import build_facade
 
 
 @pytest.fixture(scope="module")
@@ -19,27 +19,15 @@ def fpso():
     return fps_py
 
 
-def build_facade():
-    import __graft_entry__
-    __graft_entry__.build()
-    from test_facade_cpp import build_dir
-    exe = os.path.join(build_dir(), "facade_fps")
-    lib = os.path.join(ROOT, "cupoch_b200", "lib")
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-Wall", "-I" + os.path.join(ROOT, "include"),
-                           os.path.join(ROOT, "tests", "cpp", "facade_fps.cpp"), "-o", exe, "-L" + lib,
-                           "-lcupoch_b200", "-Wl,-rpath," + lib])
-    return exe
-
-
 def test_facade_fps_compiles_and_links():
-    exe = build_facade()
+    exe = build_facade("facade_fps")
     out = subprocess.run(["ldd", exe], capture_output=True, text=True).stdout
     assert "libcupoch_b200.so" in out and "not found" not in out
 
 
 @pytest.mark.gpu
 def test_facade_fps_matches_oracle(fpso):
-    exe = build_facade()
+    exe = build_facade("facade_fps")
     pts, nrm = datagen.surface(60_000, 19)
     k = 700
     with tempfile.TemporaryDirectory() as d:

@@ -9,8 +9,8 @@ import tempfile
 import numpy as np
 import pytest
 
-from conftest import ROOT
 from cupoch_b200.testing import datagen
+from test_facade_cpp import build_facade
 
 
 @pytest.fixture(scope="module")
@@ -21,28 +21,16 @@ def seg():
     return segment_plane_py
 
 
-def build_facade():
-    import __graft_entry__
-    __graft_entry__.build()
-    from test_facade_cpp import build_dir
-    exe = os.path.join(build_dir(), "facade_segment_plane")
-    lib = os.path.join(ROOT, "cupoch_b200", "lib")
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-Wall", "-I" + os.path.join(ROOT, "include"),
-                           os.path.join(ROOT, "tests", "cpp", "facade_segment_plane.cpp"), "-o", exe, "-L" + lib,
-                           "-lcupoch_b200", "-Wl,-rpath," + lib])
-    return exe
-
-
 def test_facade_segment_plane_compiles_and_links():
-    exe = build_facade()
+    exe = build_facade("facade_segment_plane")
     out = subprocess.run(["ldd", exe], capture_output=True, text=True).stdout
     assert "libcupoch_b200.so" in out and "not found" not in out
 
 
 @pytest.mark.gpu
 def test_facade_segment_plane_matches_oracle(seg):
-    exe = build_facade()
-    pts = datagen.plane_scene(50_000, 17)
+    exe = build_facade("facade_segment_plane")
+    pts =datagen.plane_scene(50_000, 17)
     seed, thr, T = 3, 0.01, 50
     libc = C.CDLL(None)
     libc.srand(C.c_uint(seed))

@@ -7,24 +7,12 @@ import tempfile
 import numpy as np
 import pytest
 
-from conftest import ROOT
 from cupoch_b200.testing import datagen
-
-
-def build_facade():
-    import __graft_entry__
-    __graft_entry__.build()
-    from test_facade_cpp import build_dir
-    exe = os.path.join(build_dir(), "facade_shot")
-    lib = os.path.join(ROOT, "cupoch_b200", "lib")
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-Wall", "-I" + os.path.join(ROOT, "include"),
-                           os.path.join(ROOT, "tests", "cpp", "facade_shot.cpp"), "-o", exe, "-L" + lib,
-                           "-lcupoch_b200", "-Wl,-rpath," + lib])
-    return exe
+from test_facade_cpp import build_facade
 
 
 def test_facade_shot_compiles_and_links():
-    exe = build_facade()
+    exe = build_facade("facade_shot")
     out = subprocess.run(["ldd", exe], capture_output=True, text=True).stdout
     assert "libcupoch_b200.so" in out and "not found" not in out
 
@@ -32,7 +20,7 @@ def test_facade_shot_compiles_and_links():
 @pytest.mark.gpu
 def test_facade_shot_matches_oracle():
     from oracle import shot_py
-    exe = build_facade()
+    exe = build_facade("facade_shot")
     pts, nrm = datagen.surface(20_000, 29)
     radius = np.float32(5.0 / np.sqrt(1e5))
     with tempfile.TemporaryDirectory() as d:

@@ -227,6 +227,10 @@ __device__ void svd3(const double *A, double *U, double *s, double *V) {
                 U[6 + j] = U[a] * U[3 + b] - U[3 + a] * U[b];
             }
         }
+    // A = 0 (one correspondence, or every model point at its centre): Eigen's JacobiSVD returns U = V = I, so Kabsch
+    // gives the identity rotation; a zero U here would make R = 0 and collapse the cloud onto one point
+    if (s[0] == 0 && s[1] == 0 && s[2] == 0)
+        for (int i = 0; i < 9; ++i) U[i] = (i % 4 == 0) ? 1.0 : 0.0;
 }
 // kabsch.cu:42-120 incl. the divide-by-model.size() quirk (:76-78,107)
 __device__ void kabsch_from_sums(const double *S, unsigned long long n_model, float *T) {

@@ -1213,6 +1213,9 @@ static void svd3(const double A[9], double U[9], double s[3], double V[9]) {
                 U[6 + j] = U[a] * U[3 + b] - U[3 + a] * U[b];
             }
         }
+    /* A = 0: Eigen's JacobiSVD returns U = V = I (kabsch.cu:108-113 then gives the identity rotation, not R = 0) */
+    if (s[0] == 0 && s[1] == 0 && s[2] == 0)
+        for (int i = 0; i < 9; ++i) U[i] = (i % 4 == 0) ? 1.0 : 0.0;
 }
 static double det3d(const double M[9]) {
     return M[0] * (M[4] * M[8] - M[5] * M[7]) - M[1] * (M[3] * M[8] - M[5] * M[6]) + M[2] * (M[3] * M[7] - M[4] * M[6]);

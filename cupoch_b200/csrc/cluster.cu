@@ -95,30 +95,24 @@ extern "C" int cphb_cluster_dbscan(const float *points, size_t n, float eps, int
     }
     const int K = max_edges + 1;
     cphb_nbr_table t;
+    cphb_scratch sc(s);
     int32_t *queue = nullptr;
     int *degree = nullptr, *visited = nullptr, *ncl = nullptr;
     unsigned *stamp = nullptr;
     int rc = cphb_nbr_table_create(points, n, 0, n, 0, eps, K, &t, s);
-    if (!rc) rc = cphb_alloc_async((void **)&degree, sizeof(int) * n, s);
-    if (!rc) rc = cphb_alloc_async((void **)&visited, sizeof(int) * n, s);
-    if (!rc) rc = cphb_alloc_async((void **)&stamp, sizeof(unsigned) * n, s);
-    if (!rc) rc = cphb_alloc_async((void **)&queue, sizeof(int32_t) * n, s);
-    if (!rc) rc = cphb_alloc_async((void **)&ncl, sizeof(int), s);
+    if (!rc) rc = sc.alloc(&degree, n);
+    if (!rc) rc = sc.alloc(&visited, n);
+    if (!rc) rc = sc.alloc(&stamp, n);
+    if (!rc) rc = sc.alloc(&queue, n);
+    if (!rc) rc = sc.alloc(&ncl, 1);
+    int h = 0;
     if (!rc) {
         CPHB_LAUNCH(dbscan_degree_kernel, (unsigned)((n + 255) / 256), 256, 0, s, t.idx, n, K, min_points, degree);
         CPHB_LAUNCH(dbscan_bfs_kernel, 1, DB_THREADS, 0, s, t.idx, degree, (unsigned)n, K, min_points, labels_out, stamp, visited,
                     queue, ncl);
-        cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess) { cphb_set_error("dbscan kernels: %s", cudaGetErrorString(e)); rc = CPHB_ERR_CUDA; }
-    }
-    int h = 0;
-    if (!rc) {
-        cudaError_t e = cudaMemcpyAsync(&h, ncl, sizeof(int), cudaMemcpyDeviceToHost, s);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-        if (e != cudaSuccess) { cphb_set_error("cphb_cluster_dbscan: %s", cudaGetErrorString(e)); rc = CPHB_ERR_CUDA; }
+        rc = cphb_read_back(&h, ncl, sizeof(int), s, "cphb_cluster_dbscan");
     }
     if (h_n_clusters) *h_n_clusters = h;
-    cphb_free_async(degree, s); cphb_free_async(visited, s); cphb_free_async(stamp, s); cphb_free_async(queue, s);
-    cphb_free_async(ncl, s);
+    sc.release();
     return cphb_nbr_table_release(&t, rc, s);
 }

@@ -84,6 +84,43 @@ static inline size_t cphb_align(size_t x, size_t a) { return (x + a - 1) / a * a
 int cphb_alloc_async(void **p, size_t bytes, cudaStream_t s);
 void cphb_free_async(void *p, cudaStream_t s);
 
+// The device scratch of one call: every buffer alloc() hands out goes back to the pool on the owner's stream when the
+// owner leaves scope, so no return path leaks it.  release() frees them at once, for callers that free before their
+// final synchronise.  More than CPHB_SCRATCH_SLOTS buffers is a programming error: alloc() reports it and allocates
+// nothing.
+#define CPHB_SCRATCH_SLOTS 16
+class cphb_scratch {
+  public:
+    explicit cphb_scratch(cudaStream_t s) : s_(s) {}
+    ~cphb_scratch() { release(); }
+    cphb_scratch(const cphb_scratch &) = delete;
+    cphb_scratch &operator=(const cphb_scratch &) = delete;
+    // count elements of T; returns cphb_alloc_async's rc
+    template <class T>
+    int alloc(T **p, size_t count) {
+        if (n_ == CPHB_SCRATCH_SLOTS) {
+            cphb_set_error("cphb_scratch: more than %d buffers", CPHB_SCRATCH_SLOTS);
+            return CPHB_ERR_INVALID;
+        }
+        const int rc = cphb_alloc_async((void **)p, sizeof(T) * count, s_);
+        if (!rc) p_[n_++] = *p;
+        return rc;
+    }
+    void release() {
+        for (int i = 0; i < n_; ++i) cphb_free_async(p_[i], s_);
+        n_ = 0;
+    }
+
+  private:
+    cudaStream_t s_;
+    void *p_[CPHB_SCRATCH_SLOTS];
+    int n_ = 0;
+};
+
+// pending launch error, then `bytes` from d to h (0: none), then a synchronise of s; the first failure is reported as
+// "<who>: <CUDA error>" and returns CPHB_ERR_CUDA
+int cphb_read_back(void *h, const void *d, size_t bytes, cudaStream_t s, const char *who);
+
 // radix sort of (key,value) u32 pairs by the low `bits` bits (CUB, stable; index
 // build, source ordering and SegmentPlane's sampler -- never inside the ICP
 // per-iteration loop). sort.cu

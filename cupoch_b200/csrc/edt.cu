@@ -343,15 +343,14 @@ extern "C" int cphb_dt_set_geometry(cphb_dt *g, float voxel_size, const float or
 static int edt_sweeps(cphb_dt *g, int with_distance, cudaStream_t s) {
     const int r = g->res;
     const size_t lines = (size_t)r * r;
+    cphb_scratch sc(s);
     uint32_t *stack = nullptr;
-    int rc = cphb_alloc_async((void **)&stack, sizeof(uint32_t) * g->cells, s);
+    int rc = sc.alloc(&stack, g->cells);
     if (rc) return rc;
     CPHB_LAUNCH(edt_sweep_z_kernel, (unsigned)((lines * 32 + 255) / 256), 256, 0, s, (const unsigned *)g->dist, r, g->nearest);
     CPHB_LAUNCH(edt_sweep_kernel<1>, (unsigned)((lines + 127) / 128), 128, 0, s, g->nearest, stack, g->dist, r, g->voxel_size, with_distance);
     CPHB_LAUNCH(edt_sweep_kernel<0>, (unsigned)((lines + 127) / 128), 128, 0, s, g->nearest, stack, g->dist, r, g->voxel_size, with_distance);
-    cudaError_t e = cudaGetLastError();
-    cphb_free_async(stack, s);
-    if (e != cudaSuccess) { cphb_set_error("edt sweeps: %s", cudaGetErrorString(e)); return CPHB_ERR_CUDA; }
+    CPHB_CHECK_LAUNCH();
     return CPHB_OK;
 }
 

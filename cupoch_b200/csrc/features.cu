@@ -106,10 +106,11 @@ static int normals_impl(const float *points, size_t n, int knn, float radius, in
     const float r2 = (knn > 0) ? INFINITY : radius * radius;  // kdtree_flann.inl:120
     const bool self_order = (first == 0 && count == n);
     cphb_index *ix = nullptr;
+    cphb_scratch sc(s);
     uint32_t *perm = nullptr;
     int rc = cphb_index_create(points, n, s, &ix);
     if (!rc && !self_order && count > 32) {
-        rc = cphb_alloc_async((void **)&perm, sizeof(uint32_t) * count, s);
+        rc = sc.alloc(&perm, count);
         if (!rc) rc = cphb_hilbert_order_n(points + 3 * first, count, perm, ix->bounds, 1, count < n ? count : n, s);
     }
     if (!rc) {
@@ -117,7 +118,7 @@ static int normals_impl(const float *points, size_t n, int knn, float radius, in
         rc = launch_fused(ix, normals_fused_kernel<3>, normals_fused_kernel<5>, lanes, k, s, points, first, count, perm,
                           self_order ? 1 : 0, r2, k, out_normals);
     }
-    cphb_free_async(perm, s);
+    sc.release();
     const cudaError_t e = cudaStreamSynchronize(s);
     cphb_index_destroy(ix);
     if (!rc && e != cudaSuccess) { cphb_set_error("normals_fused_kernel: %s", cudaGetErrorString(e)); rc = CPHB_ERR_CUDA; }

@@ -202,27 +202,18 @@ __global__ void __launch_bounds__(FLT_BLOCK) keep_write_kernel(const uint8_t *__
 // keep flags -> ascending indices in indices_out, count to *h_n_out (synchronises)
 int cphb_compact_flags(const uint8_t *keep, size_t n, int32_t *indices_out, size_t *h_n_out, cudaStream_t s) {
     const unsigned nb = (unsigned)((n + FLT_BLOCK - 1) / FLT_BLOCK);
+    cphb_scratch sc(s);
     unsigned *counts = nullptr;
     unsigned long long *total = nullptr;
-    int rc = cphb_alloc_async((void **)&counts, sizeof(unsigned) * (size_t)nb + 16, s);
-    if (!rc) rc = cphb_alloc_async((void **)&total, sizeof(unsigned long long), s);
-    if (!rc) {
-        CPHB_LAUNCH(keep_count_kernel, nb, FLT_BLOCK, 0, s, keep, n, counts);
-        CPHB_LAUNCH(keep_scan_kernel, 1, FLT_BLOCK, 0, s, counts, nb, total);
-        CPHB_LAUNCH(keep_write_kernel, nb, FLT_BLOCK, 0, s, keep, n, counts, indices_out);
-        cudaError_t e = cudaGetLastError();
-        unsigned long long h = 0;
-        if (e == cudaSuccess) e = cudaMemcpyAsync(&h, total, sizeof(h), cudaMemcpyDeviceToHost, s);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-        if (e != cudaSuccess) {
-            cphb_set_error("cphb_compact_flags: %s", cudaGetErrorString(e));
-            rc = CPHB_ERR_CUDA;
-        } else {
-            *h_n_out = (size_t)h;
-        }
-    }
-    cphb_free_async(counts, s);
-    cphb_free_async(total, s);
+    int rc = sc.alloc(&counts, (size_t)nb + 4);
+    if (!rc) rc = sc.alloc(&total, 1);
+    if (rc) return rc;
+    CPHB_LAUNCH(keep_count_kernel, nb, FLT_BLOCK, 0, s, keep, n, counts);
+    CPHB_LAUNCH(keep_scan_kernel, 1, FLT_BLOCK, 0, s, counts, nb, total);
+    CPHB_LAUNCH(keep_write_kernel, nb, FLT_BLOCK, 0, s, keep, n, counts, indices_out);
+    unsigned long long h = 0;
+    rc = cphb_read_back(&h, total, sizeof(h), s, "cphb_compact_flags");
+    if (!rc) *h_n_out = (size_t)h;
     return rc;
 }
 
@@ -248,14 +239,15 @@ extern "C" int cphb_remove_radius_outliers(const float *points, size_t n, int nb
     }
     const int k = nb_points + 1;
     cphb_nbr_table t;
+    cphb_scratch sc(s);
     uint8_t *keep = nullptr;
     int rc = cphb_nbr_table_create(points, n, 0, n, 0, radius, k, &t, s);  // the reference builds a fresh tree too (:324-325)
-    if (!rc) rc = cphb_alloc_async((void **)&keep, n, s);
+    if (!rc) rc = sc.alloc(&keep, n);
     if (!rc) {
         CPHB_LAUNCH(radius_keep_kernel, (unsigned)((n + 255) / 256), 256, 0, s, t.idx, n, k, nb_points, keep);
         rc = cphb_compact_flags(keep, n, indices_out, h_n_out, s);
     }
-    cphb_free_async(keep, s);
+    sc.release();
     return cphb_nbr_table_release(&t, rc, s);
 }
 
@@ -280,14 +272,15 @@ extern "C" int cphb_remove_statistical_outliers(const float *points, size_t n, i
     const int k = nb_neighbors;
     const unsigned nb = (unsigned)((n + FLT_BLOCK - 1) / FLT_BLOCK);
     cphb_nbr_table t;
+    cphb_scratch sc(s);
     float *avg = nullptr, *scalars = nullptr;
     double *partial = nullptr;
     uint8_t *keep = nullptr;
     int rc = cphb_nbr_table_create(points, n, 0, n, k, 0.f, 0, &t, s);
-    if (!rc) rc = cphb_alloc_async((void **)&avg, sizeof(float) * n, s);
-    if (!rc) rc = cphb_alloc_async((void **)&scalars, sizeof(float) * 4, s);
-    if (!rc) rc = cphb_alloc_async((void **)&partial, sizeof(double) * 2 * (size_t)nb, s);
-    if (!rc) rc = cphb_alloc_async((void **)&keep, n, s);
+    if (!rc) rc = sc.alloc(&avg, n);
+    if (!rc) rc = sc.alloc(&scalars, 4);
+    if (!rc) rc = sc.alloc(&partial, 2 * (size_t)nb);
+    if (!rc) rc = sc.alloc(&keep, n);
     if (!rc) {
         const unsigned g256 = (unsigned)((n + 255) / 256);
         CPHB_LAUNCH(row_mean_kernel, g256, 256, 0, s, t.d2, n, k, avg);
@@ -297,16 +290,9 @@ extern "C" int cphb_remove_statistical_outliers(const float *points, size_t n, i
         CPHB_LAUNCH(stat_final_kernel, 1, FLT_BLOCK, 0, s, partial, nb, 1, std_ratio, scalars);
         CPHB_LAUNCH(stat_keep_kernel, g256, 256, 0, s, avg, n, scalars, keep);
         rc = cphb_compact_flags(keep, n, indices_out, h_n_out, s);
-        if (!rc && h_stats) {
-            cudaError_t e = cudaMemcpyAsync(h_stats, scalars, sizeof(float) * 3, cudaMemcpyDeviceToHost, s);
-            if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-            if (e != cudaSuccess) { cphb_set_error("cphb_remove_statistical_outliers: %s", cudaGetErrorString(e)); rc = CPHB_ERR_CUDA; }
-        }
+        if (!rc && h_stats) rc = cphb_read_back(h_stats, scalars, sizeof(float) * 3, s, "cphb_remove_statistical_outliers");
     }
-    cphb_free_async(avg, s);
-    cphb_free_async(scalars, s);
-    cphb_free_async(partial, s);
-    cphb_free_async(keep, s);
+    sc.release();
     return cphb_nbr_table_release(&t, rc, s);
 }
 

@@ -108,15 +108,16 @@ extern "C" int cphb_compute_fpfh_feature(const float *points, const float *norma
         return CPHB_ERR_INVALID;
     }
     cphb_nbr_table t;
+    cphb_scratch sc(s);
     float *spfh = nullptr;
     int rc = cphb_nbr_table_create(points, n, 0, n, knn, radius, max_nn, &t, s);
-    if (!rc) rc = cphb_alloc_async((void **)&spfh, sizeof(float) * n * 33, s);
+    if (!rc) rc = sc.alloc(&spfh, n * 33);
     if (!rc) {
         CPHB_LAUNCH(spfh_kernel, (unsigned)((n + 127) / 128), 128, 0, s, points, normals, n, t.idx, k, spfh);
         CPHB_LAUNCH(fpfh_kernel, (unsigned)((n + 127) / 128), 128, 0, s, spfh, n, t.idx, t.d2, k, out_features);
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) { cphb_set_error("fpfh kernels: %s", cudaGetErrorString(e)); rc = CPHB_ERR_CUDA; }
     }
-    cphb_free_async(spfh, s);
+    sc.release();
     return cphb_nbr_table_release(&t, rc, s);
 }

@@ -147,10 +147,11 @@ extern "C" int cphb_farthest_point_down_sample(const float *points, size_t n, si
     a.dist = nullptr;
     a.slots = nullptr;
     if (res) smem = a.chunk * sizeof(float4);
-    int rc = cphb_alloc_async((void **)&a.slots, 3 * sizeof(unsigned long long), s);
+    cphb_scratch sc(s);
+    int rc = sc.alloc(&a.slots, 3);
     if (!rc && !res) {
         if (d2_out) a.dist = d2_out;
-        else rc = cphb_alloc_async((void **)&a.dist, n * sizeof(float), s);
+        else rc = sc.alloc(&a.dist, n);
     }
     if (!rc) {
         cudaError_t e = cudaMemsetAsync(a.slots, 0, 3 * sizeof(unsigned long long), s);
@@ -162,7 +163,5 @@ extern "C" int cphb_farthest_point_down_sample(const float *points, size_t n, si
             rc = CPHB_ERR_CUDA;
         }
     }
-    cphb_free_async(a.slots, s);
-    if (a.dist != d2_out) cphb_free_async(a.dist, s);
     return rc;
 }

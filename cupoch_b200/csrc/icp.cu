@@ -782,13 +782,13 @@ extern "C" int cphb_transform(float *points, float *normals, float *covariances,
                               const float h_T[16], void *stream) {
     cudaStream_t s = (cudaStream_t)stream;
     if (n == 0) return CPHB_OK;
+    cphb_scratch sc(s);
     float *Td = nullptr;
-    int rc = cphb_alloc_async((void **)&Td, 64, s);
+    int rc = sc.alloc(&Td, 16);
     if (rc) return rc;
     CPHB_CUDA(cudaMemcpyAsync(Td, h_T, 64, cudaMemcpyHostToDevice, s));
     CPHB_LAUNCH(transform_kernel, (unsigned)((n + 255) / 256), 256, 0, s, points, normals, covariances, cov_col_major, n, Td);
     CPHB_CHECK_LAUNCH();
-    cphb_free_async(Td, s);
     return CPHB_OK;
 }
 
@@ -824,9 +824,10 @@ static int run_estimate(int estimation, const cphb_cloud *source, const cphb_clo
     a.corr = corr;
     a.n_corr = (unsigned)n_corr;
     unsigned grid = (unsigned)((n_corr + ICP_BLOCK - 1) / ICP_BLOCK);
+    cphb_scratch sc(s);
     char *buf = nullptr;
     size_t bytes = cphb_align(sizeof(double) * 32 * grid, 256) + 256 + 256 + 64;
-    int rc = cphb_alloc_async((void **)&buf, bytes, s);
+    int rc = sc.alloc(&buf, bytes);
     if (rc) return rc;
     a.partials = (double *)buf;
     a.total = (double *)(buf + cphb_align(sizeof(double) * 32 * grid, 256));
@@ -846,11 +847,7 @@ static int run_estimate(int estimation, const cphb_cloud *source, const cphb_clo
         if (h_T) CPHB_LAUNCH(estimate_solve_kernel<decltype(k)::value>, 1, 32, 0, s, a.total, nm, dt, have, Td);
     });
     if (h_T) CPHB_CUDA(cudaMemcpyAsync(h_T, Td, 64, cudaMemcpyDeviceToHost, s));
-    CPHB_CHECK_LAUNCH();
-    CPHB_CUDA(cudaMemcpyAsync(h_S, a.total, sizeof(double) * 32, cudaMemcpyDeviceToHost, s));
-    CPHB_CUDA(cudaStreamSynchronize(s));
-    cphb_free_async(buf, s);
-    return CPHB_OK;
+    return cphb_read_back(h_S, a.total, sizeof(double) * 32, s, "estimate");
 }
 
 extern "C" int cphb_compute_transformation(int estimation, const cphb_cloud *source, const cphb_cloud *target,
@@ -890,15 +887,14 @@ extern "C" int cphb_kabsch(const float *model, size_t n_model, const float *targ
     memset(&tgt, 0, sizeof(tgt));
     src.points = model; src.n = n_model;
     tgt.points = target; tgt.n = n_model;
-    int32_t *tmp = nullptr;
+    cphb_scratch sc(s);
     if (!corr) {
         n_corr = n_model;
-        int rc = cphb_alloc_async((void **)&tmp, sizeof(int32_t) * 2 * (n_model ? n_model : 1), s);
+        int32_t *tmp = nullptr;
+        const int rc = sc.alloc(&tmp, 2 * (n_model ? n_model : 1));
         if (rc) return rc;
         if (n_model) CPHB_LAUNCH(iota_pairs_kernel, (unsigned)((n_model + 255) / 256), 256, 0, s, tmp, (unsigned)n_model);
         corr = tmp;
     }
-    int rc = cphb_compute_transformation(CPHB_EST_POINT_TO_POINT, &src, &tgt, corr, n_corr, nullptr, h_T, stream);
-    cphb_free_async(tmp, s);
-    return rc;
+    return cphb_compute_transformation(CPHB_EST_POINT_TO_POINT, &src, &tgt, corr, n_corr, nullptr, h_T, stream);
 }

@@ -59,6 +59,14 @@ int cphb_alloc_async(void **p, size_t bytes, cudaStream_t s) {
 void cphb_free_async(void *p, cudaStream_t s) {
     if (p) cudaFreeAsync(p, s);
 }
+int cphb_read_back(void *h, const void *d, size_t bytes, cudaStream_t s, const char *who) {
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess && bytes) e = cudaMemcpyAsync(h, d, bytes, cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    if (e == cudaSuccess) return CPHB_OK;
+    cphb_set_error("%s: %s", who, cudaGetErrorString(e));
+    return CPHB_ERR_CUDA;
+}
 
 extern "C" int cphb_reserve_pool(size_t bytes) {
     void *p = nullptr;
@@ -473,16 +481,15 @@ int cphb_hilbert_order(const float *xyz, size_t n, uint32_t *perm_out, float *bo
 int cphb_hilbert_order_n(const float *xyz, size_t n, uint32_t *perm_out, float *bounds_dev6, int bounds_given,
                          size_t n_ref, cudaStream_t s) {
     if (n == 0) return CPHB_OK;
+    cphb_scratch sc(s);
     unsigned *b = (unsigned *)bounds_dev6;
-    if (!b) bounds_given = 0;
-    void *own = nullptr;
     if (!b) {
-        int rc = cphb_alloc_async(&own, 32, s);
+        bounds_given = 0;
+        const int rc = sc.alloc(&b, 8);
         if (rc) return rc;
-        b = (unsigned *)own;
     }
     uint32_t *scratch = nullptr;
-    int rc = cphb_alloc_async((void **)&scratch, sizeof(uint32_t) * 3 * n, s);
+    int rc = sc.alloc(&scratch, 3 * n);
     if (rc) return rc;
     uint32_t *keys = scratch, *keys2 = scratch + n, *vals = scratch + 2 * n;
     if (!bounds_given) {
@@ -501,24 +508,11 @@ int cphb_hilbert_order_n(const float *xyz, size_t n, uint32_t *perm_out, float *
     if (levels < 4) levels = 4;
     CPHB_LAUNCH(hilbert_key_kernel, (unsigned)((n + 255) / 256), 256, 0, s, xyz, n, b, 30 - 3 * levels, keys, vals);
     CPHB_CHECK_LAUNCH();
-    rc = cphb_sort_pairs_u32(keys, keys2, vals, perm_out, n, 3 * levels, s);
-    cphb_free_async(scratch, s);
-    cphb_free_async(own, s);
-    return rc;
+    return cphb_sort_pairs_u32(keys, keys2, vals, perm_out, n, 3 * levels, s);
 }
 
-extern "C" int cphb_index_create(const float *xyz, size_t n, void *stream, cphb_index **out) {
-    cudaStream_t s = (cudaStream_t)stream;
-    if (!out || (n && !xyz)) {
-        cphb_set_error("cphb_index_create: null argument");
-        return CPHB_ERR_INVALID;
-    }
-    if (n > (size_t)0x7fffffff) {
-        cphb_set_error("cphb_index_create: n=%zu exceeds int32 indices", n);
-        return CPHB_ERR_INVALID;
-    }
-    cphb_index *ix = new cphb_index();
-    memset(ix, 0, sizeof(*ix));
+// fills the zeroed handle ix; on failure the caller destroys it (with its arena, if one was allocated)
+static int index_build(cphb_index *ix, const float *xyz, size_t n, cudaStream_t s) {
     CPHB_CUDA(cudaGetDevice(&ix->device));
     ix->stream = s;
     size_t count[CPHB_LEVELS], pad[CPHB_LEVELS];
@@ -529,7 +523,6 @@ extern "C" int cphb_index_create(const float *xyz, size_t n, void *stream, cphb_
     }
     if (count[CPHB_LEVELS - 1] > 32) {
         cphb_set_error("cphb_index_create: n=%zu too large for %d levels", n, CPHB_LEVELS);
-        delete ix;
         return CPHB_ERR_INVALID;
     }
     size_t n_pad = (count[0] ? count[0] : 1) * CPHB_LEAF;
@@ -547,12 +540,10 @@ extern "C" int cphb_index_create(const float *xyz, size_t n, void *stream, cphb_
     size_t off_inv = off;
     off = cphb_align(off + sizeof(uint32_t) * (n ? n : 1), 256);
     ix->arena_bytes = off;
-    int rc = cphb_alloc_async(&ix->arena, off, s);
-    if (rc) {
-        delete ix;
-        return rc;
-    }
-    char *base = (char *)ix->arena;
+    char *base = nullptr;
+    int rc = cphb_alloc_async((void **)&base, off, s);
+    if (rc) return rc;
+    ix->arena = base;
     float4 *pts = (float4 *)(base + off_pts);
     Box *boxes[CPHB_LEVELS];
     for (int l = 0; l < CPHB_LEVELS; ++l) boxes[l] = (Box *)(base + off_box[l]);
@@ -562,11 +553,7 @@ extern "C" int cphb_index_create(const float *xyz, size_t n, void *stream, cphb_
 
     if (n) {
         rc = cphb_hilbert_order(xyz, n, perm, ix->bounds, 0, s);
-        if (rc) {
-            cphb_free_async(ix->arena, s);
-            delete ix;
-            return rc;
-        }
+        if (rc) return rc;
     } else {
         CPHB_LAUNCH(bounds_init_kernel, 1, 32, 0, s, (unsigned *)ix->bounds);
     }
@@ -590,6 +577,25 @@ extern "C" int cphb_index_create(const float *xyz, size_t n, void *stream, cphb_
     int top = 0;
     while (count[top] > 32) ++top;
     ix->v.top = top;
+    return CPHB_OK;
+}
+
+extern "C" int cphb_index_create(const float *xyz, size_t n, void *stream, cphb_index **out) {
+    if (!out || (n && !xyz)) {
+        cphb_set_error("cphb_index_create: null argument");
+        return CPHB_ERR_INVALID;
+    }
+    if (n > (size_t)0x7fffffff) {
+        cphb_set_error("cphb_index_create: n=%zu exceeds int32 indices", n);
+        return CPHB_ERR_INVALID;
+    }
+    cphb_index *ix = new cphb_index();
+    memset(ix, 0, sizeof(*ix));
+    const int rc = index_build(ix, xyz, n, (cudaStream_t)stream);
+    if (rc) {
+        cphb_index_destroy(ix);
+        return rc;
+    }
     *out = ix;
     return CPHB_OK;
 }
@@ -605,18 +611,17 @@ extern "C" int cphb_min_max_bound(const float *points, size_t n, float h_min[3],
     cudaStream_t s = (cudaStream_t)stream;
     for (int a = 0; a < 3; ++a) h_min[a] = h_max[a] = 0.f;  // reference: Zero() for an empty cloud
     if (n == 0) return CPHB_OK;
+    cphb_scratch sc(s);
     unsigned *b = nullptr;
-    int rc = cphb_alloc_async((void **)&b, 32, s);
+    int rc = sc.alloc(&b, 8);
     if (rc) return rc;
     CPHB_LAUNCH(bounds_init_kernel, 1, 32, 0, s, b);
     int grid = (int)((n + 255) / 256);
     if (grid > CPHB_SMS * 8) grid = CPHB_SMS * 8;
     CPHB_LAUNCH(bounds_kernel, grid, 256, 0, s, points, n, b);
-    CPHB_CHECK_LAUNCH();
     unsigned h[6];
-    CPHB_CUDA(cudaMemcpyAsync(h, b, sizeof(h), cudaMemcpyDeviceToHost, s));
-    CPHB_CUDA(cudaStreamSynchronize(s));
-    cphb_free_async(b, s);
+    rc = cphb_read_back(h, b, sizeof(h), s, "cphb_min_max_bound");
+    if (rc) return rc;
     for (int a = 0; a < 3; ++a) {
         h_min[a] = ord2f(h[a]);
         h_max[a] = ord2f(h[3 + a]);

@@ -334,18 +334,19 @@ extern "C" int cphb_occgrid_insert(cphb_occgrid *g, const float *points, size_t 
     cudaStream_t s = (cudaStream_t)stream;
     if (!g || !viewpoint || (n && !points)) { cphb_set_error("cphb_occgrid_insert: null argument"); return CPHB_ERR_INVALID; }
     if (n == 0) return CPHB_OK;  // occupancygrid.cu:465
+    cphb_scratch sc(s);
     float *ranged = nullptr;
     unsigned char *hit = nullptr;
-    int rc = cphb_alloc_async((void **)&ranged, sizeof(float) * 3 * n, s);
-    if (!rc) rc = cphb_alloc_async((void **)&hit, n, s);
-    if (rc) { cphb_free_async(ranged, s); return rc; }
+    int rc = sc.alloc(&ranged, 3 * n);
+    if (!rc) rc = sc.alloc(&hit, n);
+    if (rc) return rc;
     unsigned *max_bits = g->scratch + 8;
     CPHB_CUDA(cudaMemsetAsync(max_bits, 0, 4, s));
     const unsigned grid = (unsigned)((n + 255) / 256);
     CPHB_LAUNCH(occ_range_kernel, grid, 256, 0, s, points, n, viewpoint[0], viewpoint[1], viewpoint[2], max_range, ranged, hit, max_bits);
     unsigned h_bits = 0;
-    CPHB_CUDA(cudaMemcpyAsync(&h_bits, max_bits, 4, cudaMemcpyDeviceToHost, s));  // the reference reads max_element back too (:490-492)
-    CPHB_CUDA(cudaStreamSynchronize(s));
+    rc = cphb_read_back(&h_bits, max_bits, 4, s, "cphb_occgrid_insert");  // the reference reads max_element back too (:490-492)
+    if (rc) return rc;
     float max_dist;
     memcpy(&max_dist, &h_bits, 4);
     const int n_div = (int)ceilf(max_dist / g->voxel_size);
@@ -361,8 +362,6 @@ extern "C" int cphb_occgrid_insert(cphb_occgrid *g, const float *points, size_t 
     CPHB_LAUNCH(occ_apply_hit_kernel, grid, 256, 0, s, ranged, hit, n, o[0], o[1], o[2], g->voxel_size, g->res, g->occ_bits, g->prob,
                 g->idx_bits, g->bounds, g->prm.prob_hit_log, g->prm.clamping_thres_min, g->prm.clamping_thres_max);
     CPHB_CHECK_LAUNCH();
-    cphb_free_async(ranged, s);
-    cphb_free_async(hit, s);
     return CPHB_OK;
 }
 
@@ -386,13 +385,13 @@ extern "C" int cphb_occgrid_add_voxel(cphb_occgrid *g, const int32_t voxel[3], i
         cphb_set_error("[OccupancyGrid] a provided voxel is not in the occupancy grid range.");
         return CPHB_ERR_INVALID;
     }
+    cphb_scratch sc(s);
     int32_t *d = nullptr;
-    int rc = cphb_alloc_async((void **)&d, 16, s);
+    int rc = sc.alloc(&d, 4);
     if (rc) return rc;
     CPHB_CUDA(cudaMemcpyAsync(d, voxel, 12, cudaMemcpyHostToDevice, s));
     rc = cphb_occgrid_add_voxels(g, d, 1, occupied, stream);
     CPHB_CUDA(cudaStreamSynchronize(s));  // (the host array may go out of scope)
-    cphb_free_async(d, s);
     return rc;
 }
 
@@ -450,27 +449,24 @@ extern "C" int cphb_occgrid_extract(const cphb_occgrid *g, int which, int32_t *o
     if (hi[0] < lo[0] || hi[1] < lo[1] || hi[2] < lo[2]) return CPHB_OK;
     const int dx = hi[0] - lo[0] + 1, dy = hi[1] - lo[1] + 1, dz = hi[2] - lo[2] + 1;
     const size_t m = (size_t)dx * dy * dz;
+    cphb_scratch sc(s);
     unsigned char *keep = nullptr;
     int32_t *sel = nullptr;
-    rc = cphb_alloc_async((void **)&keep, m, s);
-    if (!rc) rc = cphb_alloc_async((void **)&sel, sizeof(int32_t) * m, s);
-    if (rc) { cphb_free_async(keep, s); return rc; }
+    rc = sc.alloc(&keep, m);
+    if (!rc) rc = sc.alloc(&sel, m);
+    if (rc) return rc;
     CPHB_LAUNCH(occ_extract_flag_kernel, (unsigned)((m + 255) / 256), 256, 0, s, g->prob, g->res, lo[0], lo[1], lo[2], dx, dy, dz,
                 g->prm.occ_prob_thres_log, which, keep);
     size_t cnt = 0;
     rc = cphb_compact_flags(keep, m, sel, &cnt, s);
-    if (!rc) {
-        *h_count = cnt;
-        const size_t w = cnt < capacity ? cnt : capacity;
-        if (w && (out_index || out_prob))
-            CPHB_LAUNCH(occ_extract_write_kernel, (unsigned)((w + 255) / 256), 256, 0, s, g->prob, g->idx_bits, g->res, lo[0], lo[1], lo[2], dy,
-                        dz, sel, w, out_index, out_prob);
-        cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess) { cphb_set_error("occ_extract: %s", cudaGetErrorString(e)); rc = CPHB_ERR_CUDA; }
-    }
-    cphb_free_async(keep, s);
-    cphb_free_async(sel, s);
-    return rc;
+    if (rc) return rc;
+    *h_count = cnt;
+    const size_t w = cnt < capacity ? cnt : capacity;
+    if (w && (out_index || out_prob))
+        CPHB_LAUNCH(occ_extract_write_kernel, (unsigned)((w + 255) / 256), 256, 0, s, g->prob, g->idx_bits, g->res, lo[0], lo[1], lo[2], dy,
+                    dz, sel, w, out_index, out_prob);
+    CPHB_CHECK_LAUNCH();
+    return CPHB_OK;
 }
 
 // DenseGrid::GetVoxelIndex + OccupancyGrid::GetVoxel (densegrid.inl:137-146, occupancygrid.cu:351-356): *h_known = the cell

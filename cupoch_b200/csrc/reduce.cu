@@ -64,16 +64,13 @@ static int sum_values(const F &f, size_t n, double *h_out, cudaStream_t s) {
     if (n == 0) return CPHB_OK;
     unsigned grid = (unsigned)((n + RED_BLOCK - 1) / RED_BLOCK);
     if (grid > RED_MAX_BLOCKS) grid = RED_MAX_BLOCKS;
+    cphb_scratch sc(s);
     double *buf = nullptr;
-    int rc = cphb_alloc_async((void **)&buf, sizeof(double) * NV * ((size_t)grid + 1), s);
+    int rc = sc.alloc(&buf, NV * ((size_t)grid + 1));
     if (rc) return rc;
     CPHB_LAUNCH((sum_values_kernel<NV, F>), grid, RED_BLOCK, 0, s, f, n, buf);
     CPHB_LAUNCH(sum_partials_kernel<NV>, 1, 32, 0, s, buf, grid, buf + (size_t)grid * NV);
-    CPHB_CHECK_LAUNCH();
-    CPHB_CUDA(cudaMemcpyAsync(h_out, buf + (size_t)grid * NV, sizeof(double) * NV, cudaMemcpyDeviceToHost, s));
-    CPHB_CUDA(cudaStreamSynchronize(s));
-    cphb_free_async(buf, s);
-    return CPHB_OK;
+    return cphb_read_back(h_out, buf + (size_t)grid * NV, sizeof(double) * NV, s, "sum_values");
 }
 
 // ---------------------------------------------------------------------------------------------------------------------

@@ -95,8 +95,8 @@ static int search_launch(const cphb_index *index, const float *query, const uint
     }
     if (h_count) {
         unsigned long long h = 0;
-        CPHB_CUDA(cudaMemcpyAsync(&h, count, 8, cudaMemcpyDeviceToHost, s));
-        CPHB_CUDA(cudaStreamSynchronize(s));
+        const int rc = cphb_read_back(&h, count, 8, s, "search");
+        if (rc) return rc;
         *h_count = (int64_t)h;
     }
     return CPHB_OK;
@@ -119,17 +119,16 @@ static int search_impl(const cphb_index *index, const float *query, size_t nq, f
     }
     if (h_count) *h_count = 0;
     if (k == 0) return CPHB_OK;
+    cphb_scratch sc(s);
     uint32_t *perm = nullptr;
     unsigned long long *count = nullptr;
     int rc = CPHB_OK;
     if (nq > 32) {
-        rc = cphb_alloc_async((void **)&perm, sizeof(uint32_t) * nq, s);
+        rc = sc.alloc(&perm, nq);
         if (!rc) rc = cphb_hilbert_order_n(query, nq, perm, index->bounds, 1, nq < index->v.n ? nq : (size_t)index->v.n, s);
     }
-    if (!rc && h_count) rc = cphb_alloc_async((void **)&count, 16, s);
+    if (!rc && h_count) rc = sc.alloc(&count, 2);
     if (!rc) rc = search_launch(index, query, perm, nq, r2, k, idx, d2, count, h_count, s);
-    cphb_free_async(perm, s);
-    cphb_free_async(count, s);
     return rc;
 }
 

@@ -296,21 +296,22 @@ extern "C" int cphb_segment_plane(const float *points, size_t n, float distance_
     SegState *st = nullptr;
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
     const size_t Tz = T > 0 ? (size_t)T : 1;
+    cphb_scratch sc(s);
     int rc = CPHB_OK;
     if (T > 0) {
-        rc = cphb_alloc_async((void **)&keys, sizeof(uint32_t) * n, s);
-        if (!rc) rc = cphb_alloc_async((void **)&keys_out, sizeof(uint32_t) * n, s);
-        if (!rc) rc = cphb_alloc_async((void **)&cards, sizeof(uint32_t) * n, s);
-        if (!rc) rc = cphb_alloc_async((void **)&cards_alt, sizeof(uint32_t) * n, s);
-        if (!rc) rc = cphb_alloc_async((void **)&pcnt, sizeof(int) * n_tiles * Tz, s);
-        if (!rc) rc = cphb_alloc_async((void **)&psum, sizeof(double) * n_tiles * Tz, s);
+        rc = sc.alloc(&keys, n);
+        if (!rc) rc = sc.alloc(&keys_out, n);
+        if (!rc) rc = sc.alloc(&cards, n);
+        if (!rc) rc = sc.alloc(&cards_alt, n);
+        if (!rc) rc = sc.alloc(&pcnt, n_tiles * Tz);
+        if (!rc) rc = sc.alloc(&psum, n_tiles * Tz);
     }
-    if (!rc) rc = cphb_alloc_async((void **)&samples, sizeof(int32_t) * 3 * Tz, s);
-    if (!rc) rc = cphb_alloc_async((void **)&planes, sizeof(float4) * Tz, s);
-    if (!rc) rc = cphb_alloc_async((void **)&fr, sizeof(float2) * Tz, s);
-    if (!rc) rc = cphb_alloc_async((void **)&partial, sizeof(double) * 6 * n_tiles, s);
-    if (!rc) rc = cphb_alloc_async((void **)&keep, n, s);
-    if (!rc) rc = cphb_alloc_async((void **)&st, sizeof(SegState), s);
+    if (!rc) rc = sc.alloc(&samples, 3 * Tz);
+    if (!rc) rc = sc.alloc(&planes, Tz);
+    if (!rc) rc = sc.alloc(&fr, Tz);
+    if (!rc) rc = sc.alloc(&partial, 6 * n_tiles);
+    if (!rc) rc = sc.alloc(&keep, n);
+    if (!rc) rc = sc.alloc(&st, 1);
     if (!rc && h_phase_ms) {
         for (int k = 0; k < 4 && !rc; ++k)
             if (cudaEventCreate(&ev[k]) != cudaSuccess) {
@@ -361,13 +362,8 @@ extern "C" int cphb_segment_plane(const float *points, size_t n, float distance_
         }
         if (ev[3]) cudaEventRecord(ev[3], s);
         SegState h;
-        cudaError_t e = cudaGetLastError();
-        if (e == cudaSuccess) e = cudaMemcpyAsync(&h, st, sizeof(h), cudaMemcpyDeviceToHost, s);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-        if (e != cudaSuccess) {
-            cphb_set_error("cphb_segment_plane: %s", cudaGetErrorString(e));
-            rc = CPHB_ERR_CUDA;
-        } else {
+        rc = cphb_read_back(&h, st, sizeof(h), s, "cphb_segment_plane");
+        if (!rc) {
             h_plane[0] = h.plane.x;
             h_plane[1] = h.plane.y;
             h_plane[2] = h.plane.z;
@@ -385,18 +381,7 @@ extern "C" int cphb_segment_plane(const float *points, size_t n, float distance_
             }
         }
     }
-    cphb_free_async(keys, s);
-    cphb_free_async(keys_out, s);
-    cphb_free_async(cards, s);
-    cphb_free_async(cards_alt, s);
-    cphb_free_async(samples, s);
-    cphb_free_async(planes, s);
-    cphb_free_async(fr, s);
-    cphb_free_async(pcnt, s);
-    cphb_free_async(psum, s);
-    cphb_free_async(partial, s);
-    cphb_free_async(keep, s);
-    cphb_free_async(st, s);
+    sc.release();
     cudaStreamSynchronize(s);
     for (int k = 0; k < 4; ++k)
         if (ev[k]) cudaEventDestroy(ev[k]);

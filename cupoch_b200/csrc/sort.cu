@@ -17,13 +17,13 @@ static int sort_pairs(const K *keys_in, K *keys_out, const uint32_t *vals_in, ui
     size_t tmp_bytes = 0;
     CPHB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, keys_in, keys_out, vals_in, vals_out,
                                               (int)n, 0, bits, s));
-    void *tmp = nullptr;
-    int rc = cphb_alloc_async(&tmp, tmp_bytes ? tmp_bytes : 16, s);
+    cphb_scratch sc(s);
+    char *tmp = nullptr;
+    int rc = sc.alloc(&tmp, tmp_bytes ? tmp_bytes : 16);
     if (rc) return rc;
     cudaError_t e = cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, keys_in, keys_out, vals_in, vals_out,
                                                     (int)n, 0, bits, s);
     g_cphb_launches += (bits + 7) / 8 + 1;  // histogram + one onesweep pass per 8 bits
-    cphb_free_async(tmp, s);
     if (e != cudaSuccess) {
         cphb_set_error("cub::DeviceRadixSort::SortPairs: %s", cudaGetErrorString(e));
         return CPHB_ERR_CUDA;

@@ -344,9 +344,10 @@ static int voxel_dense(const float *points, const float *a1, const float *a2, si
                        int a1_is_normal, float *out_p, float *out_a1, float *out_a2, size_t *h_n_out, cudaStream_t s) {
     constexpr int S = dense_stride<A>();
     const unsigned nb = (unsigned)((cells + VD_BLOCK - 1) / VD_BLOCK);
+    cphb_scratch sc(s);
     char *base = nullptr;
     const size_t acc_bytes = cphb_align(sizeof(double) * S * cells, 256);
-    int rc = cphb_alloc_async((void **)&base, acc_bytes + sizeof(unsigned) * ((size_t)nb + 8), s);
+    int rc = sc.alloc(&base, acc_bytes + sizeof(unsigned) * ((size_t)nb + 8));
     if (rc) return rc;
     double *acc = (double *)base;
     unsigned *bc = (unsigned *)(base + acc_bytes), *total = bc + nb;
@@ -358,7 +359,7 @@ static int voxel_dense(const float *points, const float *a1, const float *a2, si
     CPHB_CHECK_LAUNCH();
     unsigned h = 0;
     CPHB_CUDA(cudaMemcpyAsync(&h, total, 4, cudaMemcpyDeviceToHost, s));
-    cphb_free_async(base, s);
+    sc.release();
     CPHB_CUDA(cudaStreamSynchronize(s));
     *h_n_out = h;
     return CPHB_OK;
@@ -442,8 +443,9 @@ static int voxel_down_sample_impl(const float *points, const float *normals, con
     auto take = [&](size_t bytes) { size_t o = off; off = cphb_align(off + bytes, 256); return o; };
     size_t o_keys = take(T * 8), o_ids = take(T * 4), o_dk = take(cap * 8), o_dk2 = take(cap * 8);
     size_t o_di = take(cap * 4), o_ord = take(cap * 4), o_sums = take(cap * 3 * A * 8), o_cnt = take(cap * 4), o_ctr = take(16);
+    cphb_scratch sc(s);
     char *base = nullptr;
-    rc = cphb_alloc_async((void **)&base, off, s);
+    rc = sc.alloc(&base, off);
     if (rc) return rc;
     unsigned long long *keys = (unsigned long long *)(base + o_keys);
     unsigned *ids = (unsigned *)(base + o_ids);
@@ -462,13 +464,12 @@ static int voxel_down_sample_impl(const float *points, const float *normals, con
     if (A == 1) CPHB_LAUNCH(voxel_accum_kernel<1>, gridn, 256, 0, s, points, a1, a2, n, g, keys, ids, mask, sums, counts);
     else if (A == 2) CPHB_LAUNCH(voxel_accum_kernel<2>, gridn, 256, 0, s, points, a1, a2, n, g, keys, ids, mask, sums, counts);
     else CPHB_LAUNCH(voxel_accum_kernel<3>, gridn, 256, 0, s, points, a1, a2, n, g, keys, ids, mask, sums, counts);
-    CPHB_CHECK_LAUNCH();
     unsigned h_cnt = 0;
-    CPHB_CUDA(cudaMemcpyAsync(&h_cnt, counter, 4, cudaMemcpyDeviceToHost, s));
-    CPHB_CUDA(cudaStreamSynchronize(s));
+    rc = cphb_read_back(&h_cnt, counter, 4, s, "cphb_voxel_down_sample");
+    if (rc) return rc;
     const unsigned n_out = h_cnt;
     rc = cphb_sort_pairs_u64((const uint64_t *)dk, (uint64_t *)dk2, di, order, n_out, bx + by + bz, s);
-    if (rc) { cphb_free_async(base, s); return rc; }
+    if (rc) return rc;
     unsigned gridv = (n_out + 255) / 256;
     if (n_out) {
         if (A == 1) CPHB_LAUNCH(voxel_final_kernel<1>, gridv, 256, 0, s, order, n_out, sums, counts, 0, out_points, nullptr, nullptr);
@@ -478,7 +479,7 @@ static int voxel_down_sample_impl(const float *points, const float *normals, con
         else CPHB_LAUNCH(voxel_final_kernel<3>, gridv, 256, 0, s, order, n_out, sums, counts, 1, out_points, out_normals, out_colors);
         CPHB_CHECK_LAUNCH();
     }
-    cphb_free_async(base, s);
+    sc.release();
     CPHB_CUDA(cudaStreamSynchronize(s));
     *h_n_out = n_out;
     return CPHB_OK;

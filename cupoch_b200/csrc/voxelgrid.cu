@@ -133,8 +133,9 @@ extern "C" int cphb_voxel_grid_from_point_cloud(const float *points, const float
     size_t off = 0;
     auto take = [&](size_t bytes) { size_t o = off; off = cphb_align(off + bytes, 256); return o; };
     const size_t o_k = take(n * 8), o_k2 = take(n * 8), o_v = take(n * 4), o_ord = take(n * 4), o_head = take(n), o_st = take(n * 4);
+    cphb_scratch sc(s);
     char *base = nullptr;
-    rc = cphb_alloc_async((void **)&base, off, s);
+    rc = sc.alloc(&base, off);
     if (rc) return rc;
     unsigned long long *keys = (unsigned long long *)(base + o_k), *keys2 = (unsigned long long *)(base + o_k2);
     uint32_t *vals = (uint32_t *)(base + o_v), *order = (uint32_t *)(base + o_ord);
@@ -151,11 +152,9 @@ extern "C" int cphb_voxel_grid_from_point_cloud(const float *points, const float
     if (!rc && n_out) {
         CPHB_LAUNCH(vg_reduce_kernel, (unsigned)((n_out + 255) / 256), 256, 0, s, keys2, order, starts, n_out, n, colors, P, out_keys,
                     out_colors);
-        cudaError_t e = cudaGetLastError();
-        if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-        if (e != cudaSuccess) { cphb_set_error("cphb_voxel_grid_from_point_cloud: %s", cudaGetErrorString(e)); rc = CPHB_ERR_CUDA; }
+        rc = cphb_read_back(nullptr, nullptr, 0, s, "cphb_voxel_grid_from_point_cloud");
     }
-    cphb_free_async(base, s);
+    sc.release();
     cudaStreamSynchronize(s);
     if (!rc) *h_n_out = n_out;
     return rc;

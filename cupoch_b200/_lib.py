@@ -103,6 +103,13 @@ _SIGNATURES = {
     "cphb_gaussian_filter": (C.c_int, [_P, _P, _P, C.c_size_t, C.c_float, C.c_float, C.c_int, _P, _P, _P,
                                        C.POINTER(C.c_size_t), _P]),
     "cphb_select_by_index": (C.c_int, [_P, _P, _P, C.c_size_t, _P, C.c_size_t, _P, _P, _P, _P]),
+    "cphb_aabb_point_indices": (C.c_int, [_P, C.c_size_t, _F3, _F3, _P, C.POINTER(C.c_size_t), _P]),
+    "cphb_obb_point_indices": (C.c_int, [_P, C.c_size_t, _F3, _P, C.POINTER(C.c_size_t), _P]),
+    "cphb_finite_point_indices": (C.c_int, [_P, C.c_size_t, C.c_int, C.c_int, _P, C.POINTER(C.c_size_t), _P]),
+    "cphb_oriented_bounding_box": (C.c_int, [_P, C.c_size_t, _F3, _F3, _F3, _P]),
+    "cphb_uniform_down_sample": (C.c_int, [_P, _P, _P, C.c_size_t, C.c_size_t, _P, _P, _P, C.POINTER(C.c_size_t), _P]),
+    "cphb_normalize_normals": (C.c_int, [_P, C.c_size_t, _P]),
+    "cphb_orient_normals": (C.c_int, [_P, C.c_size_t, _F3, _P]),
     "cphb_segment_plane": (C.c_int, [_P, C.c_size_t, C.c_float, C.c_int, C.c_int, _I3, _F3, _P, C.POINTER(C.c_size_t),
                                      _I3, _F3, _F3, _P]),
     "cphb_farthest_point_down_sample": (C.c_int, [_P, C.c_size_t, C.c_size_t, _P, _P, _P]),

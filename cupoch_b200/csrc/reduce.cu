@@ -236,8 +236,9 @@ extern "C" int cphb_kabsch_weighted(const float *model, const float *target, con
 }
 
 // one-sided Jacobi SVD (double) on the host -- the same algorithm as svd3 in icp_solve.cuh (stands in for
-// Eigen::JacobiSVD<Matrix3f>; R = V diag(1,1,det(UV)) U^T is unique whatever the SVD's sign / ordering conventions)
-static void host_svd3(const double *A, double *U, double *sv, double *V) {
+// Eigen::JacobiSVD<Matrix3f>; R = V diag(1,1,det(UV)) U^T is unique whatever the SVD's sign / ordering conventions).
+// Also the symmetric eigensolver of OrientedBoundingBox::CreateFromPoints (crop.cu).
+void cphb_host_svd3(const double *A, double *U, double *sv, double *V) {
     double B[9];
     for (int i = 0; i < 9; ++i) { B[i] = A[i]; V[i] = (i % 4 == 0) ? 1.0 : 0.0; }
     for (int sweep = 0; sweep < 60; ++sweep) {
@@ -283,7 +284,7 @@ static void host_svd3(const double *A, double *U, double *sv, double *V) {
 }
 void cphb_kabsch_rotation_from_h(const double H[9], double R[9]) {
     double U[9], sv[3], V[9], UV[9];
-    host_svd3(H, U, sv, V);
+    cphb_host_svd3(H, U, sv, V);
     for (int i = 0; i < 3; ++i)
         for (int j = 0; j < 3; ++j) UV[3 * i + j] = U[3 * i] * V[j] + U[3 * i + 1] * V[3 + j] + U[3 * i + 2] * V[6 + j];
     double dd = UV[0] * (UV[4] * UV[8] - UV[5] * UV[7]) - UV[1] * (UV[3] * UV[8] - UV[5] * UV[6]) +

@@ -1,4 +1,4 @@
-"""cupoch.geometry mirror (hot-path subset): PointCloud, KDTreeFlann, KDTreeSearchParam*.
+"""cupoch.geometry mirror (hot-path subset): PointCloud, the bounding boxes, KDTreeFlann, KDTreeSearchParam*.
 
 Names, argument meaning and error behaviour follow src/python/cupoch_pybind/geometry/
 pointcloud.cpp and kdtree_flann.cpp; computation goes through the C ABI only.
@@ -328,6 +328,252 @@ class PointCloud:
         _lib.check(_lib.lib().cphb_estimate_normals(self._points.ptr, n, knn, radius, max_nn, out.ptr, None))
         self._normals = out
         return True
+
+    # -- bounding boxes and cleanup (SURVEY 8f rank 10) ----------------------
+    def get_axis_aligned_bounding_box(self):
+        """GetAxisAlignedBoundingBox: the min / max bound box (the zero box for an empty cloud)"""
+        return AxisAlignedBoundingBox(*self._bounds())
+
+    def get_oriented_bounding_box(self):
+        """GetOrientedBoundingBox (boundingvolume.cu:219-269): PCA box; see cphb_oriented_bounding_box"""
+        return OrientedBoundingBox.create_from_points(self._points)
+
+    def _select(self, fn, *args):
+        """(cloud of the rows a cphb_*_point_indices call keeps, their count)"""
+        n = len(self)
+        if n == 0:
+            return PointCloud(), 0
+        d_idx = DeviceArray((n,), np.int32)
+        m = C.c_size_t(0)
+        _lib.check(fn(self._points.ptr, n, *args, d_idx.ptr, C.byref(m), None))
+        return self._filtered(d_idx, m.value)[0], m.value
+
+    def crop(self, bounding_box):
+        """Crop(AxisAlignedBoundingBox | OrientedBoundingBox) (pointcloud.cu:340-356): the rows inside the box, with their
+        normals and colours.  An empty box (volume <= 0) is logged and the crop still runs, as in the reference."""
+        if not isinstance(bounding_box, (AxisAlignedBoundingBox, OrientedBoundingBox)):
+            raise TypeError("crop() takes an AxisAlignedBoundingBox or an OrientedBoundingBox")
+        if bounding_box.is_empty():
+            print("[cupoch_b200][error] [CropPointCloud] AxisAlignedBoundingBox either has zeros size, or has wrong "
+                  "bounds.", file=sys.stderr)
+        if isinstance(bounding_box, AxisAlignedBoundingBox):
+            lo, hi = bounding_box._f3s()
+            return self._select(_lib.lib().cphb_aabb_point_indices, lo, hi)[0]
+        return self._select(_lib.lib().cphb_obb_point_indices, bounding_box._box24())[0]
+
+    def pass_through_filter(self, axis_no, min_bound, max_bound):
+        """PassThroughFilter (pointcloud.cu:436-460): the rows with min_bound <= p[axis_no] <= max_bound (NaN kept).
+        axis_no outside 0..2 is logged and gives an empty cloud.  Covariances survive only when no row is removed (the
+        reference copies the whole cloud and compacts points, normals and colours)."""
+        axis_no = int(axis_no)
+        if not 0 <= axis_no < 3:
+            print("[cupoch_b200][error] [PassThroughFilter] Illegal input parameters, axis_no must be 0, 1 or 2.",
+                  file=sys.stderr)
+            return PointCloud()
+        lo, hi = [-np.inf] * 3, [np.inf] * 3
+        lo[axis_no], hi[axis_no] = float(min_bound), float(max_bound)
+        out, m = self._select(_lib.lib().cphb_aabb_point_indices, (C.c_float * 3)(*lo), (C.c_float * 3)(*hi))
+        if m == len(self) and self.has_covariances():
+            out._covariances = self.clone()._covariances
+        return out
+
+    def remove_none_finite_points(self, remove_nan=True, remove_infinite=True):
+        """RemoveNoneFinitePoints (pointcloud.cu:359-385), in place: points, normals and colours are compacted; when rows
+        are removed the covariances no longer match the points and are dropped (has_covariances() becomes false)."""
+        n = len(self)
+        out, m = self._select(_lib.lib().cphb_finite_point_indices, int(bool(remove_nan)), int(bool(remove_infinite)))
+        if m != n:
+            hn, hc = self.has_normals(), self.has_colors()
+            self._points = out._points if m else DeviceArray((0, 3), np.float32)
+            if hn:
+                self._normals = out._normals if m else DeviceArray((0, 3), np.float32)
+            if hc:
+                self._colors = out._colors if m else DeviceArray((0, 3), np.float32)
+            self._covariances = self._color_gradient = None
+        return self
+
+    def uniform_down_sample(self, every_k_points):
+        """UniformDownSample (down_sample.cu:275-300): rows 0, k, 2k, ... -- n // k of them (the reference sizes its
+        output so but copies one more row when k does not divide n).  k == 0 is logged and gives an empty cloud."""
+        k = int(every_k_points)
+        if k <= 0:
+            print("[cupoch_b200][error] [UniformDownSample] Illegal sample rate.", file=sys.stderr)
+            return PointCloud()
+        out = PointCloud()
+        n = len(self)
+        m = n // k
+        if m == 0:
+            return out
+        hn, hc = self.has_normals(), self.has_colors()
+        op = DeviceArray((m, 3), np.float32)
+        on = DeviceArray((m, 3), np.float32) if hn else None
+        oc = DeviceArray((m, 3), np.float32) if hc else None
+        got = C.c_size_t(0)
+        _lib.check(_lib.lib().cphb_uniform_down_sample(
+            self._points.ptr, self._normals.ptr if hn else None, self._colors.ptr if hc else None, n, k, op.ptr,
+            on.ptr if hn else None, oc.ptr if hc else None, C.byref(got), None))
+        _lib.check(_lib.lib().cphb_stream_synchronize(None))
+        out._points, out._normals, out._colors = op, on, oc
+        return out
+
+    def normalize_normals(self):
+        """NormalizeNormals (pointcloud.cu:282-285), in place: every non-zero normal divided by its length"""
+        if self._normals is not None and len(self._normals):
+            _lib.check(_lib.lib().cphb_normalize_normals(self._normals.ptr, len(self._normals), None))
+            _lib.check(_lib.lib().cphb_stream_synchronize(None))
+        return self
+
+    def orient_normals_to_align_with_direction(self, orientation_reference=(0.0, 0.0, 1.0)):
+        """OrientNormalsToAlignWithDirection (estimate_normals.cu:129-141), in place: a zero normal becomes the
+        reference, a normal pointing away from it (n . ref < 0) is negated.  No normals: warns, returns False."""
+        if not self.has_normals():
+            print("[cupoch_b200][warning] [OrientNormalsToAlignWithDirection] No normals in the PointCloud. Call "
+                  "EstimateNormals() first.", file=sys.stderr)
+            return False
+        ref = (C.c_float * 3)(*[float(x) for x in np.asarray(orientation_reference, np.float32).reshape(3)])
+        _lib.check(_lib.lib().cphb_orient_normals(self._normals.ptr, len(self), ref, None))
+        _lib.check(_lib.lib().cphb_stream_synchronize(None))
+        return True
+
+
+def _v3(v):
+    return np.asarray(v, np.float32).reshape(3).copy()
+
+
+class AxisAlignedBoundingBox:
+    """geometry::AxisAlignedBoundingBox<3> (boundingvolume.h:141-232; pybind boundingvolume.cpp): min_bound, max_bound
+    and color are plain float32[3] attributes."""
+
+    def __init__(self, min_bound=(0.0, 0.0, 0.0), max_bound=(0.0, 0.0, 0.0)):
+        self.min_bound, self.max_bound = _v3(min_bound), _v3(max_bound)
+        self.color = np.zeros(3, np.float32)
+
+    def __repr__(self):
+        return "geometry::AxisAlignedBoundingBox with min: (%f, %f, %f), max: (%f, %f, %f)" % (
+            *self.min_bound.tolist(), *self.max_bound.tolist())
+
+    def get_min_bound(self):
+        return self.min_bound.copy()
+
+    def get_max_bound(self):
+        return self.max_bound.copy()
+
+    def get_center(self):
+        return ((self.min_bound + self.max_bound) * np.float32(0.5)).astype(np.float32)
+
+    def get_extent(self):
+        return (self.max_bound - self.min_bound).astype(np.float32)
+
+    def get_half_extent(self):
+        return (self.get_extent() * np.float32(0.5)).astype(np.float32)
+
+    def get_max_extent(self):
+        return float(self.get_extent().max())
+
+    def volume(self):
+        e = self.get_extent()
+        return float(e[0] * e[1] * e[2])
+
+    def is_empty(self):
+        return self.volume() <= 0
+
+    def get_axis_aligned_bounding_box(self):
+        return AxisAlignedBoundingBox(self.min_bound, self.max_bound)
+
+    def get_oriented_bounding_box(self):
+        return OrientedBoundingBox.create_from_axis_aligned_bounding_box(self)
+
+    def get_box_points(self):
+        """GetBoxPoints (boundingvolume.cu:388-401) -> float32 [8, 3]"""
+        lo, hi, e = self.min_bound, self.max_bound, self.get_extent()
+        z = np.float32(0)
+        ex, ey, ez = np.array([e[0], z, z]), np.array([z, e[1], z]), np.array([z, z, e[2]])
+        return np.stack([lo, lo + ex, lo + ey, lo + ez, hi, hi - ex, hi - ey, hi - ez]).astype(np.float32)
+
+    def _f3s(self):
+        return (C.c_float * 3)(*self.min_bound.tolist()), (C.c_float * 3)(*self.max_bound.tolist())
+
+    def get_point_indices_within_bounding_box(self, points):
+        """ascending int32 indices (device) of the points inside the box, bounds inclusive; NaN points are kept"""
+        return _point_indices(points, _lib.lib().cphb_aabb_point_indices, *self._f3s())
+
+    @staticmethod
+    def create_from_points(points):
+        """CreateFromPoints (boundingvolume.cu:378-395): the points' min / max bound, the zero box when empty"""
+        return PointCloud(points).get_axis_aligned_bounding_box()
+
+
+class OrientedBoundingBox:
+    """geometry::OrientedBoundingBox (boundingvolume.h:40-139; pybind boundingvolume.cpp): center, R (3x3, columns are
+    the box axes) and extent are plain float32 attributes; color is kept for the reference's interface."""
+
+    def __init__(self, center=(0.0, 0.0, 0.0), R=np.eye(3), extent=(0.0, 0.0, 0.0)):
+        self.center, self.extent = _v3(center), _v3(extent)
+        self.R = np.asarray(R, np.float32).reshape(3, 3).copy()
+        self.color = np.zeros(3, np.float32)
+
+    def __repr__(self):
+        return "geometry::OrientedBoundingBox: center: (%f, %f, %f), extent: %f, %f, %f)" % (
+            *self.center.tolist(), *self.extent.tolist())
+
+    def get_center(self):
+        return self.center.copy()
+
+    def _size(self):
+        return np.abs(self.R.astype(np.float32) @ self.extent.astype(np.float32)).astype(np.float32)
+
+    def get_min_bound(self):
+        return (self.center - np.float32(0.5) * self._size()).astype(np.float32)
+
+    def get_max_bound(self):
+        return (self.center + np.float32(0.5) * self._size()).astype(np.float32)
+
+    def volume(self):
+        return float(self.extent[0] * self.extent[1] * self.extent[2])
+
+    def is_empty(self):
+        return self.volume() <= 0
+
+    def get_axis_aligned_bounding_box(self):
+        return AxisAlignedBoundingBox(self.get_min_bound(), self.get_max_bound())
+
+    def get_box_points(self):
+        """GetBoxPoints (boundingvolume.cu:180-194) in float32: axis k = R[:, k] * (extent[k] / 2), the corners
+        center -+ x -+ y -+ z evaluated left to right -> [8, 3]"""
+        c, h = self.center, (self.extent / np.float32(2)).astype(np.float32)
+        x, y, z = self.R[:, 0] * h[0], self.R[:, 1] * h[1], self.R[:, 2] * h[2]
+        return np.stack([c - x - y - z, c + x - y - z, c - x + y - z, c - x - y + z,
+                         c + x + y + z, c - x + y + z, c + x - y + z, c + x + y - z]).astype(np.float32)
+
+    def _box24(self):
+        return (C.c_float * 24)(*self.get_box_points().reshape(-1).tolist())
+
+    def get_point_indices_within_bounding_box(self, points):
+        """ascending int32 indices (device) of the points the six plane tests keep (boundingvolume.cu:38-79,228-244)"""
+        return _point_indices(points, _lib.lib().cphb_obb_point_indices, self._box24())
+
+    @staticmethod
+    def create_from_axis_aligned_bounding_box(aabox):
+        return OrientedBoundingBox(aabox.get_center(), np.eye(3), aabox.get_extent())
+
+    @staticmethod
+    def create_from_points(points):
+        """CreateFromPoints (boundingvolume.cu:219-269): see cphb_oriented_bounding_box.  Empty input: the zero box."""
+        pts = points if isinstance(points, DeviceArray) else Vector3fVector(points)
+        n = 0 if pts is None else len(pts)
+        c, R, e = (C.c_float * 3)(), (C.c_float * 9)(), (C.c_float * 3)()
+        _lib.check(_lib.lib().cphb_oriented_bounding_box(pts.ptr if n else None, n, c, R, e, None))
+        return OrientedBoundingBox(np.array(c, np.float32), np.array(R, np.float32).reshape(3, 3), np.array(e, np.float32))
+
+
+def _point_indices(points, fn, *args):
+    pts = points if isinstance(points, DeviceArray) else Vector3fVector(points)
+    n = 0 if pts is None else len(pts)
+    d_idx = DeviceArray((n,), np.int32)
+    m = C.c_size_t(0)
+    if n:
+        _lib.check(fn(pts.ptr, n, *args, d_idx.ptr, C.byref(m), None))
+    return DeviceArray((m.value,), np.int32, ptr=d_idx.ptr, base=d_idx)
 
 
 class VoxelGrid:

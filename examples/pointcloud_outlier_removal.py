@@ -11,6 +11,9 @@ if __name__ == "__main__":
     pcd = cph.geometry.PointCloud(noisy)
     print("Downsample the point cloud with a voxel of 0.005")
     voxel_down_pcd = pcd.voxel_down_sample(voxel_size=0.005)
+    print("Every 5th point of the point cloud")
+    uni_down_pcd = pcd.uniform_down_sample(every_k_points=5)
+    print("kept", len(uni_down_pcd), "of", len(pcd))
     print("Statistical outlier removal")
     cl, ind = voxel_down_pcd.remove_statistical_outlier(nb_neighbors=20, std_ratio=2.0)
     print("kept", len(cl), "of", len(voxel_down_pcd))

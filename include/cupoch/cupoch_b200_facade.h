@@ -14,6 +14,8 @@
 #include <cstring>
 #include <memory>
 #include <stdexcept>
+#include <algorithm>
+#include <array>
 #include <tuple>
 #include <utility>
 #include <limits>
@@ -69,6 +71,11 @@ struct Matrix3f {  // column-major like Eigen's default
     Matrix3f() : m{0, 0, 0, 0, 0, 0, 0, 0, 0} {}
     float &operator()(int r, int c) { return m[3 * c + r]; }
     float operator()(int r, int c) const { return m[3 * c + r]; }
+    static Matrix3f Identity() {
+        Matrix3f I;
+        I.m[0] = I.m[4] = I.m[8] = 1.f;
+        return I;
+    }
 };
 struct Matrix4f {  // column-major
     float m[16];
@@ -284,6 +291,154 @@ private:
 
 // --------------------------------------------------------------------------- geometry
 namespace geometry {
+namespace detail {
+inline Eigen::Vector3f v3(float x, float y, float z) { return Eigen::Vector3f(x, y, z); }
+// ascending int32 indices from a cphb_*_point_indices call, widened to the reference's size_t
+template <class F>
+inline utility::device_vector<size_t> point_indices(const utility::device_vector<Eigen::Vector3f> &points, F call) {
+    utility::device_vector<size_t> out;
+    const size_t n = points.size();
+    if (n == 0) return out;
+    utility::device_vector<int32_t> idx(n);
+    size_t m = 0;
+    utility::check(call(reinterpret_cast<const float *>(points.data()), n, idx.data(), &m));
+    idx.resize(m);
+    std::vector<int32_t> h32 = idx.to_host();
+    out = std::vector<size_t>(h32.begin(), h32.end());
+    return out;
+}
+}  // namespace detail
+
+template <int Dim>
+class AxisAlignedBoundingBox;
+
+/// geometry::OrientedBoundingBox (boundingvolume.h:40-139): center_, R_ (columns are the box axes), extent_.
+class OrientedBoundingBox {
+public:
+    OrientedBoundingBox() : center_(0, 0, 0), R_(Eigen::Matrix3f::Identity()), extent_(0, 0, 0), color_(0, 0, 0) {}
+    OrientedBoundingBox(const Eigen::Vector3f &center, const Eigen::Matrix3f &R, const Eigen::Vector3f &extent)
+        : center_(center), R_(R), extent_(extent), color_(0, 0, 0) {}
+    float Volume() const { return extent_(0) * extent_(1) * extent_(2); }  // boundingvolume.cu:176-178
+    bool IsEmpty() const { return Volume() <= 0; }
+    Eigen::Vector3f GetCenter() const { return center_; }
+    Eigen::Vector3f GetMinBound() const { return bound(-1.f); }  // boundingvolume.cu:115-123: center -+ 0.5 |R extent|
+    Eigen::Vector3f GetMaxBound() const { return bound(1.f); }
+    /// GetBoxPoints (boundingvolume.cu:180-194): axis k = R.col(k) * (extent(k) / 2), corners center -+ x -+ y -+ z
+    std::array<Eigen::Vector3f, 8> GetBoxPoints() const {
+        float ax[3][3];
+        for (int k = 0; k < 3; ++k)
+            for (int r = 0; r < 3; ++r) ax[k][r] = R_(r, k) * (extent_(k) / 2);
+        static const int S[8][3] = {{-1, -1, -1}, {1, -1, -1}, {-1, 1, -1}, {-1, -1, 1}, {1, 1, 1}, {-1, 1, 1}, {1, -1, 1}, {1, 1, -1}};
+        std::array<Eigen::Vector3f, 8> p;
+        for (int i = 0; i < 8; ++i) {
+            float v[3];
+            for (int r = 0; r < 3; ++r) {
+                v[r] = center_(r);
+                for (int k = 0; k < 3; ++k) v[r] = S[i][k] > 0 ? v[r] + ax[k][r] : v[r] - ax[k][r];
+            }
+            p[i] = detail::v3(v[0], v[1], v[2]);
+        }
+        return p;
+    }
+    /// GetPointIndicesWithinBoundingBox (boundingvolume.cu:228-244): the six determinant plane tests (cphb_obb_point_indices)
+    utility::device_vector<size_t> GetPointIndicesWithinBoundingBox(const utility::device_vector<Eigen::Vector3f> &points) const {
+        const auto bp = GetBoxPoints();
+        float box[24];
+        for (int i = 0; i < 8; ++i)
+            for (int r = 0; r < 3; ++r) box[3 * i + r] = bp[i](r);
+        return detail::point_indices(points, [&](const float *p, size_t n, int32_t *idx, size_t *m) {
+            return cphb_obb_point_indices(p, n, box, idx, m, nullptr);
+        });
+    }
+    static OrientedBoundingBox CreateFromAxisAlignedBoundingBox(const AxisAlignedBoundingBox<3> &aabox);
+    /// CreateFromPoints (boundingvolume.cu:219-269; cphb_oriented_bounding_box): PCA axes by descending eigenvalue, each
+    /// signed so its largest-magnitude component is positive; the zero box with R = I for no points.
+    static OrientedBoundingBox CreateFromPoints(const utility::device_vector<Eigen::Vector3f> &points) {
+        float c[3], R[9], e[3];
+        utility::check(cphb_oriented_bounding_box(reinterpret_cast<const float *>(points.data()), points.size(), c, R, e, nullptr));
+        Eigen::Matrix3f M;
+        for (int r = 0; r < 3; ++r)
+            for (int k = 0; k < 3; ++k) M(r, k) = R[3 * r + k];
+        return OrientedBoundingBox(detail::v3(c[0], c[1], c[2]), M, detail::v3(e[0], e[1], e[2]));
+    }
+
+public:
+    Eigen::Vector3f center_;
+    Eigen::Matrix3f R_;
+    Eigen::Vector3f extent_;
+    Eigen::Vector3f color_;
+
+private:
+    Eigen::Vector3f bound(float sign) const {
+        float v[3];
+        for (int r = 0; r < 3; ++r) {
+            const float size = std::fabs(R_(r, 0) * extent_(0) + R_(r, 1) * extent_(1) + R_(r, 2) * extent_(2));
+            v[r] = center_(r) + sign * 0.5f * size;
+        }
+        return detail::v3(v[0], v[1], v[2]);
+    }
+};
+
+/// geometry::AxisAlignedBoundingBox<3> (boundingvolume.h:141-232): min_bound_, max_bound_.
+template <>
+class AxisAlignedBoundingBox<3> {
+public:
+    AxisAlignedBoundingBox() : min_bound_(0, 0, 0), max_bound_(0, 0, 0), color_(0, 0, 0) {}
+    AxisAlignedBoundingBox(const Eigen::Vector3f &min_bound, const Eigen::Vector3f &max_bound)
+        : min_bound_(min_bound), max_bound_(max_bound), color_(0, 0, 0) {}
+    Eigen::Vector3f GetMinBound() const { return min_bound_; }
+    Eigen::Vector3f GetMaxBound() const { return max_bound_; }
+    Eigen::Vector3f GetCenter() const {  // boundingvolume.cu:293-296
+        return detail::v3((min_bound_(0) + max_bound_(0)) * 0.5f, (min_bound_(1) + max_bound_(1)) * 0.5f,
+                          (min_bound_(2) + max_bound_(2)) * 0.5f);
+    }
+    Eigen::Vector3f GetExtent() const {
+        return detail::v3(max_bound_(0) - min_bound_(0), max_bound_(1) - min_bound_(1), max_bound_(2) - min_bound_(2));
+    }
+    Eigen::Vector3f GetHalfExtent() const {
+        const Eigen::Vector3f e = GetExtent();
+        return detail::v3(e(0) * 0.5f, e(1) * 0.5f, e(2) * 0.5f);
+    }
+    float GetMaxExtent() const {
+        const Eigen::Vector3f e = GetExtent();
+        return std::max(e(0), std::max(e(1), e(2)));
+    }
+    float Volume() const {
+        const Eigen::Vector3f e = GetExtent();
+        return e(0) * e(1) * e(2);
+    }
+    bool IsEmpty() const { return Volume() <= 0; }
+    /// GetBoxPoints (boundingvolume.cu:388-401)
+    std::array<Eigen::Vector3f, 8> GetBoxPoints() const {
+        const Eigen::Vector3f e = GetExtent(), &lo = min_bound_, &hi = max_bound_;
+        return {lo, detail::v3(lo(0) + e(0), lo(1) + 0.f, lo(2) + 0.f), detail::v3(lo(0) + 0.f, lo(1) + e(1), lo(2) + 0.f),
+                detail::v3(lo(0) + 0.f, lo(1) + 0.f, lo(2) + e(2)), hi, detail::v3(hi(0) - e(0), hi(1) - 0.f, hi(2) - 0.f),
+                detail::v3(hi(0) - 0.f, hi(1) - e(1), hi(2) - 0.f), detail::v3(hi(0) - 0.f, hi(1) - 0.f, hi(2) - e(2))};
+    }
+    /// GetPointIndicesWithinBoundingBox (boundingvolume.cu:413-425): inclusive bounds, NaN points kept
+    utility::device_vector<size_t> GetPointIndicesWithinBoundingBox(const utility::device_vector<Eigen::Vector3f> &points) const {
+        const float lo[3] = {min_bound_(0), min_bound_(1), min_bound_(2)}, hi[3] = {max_bound_(0), max_bound_(1), max_bound_(2)};
+        return detail::point_indices(points, [&](const float *p, size_t n, int32_t *idx, size_t *m) {
+            return cphb_aabb_point_indices(p, n, lo, hi, idx, m, nullptr);
+        });
+    }
+    OrientedBoundingBox GetOrientedBoundingBox() const { return OrientedBoundingBox::CreateFromAxisAlignedBoundingBox(*this); }
+    /// CreateFromPoints (boundingvolume.cu:378-395): the min / max bound, the zero box for no points
+    static AxisAlignedBoundingBox<3> CreateFromPoints(const utility::device_vector<Eigen::Vector3f> &points) {
+        float mn[3] = {0, 0, 0}, mx[3] = {0, 0, 0};
+        if (!points.empty())
+            utility::check(cphb_min_max_bound(reinterpret_cast<const float *>(points.data()), points.size(), mn, mx, nullptr));
+        return AxisAlignedBoundingBox<3>(detail::v3(mn[0], mn[1], mn[2]), detail::v3(mx[0], mx[1], mx[2]));
+    }
+
+public:
+    Eigen::Vector3f min_bound_, max_bound_, color_;
+};
+
+inline OrientedBoundingBox OrientedBoundingBox::CreateFromAxisAlignedBoundingBox(const AxisAlignedBoundingBox<3> &aabox) {
+    return OrientedBoundingBox(aabox.GetCenter(), Eigen::Matrix3f::Identity(), aabox.GetExtent());  // boundingvolume.cu:209-217
+}
+
 /// geometry::PointCloud (pointcloud.h:43-263), hot-path subset.
 class PointCloud {
 public:
@@ -454,6 +609,92 @@ public:
                                             sigma2, (int)num_max_search_points, fp(out->points_), hn ? fp(out->normals_) : nullptr,
                                             hc ? fp(out->colors_) : nullptr, &m, nullptr));
         return out;
+    }
+    AxisAlignedBoundingBox<3> GetAxisAlignedBoundingBox() const { return AxisAlignedBoundingBox<3>::CreateFromPoints(points_); }
+    OrientedBoundingBox GetOrientedBoundingBox() const { return OrientedBoundingBox::CreateFromPoints(points_); }
+    /// PointCloud::Crop (pointcloud.cu:340-356): an empty box is logged and the crop still runs
+    std::shared_ptr<PointCloud> Crop(const AxisAlignedBoundingBox<3> &bbox) const {
+        if (bbox.IsEmpty()) utility::LogError("[CropPointCloud] AxisAlignedBoundingBox either has zeros size, or has wrong bounds.");
+        return SelectByIndex(bbox.GetPointIndicesWithinBoundingBox(points_));
+    }
+    std::shared_ptr<PointCloud> Crop(const OrientedBoundingBox &bbox) const {
+        if (bbox.IsEmpty()) utility::LogError("[CropPointCloud] AxisAlignedBoundingBox either has zeros size, or has wrong bounds.");
+        return SelectByIndex(bbox.GetPointIndicesWithinBoundingBox(points_));
+    }
+    /// PointCloud::PassThroughFilter (pointcloud.cu:436-460): min_bound <= p(axis_no) <= max_bound (NaN kept); axis_no >= 3
+    /// is logged and gives an empty cloud.  Like the reference's copy-and-compact, the covariances survive only when no row
+    /// is removed.
+    std::shared_ptr<PointCloud> PassThroughFilter(size_t axis_no, float min_bound, float max_bound) {
+        if (axis_no >= 3) {
+            utility::LogError("[PassThroughFilter] Illegal input parameters, axis_no must be 0, 1 or 2.");
+            return std::make_shared<PointCloud>();
+        }
+        float lo[3] = {-INFINITY, -INFINITY, -INFINITY}, hi[3] = {INFINITY, INFINITY, INFINITY};
+        lo[axis_no] = min_bound;
+        hi[axis_no] = max_bound;
+        utility::device_vector<int32_t> kept(points_.size());
+        size_t m = 0;
+        if (!points_.empty())
+            utility::check(cphb_aabb_point_indices(cfp(points_), points_.size(), lo, hi, kept.data(), &m, nullptr));
+        auto out = gather(kept, m);
+        if (m == points_.size() && HasCovariances()) out->covariances_ = covariances_;
+        return out;
+    }
+    /// PointCloud::RemoveNoneFinitePoints (pointcloud.cu:359-385), in place: points, normals and colours are compacted;
+    /// when rows are removed the covariances no longer match and are dropped
+    PointCloud &RemoveNoneFinitePoints(bool remove_nan = true, bool remove_infinite = true) {
+        const size_t n = points_.size();
+        if (n == 0) return *this;
+        utility::device_vector<int32_t> kept(n);
+        size_t m = 0;
+        utility::check(cphb_finite_point_indices(cfp(points_), n, remove_nan, remove_infinite, kept.data(), &m, nullptr));
+        if (m == n) return *this;
+        const bool hn = HasNormals(), hc = HasColors();
+        auto out = gather(kept, m);
+        points_ = std::move(out->points_);
+        if (hn) normals_ = std::move(out->normals_);
+        if (hc) colors_ = std::move(out->colors_);
+        covariances_.clear();
+        color_gradient_.clear();
+        return *this;
+    }
+    /// PointCloud::UniformDownSample (down_sample.cu:275-300): rows 0, k, 2k, ... -- n / k of them; k == 0 is logged and
+    /// gives an empty cloud
+    std::shared_ptr<PointCloud> UniformDownSample(size_t every_k_points) const {
+        auto out = std::make_shared<PointCloud>();
+        if (every_k_points == 0) {
+            utility::LogError("[UniformDownSample] Illegal sample rate.");
+            return out;
+        }
+        const size_t n = points_.size(), m = n / every_k_points;
+        if (m == 0) return out;
+        const bool hn = HasNormals(), hc = HasColors();
+        out->points_.resize(m);
+        if (hn) out->normals_.resize(m);
+        if (hc) out->colors_.resize(m);
+        size_t got = 0;
+        utility::check(cphb_uniform_down_sample(cfp(points_), hn ? cfp(normals_) : nullptr, hc ? cfp(colors_) : nullptr, n,
+                                                every_k_points, fp(out->points_), hn ? fp(out->normals_) : nullptr,
+                                                hc ? fp(out->colors_) : nullptr, &got, nullptr));
+        utility::check(cphb_stream_synchronize(nullptr));
+        return out;
+    }
+    /// PointCloud::NormalizeNormals (pointcloud.cu:282-285), in place
+    PointCloud &NormalizeNormals() {
+        if (!normals_.empty()) utility::check(cphb_normalize_normals(fp(normals_), normals_.size(), nullptr));
+        utility::check(cphb_stream_synchronize(nullptr));
+        return *this;
+    }
+    /// PointCloud::OrientNormalsToAlignWithDirection (estimate_normals.cu:129-141), in place
+    bool OrientNormalsToAlignWithDirection(const Eigen::Vector3f &orientation_reference = Eigen::Vector3f(0.f, 0.f, 1.f)) {
+        if (!HasNormals()) {
+            utility::LogWarning("[OrientNormalsToAlignWithDirection] No normals in the PointCloud. Call EstimateNormals() first.");
+            return false;
+        }
+        const float r[3] = {orientation_reference(0), orientation_reference(1), orientation_reference(2)};
+        utility::check(cphb_orient_normals(fp(normals_), normals_.size(), r, nullptr));
+        utility::check(cphb_stream_synchronize(nullptr));
+        return true;
     }
     cphb_cloud view() const {
         cphb_cloud c;

@@ -190,6 +190,37 @@ int cphb_gaussian_filter(const float *points, const float *normals, const float 
 int cphb_select_by_index(const float *points, const float *normals, const float *colors, size_t n,
                          const int32_t *indices, size_t n_indices, float *out_points, float *out_normals,
                          float *out_colors, void *stream);
+/* Region selection (boundingvolume.cu:38-101,221-244,413-425; pointcloud.cu:38-53,105-121): indices_out (device, n
+ * int32) receives the ascending indices of the points the test keeps, *h_n_out their number (synchronises).
+ *   aabb:   kept unless p[a] < h_min[a] or p[a] > h_max[a] for some axis a (inclusive; a NaN coordinate is kept).
+ *           PassThroughFilter(axis, lo, hi) is this test with lo / hi on that axis and -inf / +inf on the others.
+ *   obb:    h_box_points = OrientedBoundingBox::GetBoxPoints() (8 x xyz); the reference's six determinant plane tests,
+ *           either sign pattern (DESIGN.md fixes the determinant's expansion order).
+ *   finite: removed when (remove_nan and a coordinate is NaN) or (remove_infinite and a coordinate is infinite).
+ * n > 2^31-1: CPHB_ERR_INVALID. */
+int cphb_aabb_point_indices(const float *points, size_t n, const float h_min[3], const float h_max[3],
+                            int32_t *indices_out, size_t *h_n_out, void *stream);
+int cphb_obb_point_indices(const float *points, size_t n, const float h_box_points[24], int32_t *indices_out,
+                           size_t *h_n_out, void *stream);
+int cphb_finite_point_indices(const float *points, size_t n, int remove_nan, int remove_infinite, int32_t *indices_out,
+                              size_t *h_n_out, void *stream);
+/* OrientedBoundingBox::CreateFromPoints (boundingvolume.cu:219-269): mean and centred covariance summed in double in
+ * the tiled order of DESIGN.md's arithmetic contract, a double symmetric eigensolve, axes sorted by descending
+ * eigenvalue, each axis signed so its largest-magnitude component (the first among equal ones) is positive; the
+ * extent and centre come from the float32 bounds of the points transformed by [R^T | -R^T mean].  h_R is row-major.
+ * n == 0: the zero box with R = I.  Synchronises. */
+int cphb_oriented_bounding_box(const float *points, size_t n, float h_center[3], float h_R[9], float h_extent[3],
+                               void *stream);
+/* PointCloud::UniformDownSample (down_sample.cu:275-300): out row t = in row t * every_k for t < n / every_k (rounded
+ * down; *h_n_out gets that count).  normals / colors in and out may be NULL (together).  every_k == 0:
+ * CPHB_ERR_INVALID.  Asynchronous. */
+int cphb_uniform_down_sample(const float *points, const float *normals, const float *colors, size_t n, size_t every_k,
+                             float *out_points, float *out_normals, float *out_colors, size_t *h_n_out, void *stream);
+/* PointCloud::NormalizeNormals (pointcloud.cu:282-285): in place, n /= sqrt(|n|^2) where |n|^2 > 0.  Asynchronous. */
+int cphb_normalize_normals(float *normals, size_t n, void *stream);
+/* PointCloud::OrientNormalsToAlignWithDirection (estimate_normals.cu:66-78,129-141): in place, a zero normal becomes
+ * h_reference, a normal with n . h_reference < 0 is negated.  Asynchronous. */
+int cphb_orient_normals(float *normals, size_t n, const float h_reference[3], void *stream);
 /* PointCloud::SegmentPlane (segmentation.cu:187-267): RANSAC plane [a,b,c,d] with |dot3(abc, p) + d| <
  * distance_threshold inliers.  h_seeds (host, num_iterations ints) are the seeds the reference draws with rand(),
  * one per iteration; iteration t samples d_cards[0..2] after a stable sort of d_cards by thrust's random_functor(

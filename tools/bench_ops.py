@@ -32,7 +32,10 @@ def main():
                     help="instead: time geometry::keypoint::ComputeISSKeypoints (defaults, automatic radii) at N = 1 M, 10 M")
     ap.add_argument("--shot", action="store_true",
                     help="instead: time registration::ComputeSHOTFeature (Radius(r, 100), r = 5 spacings) at N = 100 k, 1 M")
-    ap.add_argument("--out", default=None, help="--shot: also write the JSON object to this file")
+    ap.add_argument("--crop", action="store_true",
+                    help="instead: time crop / pass_through_filter / remove_none_finite_points / uniform_down_sample / "
+                         "get_oriented_bounding_box on the 10 M config-3 cloud with normals and colours")
+    ap.add_argument("--out", default=None, help="--shot, --crop: also write the JSON object to this file")
     ap.add_argument("--edt", action="store_true",
                     help="instead: time geometry::DistanceTransform::ComputeEDT at 256^3 and 512^3 and GetDistances of 10 M points")
     args = ap.parse_args()
@@ -46,6 +49,8 @@ def main():
         return iss(args.reps)
     if args.shot:
         return shot(args.reps, args.out)
+    if args.crop:
+        return crop(args.reps, args.points, args.out)
     import cupoch_b200 as cph
     from cupoch_b200 import _lib
     from cupoch_b200.testing import datagen
@@ -598,6 +603,108 @@ def edt_cell_codes(r):
     """x << 20 | y << 10 | z of every cell of an r^3 grid (a site is its own nearest site)"""
     g = np.arange(r, dtype=np.uint32)
     return (g[:, None, None] << 20) | (g[None, :, None] << 10) | g[None, None, :]
+
+
+H100_HBM_BYTES_PER_S = 3.35e12  # NVIDIA's H100 SXM data sheet (700 W); a share of it is not a claim that it was reached
+
+
+def crop_bytes_model(op, n, m):
+    """least HBM traffic of each call on a cloud of n points with normals and colours (three float32[3] arrays), m rows
+    out: a selection reads 12 B of xyz and writes 1 B of flag per point, then reads and writes the m gathered rows
+    (3 x 12 B each way); the uniform stride is the gather alone; the OBB reads the points for the mean, the moments and
+    the transform copy, writes and rereads the copy, and reads the transformed copy for the bounds."""
+    if op == "uniform_down_sample(5)":
+        return 72 * m
+    if op == "get_oriented_bounding_box":
+        return 12 * n * 6
+    return 13 * n + 72 * m
+
+
+def crop(reps, n, out=None):
+    """The region-selection and cleanup calls on the config-3 cloud (datagen.uniform_cube(N, 21) in [0,4)x[0,4)x[0,1),
+    unit normals, colours): CUDA-event time of the whole Python call, which ends in a host synchronise, after a cache
+    flush; each kernel's device time from torch.profiler in a separate profiled call; the bytes model above over the
+    summed kernel time as a share of the data-sheet bandwidth.  remove_none_finite_points works in place, so every rep
+    runs on a fresh copy (made outside the timed window) with 1 % of the rows NaN."""
+    import subprocess
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    import cupoch_b200 as cph
+    from cupoch_b200 import _lib
+    from cupoch_b200.testing import datagen
+    from cupoch_b200.utility import DeviceArray
+    L = _lib.lib()
+    gpu = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                         capture_output=True, text=True).stdout.strip()
+    G = cph.geometry
+    pts = datagen.uniform_cube(n, 21, hi=(4, 4, 1))
+    pc = G.PointCloud(pts)
+    pc.normals = datagen.unit_normals(n, 22)
+    pc.colors = datagen.uniform_cube(n, 23)
+    bad = pts.copy()
+    bad[np.random.default_rng(24).choice(n, n // 100, replace=False), 1] = np.nan
+    pc_bad = G.PointCloud(bad)
+    pc_bad.normals, pc_bad.colors = pc.normals, pc.colors
+    c, s_ = np.cos(np.pi / 6), np.sin(np.pi / 6)
+    obb = G.OrientedBoundingBox((2, 2, 0.5), [[c, -s_, 0], [s_, c, 0], [0, 0, 1]], (2.6, 2.6, 1.2))
+    fresh = {}
+
+    def nonfinite():
+        return fresh.pop("pc").remove_none_finite_points()
+
+    def prep_nonfinite():
+        fresh["pc"] = pc_bad.clone()
+
+    calls = [("crop(AABB [0,2]x[0,4]x[0,1])", lambda: pc.crop(G.AxisAlignedBoundingBox((0, 0, 0), (2, 4, 1))), None),
+             ("crop(OBB 30 deg about z)", lambda: pc.crop(obb), None),
+             ("pass_through_filter(2, 0.0, 0.5)", lambda: pc.pass_through_filter(2, 0.0, 0.5), None),
+             ("remove_none_finite_points(1 % NaN)", nonfinite, prep_nonfinite),
+             ("uniform_down_sample(5)", lambda: pc.uniform_down_sample(5), None),
+             ("get_oriented_bounding_box", lambda: pc.get_oriented_bounding_box(), None)]
+    flush = DeviceArray((256 << 20,), np.uint8)
+    ev = [L.cphb_event_create() for _ in range(2)]
+    rows = []
+    for name, fn, prep in calls:
+        ts = []
+        for r in range(reps + 1):  # the first call warms the allocation pool and the modules
+            if prep:
+                prep()
+            L.cphb_memset(flush.ptr, 0, flush.nbytes, None)
+            L.cphb_stream_synchronize(None)
+            L.cphb_event_record(ev[0], None)
+            res = fn()
+            L.cphb_event_record(ev[1], None)
+            L.cphb_stream_synchronize(None)
+            ms = C.c_float(0)
+            _lib.check(L.cphb_event_elapsed_ms(ev[0], ev[1], C.byref(ms)))
+            if r:
+                ts.append(ms.value)
+        m = len(res) if isinstance(res, G.PointCloud) else 0
+        if prep:
+            prep()
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            fn()
+            torch.cuda.synchronize()
+        kernels = {}
+        for e in prof.key_averages():
+            t = getattr(e, "device_time_total", getattr(e, "cuda_time_total", 0.0)) * 1e-3
+            if t > 0:
+                kernels[e.key] = kernels.get(e.key, 0.0) + t
+        kern_ms = sum(t for k, t in kernels.items() if "Memset" not in k and "Memcpy" not in k)
+        nbytes = crop_bytes_model(name, n, m)
+        rows.append({"op": name, "n": n, "rows_out": m, "call_ms_median": float(np.median(ts)),
+                     "call_ms_min": float(np.min(ts)), "kernel_ms_profiled": kernels, "kernel_ms_sum": kern_ms,
+                     "bytes_model": nbytes,
+                     "share_of_3.35TBps_over_kernel_time": nbytes / (kern_ms * 1e-3) / H100_HBM_BYTES_PER_S if kern_ms else None,
+                     "share_of_3.35TBps_over_call_time": nbytes / (float(np.median(ts)) * 1e-3) / H100_HBM_BYTES_PER_S})
+    obj = {"op": "bounding-box selection and cleanup on the config-3 cloud (uniform_cube(N, 21) in [0,4)x[0,4)x[0,1), "
+                 "normals and colours)", "gpu": gpu, "reps": reps, "rows": rows}
+    line = json.dumps(obj)
+    print(line)
+    if out:
+        with open(out, "w") as f:
+            f.write(line + "\n")
 
 
 if __name__ == "__main__":

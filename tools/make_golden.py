@@ -1,5 +1,6 @@
 #!/usr/bin/env python3
-"""Generate tests/golden/reference_vectors.json (and segment_plane_known.json) from the reference's own unit tests.
+"""Generate tests/golden/reference_vectors.json (and segment_plane_known.json, pointcloud_crop_known.json) from the
+reference's own unit tests.
 
 Run in the development container only (needs /root/reference, which does not
 exist on the GPU box).  It reads
@@ -22,6 +23,7 @@ import numpy as np
 REF = os.environ.get("CUPOCH_REFERENCE", "/root/reference")
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "tests", "golden", "reference_vectors.json")
 OUT_SEG = os.path.join(os.path.dirname(OUT), "segment_plane_known.json")  # kept apart: the vectors above are frozen
+OUT_CROP = os.path.join(os.path.dirname(OUT), "pointcloud_crop_known.json")
 
 
 def read(rel):
@@ -180,6 +182,46 @@ def main():
         json.dump(seg, f)
     print("wrote", os.path.normpath(OUT_SEG), os.path.getsize(OUT_SEG), "bytes")
     print("wrote", os.path.normpath(OUT), os.path.getsize(OUT), "bytes")
+    crop_known(table, pc, g["source"])
+
+
+def crop_known(table, pc, source):
+    """the bounding-box and cleanup known answers (pointcloud.cpp:176-220,264-302,471-533,599-657) -> OUT_CROP"""
+    b = test_body(pc, "PointCloud", "GetOrientedBoundingBox")
+    pat = re.compile(r"(\w+)\.push_back\(\{\s*(-?[\d.]+)\s*,\s*(-?[\d.]+)\s*,\s*(-?[\d.]+)\s*\}\)")
+    rows = {}
+    for var, x, y, z in pat.findall(b):
+        rows.setdefault(var, []).append([float(x), float(y), float(z)])
+    four, eight, box = rows["points"][:4], rows["points"][4:], rows["ref_points"]
+    assert len(four) == 4 and len(eight) == 8 and len(box) == 8
+    assert "Eigen::Vector3f(1.5, 1, 0.5)" in b and "Eigen::Vector3f(3, 2, 1)" in b and "Matrix3f::Identity()" in b
+    out = {"source": source, "tolerance": 1e-4}  # THRESHOLD_1E_4, the default of the reference's ExpectEQ / ExpectLE
+    out["oriented_bounding_box"] = {
+        "points_4": four, "points_8": eight, "center": [1.5, 1.0, 0.5], "extent": [3.0, 2.0, 1.0],
+        "R": [[1.0, 0.0, 0.0], [0.0, 1.0, 0.0], [0.0, 0.0, 1.0]], "box_points": box,
+        "cite": "src/tests/geometry/pointcloud.cpp:176-220 (center, extent and R exact; box points as a sorted set)"}
+    b = test_body(pc, "PointCloud", "NormalizeNormals")
+    out["normalize_normals"] = {"normals": rand_vec3f(table, 20, (0, 0, 0), (1000, 1000, 1000), 0).tolist(),
+                                "ref": pushed_vec3(b, "ref"), "cite": "src/tests/geometry/pointcloud.cpp:264-302"}
+    b = test_body(pc, "PointCloud", "UniformDownSample")
+    out["uniform_down_sample"] = {"points": rand_vec3f(table, 100, (0, 0, 0), (1000, 1000, 1000), 0).tolist(),
+                                  "every_k_points": 4, "ref": pushed_vec3(b, "ref"),
+                                  "cite": "src/tests/geometry/pointcloud.cpp:471-513"}
+    b = test_body(pc, "PointCloud", "CropPointCloud")
+    assert "minBound(200.0, 200.0, 200.0)" in b and "maxBound(800.0, 800.0, 800.0)" in b
+    out["crop"] = {"points": rand_vec3f(table, 100, (0, 0, 0), (1000, 1000, 1000), 0).tolist(),
+                   "min_bound": [200.0] * 3, "max_bound": [800.0] * 3,
+                   "cite": "src/tests/geometry/pointcloud.cpp:515-533 (every kept point lies within the bounds)"}
+    b = test_body(pc, "PointCloud", "OrientNormalsToAlignWithDirection")
+    assert "Vector3f(1.5, 0.5, 3.3)" in b and "EstimateNormals()" in b
+    out["orient_normals"] = {"points": rand_vec3f(table, 40, (0, 0, 0), (1000, 1000, 1000), 0).tolist(), "knn": 30,
+                             "reference": [1.5, 0.5, 3.3], "ref": pushed_vec3(b, "ref"),
+                             "cite": "src/tests/geometry/pointcloud.cpp:599-657 (EstimateNormals with KNN 30 first)"}
+    assert len(out["normalize_normals"]["ref"]) == 20 and len(out["uniform_down_sample"]["ref"]) == 25
+    assert len(out["orient_normals"]["ref"]) == 40
+    with open(OUT_CROP, "w") as f:
+        json.dump(out, f)
+    print("wrote", os.path.normpath(OUT_CROP), os.path.getsize(OUT_CROP), "bytes")
 
 
 if __name__ == "__main__":

@@ -10,11 +10,12 @@ keypoint.compute_iss_keypoints},
 cph.registration.{registration_icp,
 registration_generalized_icp, registration_colored_icp, ICPConvergenceCriteria, TransformationEstimation*
 (user subclasses run the generic loop), RegistrationResult, compute_fpfh_feature, compute_shot_feature, FeatureSHOT, kabsch, kabsch_weighted},
+cph.collision.{compute_intersection, Box, Sphere, Capsule, Cylinder, PrimitiveArray, CollisionResult},
 cph.utility.{Vector3fVector, compute_jtj_jtr, compute_weighted_jtj_jtr}; cupoch_b200.distributed holds the
 multi-GPU orchestration (torch.distributed).  All computation runs in libcupoch_b200.so (hand-written sm_90a CUDA);
 there is no CPU fallback.
 """
-from . import _lib, geometry, registration, utility  # noqa: F401
+from . import _lib, collision, geometry, registration, utility  # noqa: F401
 
 __version__ = "0.1.0"
 

@@ -44,10 +44,22 @@ class OccGridParams(C.Structure):
                 ("prob_miss_log", C.c_float), ("occ_prob_thres_log", C.c_float)]
 
 
+class Primitive(C.Structure):  # cphb_primitive
+    _fields_ = [("type", C.c_int32), ("transform", C.c_float * 16), ("lengths", C.c_float * 3), ("radius", C.c_float),
+                ("height", C.c_float)]
+
+
+class CollOperand(C.Structure):  # cphb_coll_operand
+    _fields_ = [("kind", C.c_int32), ("keys", C.c_void_p), ("n", C.c_size_t), ("voxel_size", C.c_float),
+                ("origin", C.c_float * 3), ("occ", C.c_void_p), ("primitives", C.c_void_p)]
+
+
 _P = C.c_void_p
 _F3 = C.POINTER(C.c_float)
 _I3 = C.POINTER(C.c_int32)
 _SIGNATURES = {
+    "cphb_compute_intersection": (C.c_int, [C.POINTER(CollOperand), C.POINTER(CollOperand), C.c_float, _P, C.c_size_t,
+                                            C.POINTER(C.c_size_t), _P]),
     "cphb_occgrid_default_params": (None, [C.POINTER(OccGridParams)]),
     "cphb_occgrid_create": (C.c_int, [C.c_float, C.c_int, _F3, _P, C.POINTER(_P)]),
     "cphb_occgrid_destroy": (None, [_P]),

@@ -148,6 +148,23 @@ int cphb_nbr_table_release(cphb_nbr_table *t, int rc, cudaStream_t s);
 
 // the grid's voxel size and origin (occgrid.cu), for the DistanceTransform built from it (edt.cu)
 void cphb_occgrid_geometry(const cphb_occgrid *g, float *voxel_size, float origin[3]);
+// what collision.cu reads of a grid (occgrid.cu): the dense log-odds, the resolution, the occupied threshold and the
+// bound box (device u32[6]: min xyz, max xyz grid indices)
+struct cphb_occgrid_view {
+    const float *prob;
+    const unsigned *bounds;
+    int res;
+    float thres;
+};
+void cphb_occgrid_view_of(const cphb_occgrid *g, cphb_occgrid_view *v);
+// the Extract{Known,Free,Occupied}Voxels predicates (occupancygrid.cu:380-408), which = 0 / 1 / 2: the one definition
+// occgrid.cu's extract and collision.cu's occupied cells (which = 2) share
+__host__ __device__ __forceinline__ bool cphb_occ_keep(float p, float thres, int which) {
+    bool k = !(p != p);
+    if (which == 1) k = k && p <= thres;
+    if (which == 2) k = k && p > thres;
+    return k;
+}
 
 // index.cu internals reused by icp.cu (Hilbert-ordering of the source)
 // perm_out[pos] = original index of the pos-th point along the Hilbert curve.

@@ -231,10 +231,7 @@ __global__ void __launch_bounds__(256) occ_extract_flag_kernel(const float *__re
     if (i >= (size_t)dx * dy * dz) return;
     const int x = (int)(i / ((size_t)dy * dz)), yz = (int)(i % ((size_t)dy * dz));
     const float p = prob[occ_index_of(x0 + x, y0 + yz / dz, z0 + yz % dz, res)];
-    bool k = !(p != p);
-    if (which == 1) k = k && p <= thres;
-    if (which == 2) k = k && p > thres;
-    keep[i] = k ? 1 : 0;
+    keep[i] = cphb_occ_keep(p, thres, which) ? 1 : 0;
 }
 __global__ void __launch_bounds__(256) occ_extract_write_kernel(const float *__restrict__ prob, const unsigned *__restrict__ idx_bits, int res,
                                                                 int x0, int y0, int z0, int dy, int dz, const int32_t *__restrict__ sel, size_t m,
@@ -319,6 +316,12 @@ extern "C" int cphb_occgrid_get_params(const cphb_occgrid *g, cphb_occgrid_param
 void cphb_occgrid_geometry(const cphb_occgrid *g, float *voxel_size, float origin[3]) {
     *voxel_size = g->voxel_size;
     for (int a = 0; a < 3; ++a) origin[a] = g->origin[a];
+}
+void cphb_occgrid_view_of(const cphb_occgrid *g, cphb_occgrid_view *v) {
+    v->prob = g->prob;
+    v->bounds = g->bounds;
+    v->res = g->res;
+    v->thres = g->prm.occ_prob_thres_log;
 }
 extern "C" int cphb_occgrid_set_geometry(cphb_occgrid *g, float voxel_size, const float origin[3]) {
     if (!g) { cphb_set_error("cphb_occgrid_set_geometry: null grid"); return CPHB_ERR_INVALID; }

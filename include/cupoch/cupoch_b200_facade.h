@@ -178,6 +178,12 @@ inline Eigen::Matrix4f from_row_major(const float in[16]) {
 }
 }  // namespace utility
 
+namespace collision {
+namespace detail {
+struct Operand;
+}  // namespace detail
+}  // namespace collision
+
 // --------------------------------------------------------------------------- knn
 namespace knn {
 static const int NUM_MAX_NN = 100;  // kdtree_search_param.h:26
@@ -913,6 +919,7 @@ public:
 
 private:
     friend class DistanceTransform;  // CreateFromOccupancyGrid reads the dense grid
+    friend struct collision::detail::Operand;  // ComputeIntersection reads it too
     void sync() const {  // the public members are the source of truth, like the reference's
         const float o[3] = {origin_[0], origin_[1], origin_[2]};
         utility::check(cphb_occgrid_set_geometry(h_, voxel_size_, o));
@@ -1370,4 +1377,236 @@ inline std::shared_ptr<Feature<352>> ComputeSHOTFeature(const geometry::PointClo
     return feature;
 }
 }  // namespace registration
+// --------------------------------------------------------------------------- collision
+namespace collision {
+
+/// collision::Primitive (primitives.h:36-66)
+class Primitive {
+public:
+    enum class PrimitiveType { Unspecified = 0, Box = 1, Sphere = 2, Capsule = 3, Cylinder = 4 };
+    Primitive() {}
+    Primitive(PrimitiveType type) : type_(type) {}
+    Primitive(PrimitiveType type, const Eigen::Matrix4f &transform) : type_(type), transform_(transform) {}
+    virtual ~Primitive() {}
+    Primitive &Transform(const Eigen::Matrix4f &transform) {  // transform_ = transform_ * transform
+        transform_ = transform_ * transform;
+        return *this;
+    }
+    virtual geometry::AxisAlignedBoundingBox<3> GetAxisAlignedBoundingBox() const { return geometry::AxisAlignedBoundingBox<3>(); }
+    PrimitiveType type_ = PrimitiveType::Unspecified;
+    Eigen::Matrix4f transform_ = Eigen::Matrix4f::Identity();
+};
+
+namespace detail {
+inline Eigen::Vector3f translation(const Eigen::Matrix4f &T) { return Eigen::Vector3f(T(0, 3), T(1, 3), T(2, 3)); }
+}  // namespace detail
+
+/// collision::Box(lengths, transform) (primitives.h:68-88); GetAxisAlignedBoundingBox as written there: +-|R l / 2|
+class Box : public Primitive {
+public:
+    Box() : Primitive(PrimitiveType::Box) {}
+    Box(const Eigen::Vector3f &lengths) : Primitive(PrimitiveType::Box), lengths_(lengths) {}
+    Box(const Eigen::Vector3f &lengths, const Eigen::Matrix4f &transform) : Primitive(PrimitiveType::Box, transform), lengths_(lengths) {}
+    geometry::AxisAlignedBoundingBox<3> GetAxisAlignedBoundingBox() const override {
+        float lo[3], hi[3];
+        for (int i = 0; i < 3; ++i) {
+            float ra = 0.f;
+            for (int j = 0; j < 3; ++j) ra += transform_(i, j) * 0.5f * lengths_[j];
+            lo[i] = -std::fabs(ra) + transform_(i, 3);
+            hi[i] = std::fabs(ra) + transform_(i, 3);
+        }
+        return geometry::AxisAlignedBoundingBox<3>(Eigen::Vector3f(lo[0], lo[1], lo[2]), Eigen::Vector3f(hi[0], hi[1], hi[2]));
+    }
+    Eigen::Vector3f lengths_ = Eigen::Vector3f(0.f, 0.f, 0.f);
+};
+
+/// collision::Sphere(radius, center) (primitives.h:90-110)
+class Sphere : public Primitive {
+public:
+    Sphere() : Primitive(PrimitiveType::Sphere) {}
+    Sphere(float radius) : Primitive(PrimitiveType::Sphere), radius_(radius) {}
+    Sphere(float radius, const Eigen::Vector3f &center) : Primitive(PrimitiveType::Sphere), radius_(radius) {
+        for (int i = 0; i < 3; ++i) transform_(i, 3) = center[i];
+    }
+    geometry::AxisAlignedBoundingBox<3> GetAxisAlignedBoundingBox() const override {
+        const Eigen::Vector3f c = detail::translation(transform_);
+        return geometry::AxisAlignedBoundingBox<3>(Eigen::Vector3f(c[0] - radius_, c[1] - radius_, c[2] - radius_),
+                                                   Eigen::Vector3f(c[0] + radius_, c[1] + radius_, c[2] + radius_));
+    }
+    float radius_ = 0.f;
+};
+
+/// collision::Capsule(radius, height, transform) (primitives.h:112-140): the segment of length height along the
+/// transform's third column
+class Capsule : public Primitive {
+public:
+    Capsule() : Primitive(PrimitiveType::Capsule) {}
+    Capsule(float radius, float height) : Primitive(PrimitiveType::Capsule), radius_(radius), height_(height) {}
+    Capsule(float radius, float height, const Eigen::Matrix4f &transform)
+        : Primitive(PrimitiveType::Capsule, transform), radius_(radius), height_(height) {}
+    geometry::AxisAlignedBoundingBox<3> GetAxisAlignedBoundingBox() const override {
+        float lo[3], hi[3];
+        for (int i = 0; i < 3; ++i) {
+            const float pa = transform_(i, 2) * (0.5f * height_);
+            lo[i] = std::min(pa, -pa) - radius_ + transform_(i, 3);
+            hi[i] = std::max(pa, -pa) + radius_ + transform_(i, 3);
+        }
+        return geometry::AxisAlignedBoundingBox<3>(Eigen::Vector3f(lo[0], lo[1], lo[2]), Eigen::Vector3f(hi[0], hi[1], hi[2]));
+    }
+    float radius_ = 0.f;
+    float height_ = 0.f;
+};
+
+/// collision::Cylinder(radius, height, transform) (primitives.h:142-185).  It never collides: the reference's collision
+/// functors fall to their default branch for it.  GetAxisAlignedBoundingBox as written there (the maximum takes the
+/// smaller end).
+class Cylinder : public Primitive {
+public:
+    Cylinder() : Primitive(PrimitiveType::Cylinder) {}
+    Cylinder(float radius, float height) : Primitive(PrimitiveType::Cylinder), radius_(radius), height_(height) {}
+    Cylinder(float radius, float height, const Eigen::Matrix4f &transform)
+        : Primitive(PrimitiveType::Cylinder, transform), radius_(radius), height_(height) {}
+    geometry::AxisAlignedBoundingBox<3> GetAxisAlignedBoundingBox() const override {
+        float pa[3], a[3], n2 = 0.f, lo[3], hi[3];
+        for (int i = 0; i < 3; ++i) {
+            pa[i] = transform_(i, 2) * (0.5f * height_);
+            a[i] = -pa[i] - pa[i];
+            n2 += a[i] * a[i];
+        }
+        for (int i = 0; i < 3; ++i) {
+            const float e = radius_ * std::sqrt(1.f - a[i] * a[i] / n2);
+            lo[i] = std::min(pa[i] - e, -pa[i] - e) + transform_(i, 3);
+            hi[i] = std::min(pa[i] + e, -pa[i] + e) + transform_(i, 3);
+        }
+        return geometry::AxisAlignedBoundingBox<3>(Eigen::Vector3f(lo[0], lo[1], lo[2]), Eigen::Vector3f(hi[0], hi[1], hi[2]));
+    }
+    float radius_ = 0.f;
+    float height_ = 0.f;
+};
+
+/// collision::PrimitivePack (primitives.h:199-231) and PrimitiveArray: built on the host, uploaded per call
+struct PrimitivePack {
+    PrimitivePack() {}
+    PrimitivePack(const Box &b) : primitive_(b), box_(b) {}
+    PrimitivePack(const Sphere &s) : primitive_(s), sphere_(s) {}
+    PrimitivePack(const Capsule &c) : primitive_(c), capsule_(c) {}
+    PrimitivePack(const Cylinder &c) : primitive_(c), cylinder_(c) {}
+    Primitive primitive_;
+    Box box_;
+    Sphere sphere_;
+    Capsule capsule_;
+    Cylinder cylinder_;
+};
+typedef std::vector<PrimitivePack> PrimitiveArray;
+
+/// collision::CollisionResult (collision.h:47-75)
+struct CollisionResult {
+    enum class CollisionType { Unspecified = 0, Primitives = 1, VoxelGrid = 2, OccupancyGrid = 3 };
+    CollisionResult() {}
+    CollisionResult(CollisionType first, CollisionType second) : first_(first), second_(second) {}
+    bool IsCollided() const { return !collision_index_pairs_.empty(); }
+    std::vector<Eigen::Vector2i> GetCollisionIndexPairs() const { return collision_index_pairs_.to_host(); }
+    std::vector<size_t> GetFirstCollisionIndices() const { return column(0); }
+    std::vector<size_t> GetSecondCollisionIndices() const { return column(1); }
+    CollisionType first_ = CollisionType::Unspecified;
+    CollisionType second_ = CollisionType::Unspecified;
+    utility::device_vector<Eigen::Vector2i> collision_index_pairs_;
+
+private:
+    std::vector<size_t> column(int c) const {  // as it is, not deduplicated (host vectors here)
+        const std::vector<Eigen::Vector2i> p = GetCollisionIndexPairs();
+        std::vector<size_t> out(p.size());
+        for (size_t i = 0; i < p.size(); ++i) out[i] = (size_t)p[i][c];
+        return out;
+    }
+};
+
+namespace detail {
+struct Operand {
+    cphb_coll_operand op{};
+    utility::device_vector<cphb_primitive> prims;
+    bool empty = false;
+    explicit Operand(const geometry::VoxelGrid &g) {
+        op.kind = CPHB_COLL_VOXEL_GRID;
+        op.keys = reinterpret_cast<const int32_t *>(g.voxels_keys_.data());
+        op.n = g.voxels_keys_.size();
+        op.voxel_size = g.voxel_size_;
+        for (int i = 0; i < 3; ++i) op.origin[i] = g.origin_[i];
+        empty = op.n == 0;
+    }
+    explicit Operand(const geometry::OccupancyGrid &g) {
+        g.sync();
+        op.kind = CPHB_COLL_OCCUPANCY_GRID;
+        op.occ = g.h_;
+    }
+    explicit Operand(const PrimitiveArray &a) {
+        std::vector<cphb_primitive> h(a.size());
+        for (size_t i = 0; i < a.size(); ++i) {
+            const PrimitivePack &p = a[i];
+            cphb_primitive &c = h[i];
+            std::memset(&c, 0, sizeof(c));
+            c.type = (int32_t)p.primitive_.type_;
+            utility::to_row_major(p.primitive_.transform_, c.transform);
+            for (int k = 0; k < 3; ++k) c.lengths[k] = p.box_.lengths_[k];
+            switch (p.primitive_.type_) {
+                case Primitive::PrimitiveType::Sphere: c.radius = p.sphere_.radius_; break;
+                case Primitive::PrimitiveType::Capsule: c.radius = p.capsule_.radius_; c.height = p.capsule_.height_; break;
+                case Primitive::PrimitiveType::Cylinder: c.radius = p.cylinder_.radius_; c.height = p.cylinder_.height_; break;
+                default: break;
+            }
+        }
+        prims = h;
+        op.kind = CPHB_COLL_PRIMITIVES;
+        op.primitives = prims.data();
+        op.n = a.size();
+        empty = a.empty();
+    }
+};
+
+inline std::shared_ptr<CollisionResult> compute(const Operand &a, const Operand &b, float margin) {
+    auto out = std::make_shared<CollisionResult>((CollisionResult::CollisionType)a.op.kind, (CollisionResult::CollisionType)b.op.kind);
+    // at most one pair per query element: a VoxelGrid or primitive query needs one call, an OccupancyGrid query is sized first
+    size_t cap = b.op.kind == CPHB_COLL_OCCUPANCY_GRID ? 0 : b.op.n, m = 0;
+    out->collision_index_pairs_.resize(cap);
+    int rc = cphb_compute_intersection(&a.op, &b.op, margin, reinterpret_cast<int32_t *>(out->collision_index_pairs_.data()), cap, &m, nullptr);
+    if (rc == CPHB_ERR_INVALID) {
+        utility::LogError(cphb_last_error());
+        out->collision_index_pairs_.resize(0);
+        return out;
+    }
+    utility::check(rc);
+    if (a.empty || b.empty) utility::LogWarning("[Intersection::Compute] target or query is empty.");
+    if (m && !cap) {
+        out->collision_index_pairs_.resize(m);
+        utility::check(cphb_compute_intersection(&a.op, &b.op, margin, reinterpret_cast<int32_t *>(out->collision_index_pairs_.data()), m, &m, nullptr));
+    }
+    out->collision_index_pairs_.resize(m);
+    return out;
+}
+}  // namespace detail
+
+/// collision::ComputeIntersection(a, b, margin) (collision.h:98-146, collision.cu:1137-1231): a is the target, b the query;
+/// each colliding query element gives (smallest colliding index in a, index in b), in ascending query order
+inline std::shared_ptr<CollisionResult> ComputeIntersection(const geometry::VoxelGrid &voxelgrid1, const geometry::VoxelGrid &voxelgrid2, float margin = 0.0f) {
+    return detail::compute(detail::Operand(voxelgrid1), detail::Operand(voxelgrid2), margin);
+}
+inline std::shared_ptr<CollisionResult> ComputeIntersection(const geometry::VoxelGrid &voxelgrid, const geometry::OccupancyGrid &occgrid, float margin = 0.0f) {
+    return detail::compute(detail::Operand(voxelgrid), detail::Operand(occgrid), margin);
+}
+inline std::shared_ptr<CollisionResult> ComputeIntersection(const geometry::OccupancyGrid &occgrid, const geometry::VoxelGrid &voxelgrid, float margin = 0.0f) {
+    return detail::compute(detail::Operand(occgrid), detail::Operand(voxelgrid), margin);
+}
+inline std::shared_ptr<CollisionResult> ComputeIntersection(const geometry::VoxelGrid &voxelgrid, const PrimitiveArray &primitives, float margin = 0.0f) {
+    return detail::compute(detail::Operand(voxelgrid), detail::Operand(primitives), margin);
+}
+inline std::shared_ptr<CollisionResult> ComputeIntersection(const PrimitiveArray &primitives, const geometry::VoxelGrid &voxelgrid, float margin = 0.0f) {
+    return detail::compute(detail::Operand(primitives), detail::Operand(voxelgrid), margin);
+}
+inline std::shared_ptr<CollisionResult> ComputeIntersection(const geometry::OccupancyGrid &occgrid, const PrimitiveArray &primitives, float margin = 0.0f) {
+    return detail::compute(detail::Operand(occgrid), detail::Operand(primitives), margin);
+}
+inline std::shared_ptr<CollisionResult> ComputeIntersection(const PrimitiveArray &primitives, const geometry::OccupancyGrid &occgrid, float margin = 0.0f) {
+    return detail::compute(detail::Operand(primitives), detail::Operand(occgrid), margin);
+}
+}  // namespace collision
 }  // namespace cupoch

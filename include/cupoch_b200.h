@@ -478,6 +478,55 @@ int cphb_dt_get_voxel(const cphb_dt *dt, const float point[3], int *h_found, int
 const float *cphb_dt_distance_data(const cphb_dt *dt);   /* device distance[res^3], borrowed */
 const uint32_t *cphb_dt_nearest_data(const cphb_dt *dt); /* device nearest[res^3] (packed as above), borrowed */
 
+/* ------------------------------------------------------------------------ *
+ * collision::ComputeIntersection (collision.h:36-160, collision.cu:1137-1231)
+ * between VoxelGrids, OccupancyGrids and primitives.  Every grid element is an
+ * integer key k with the box [k * vs + origin, (k + 1) * vs + origin]: a
+ * VoxelGrid key as stored, an OccupancyGrid cell (x, y, z) as k = (x, y, z) -
+ * resolution / 2.  An OccupancyGrid's elements are its occupied cells
+ * (!isnan(p) && p > occ_prob_thres_log, inside its bound box, as
+ * cphb_occgrid_extract(which = 2) lists them: ascending linear index) and an
+ * element's index is its linear cell index x * res^2 + y * res + z.
+ * ------------------------------------------------------------------------ */
+enum { /* collision::Primitive::PrimitiveType */
+    CPHB_PRIM_UNSPECIFIED = 0,
+    CPHB_PRIM_BOX = 1,
+    CPHB_PRIM_SPHERE = 2,
+    CPHB_PRIM_CAPSULE = 3,
+    CPHB_PRIM_CYLINDER = 4 /* never collides (the reference's default branch) */
+};
+typedef struct cphb_primitive { /* primitives.h:30-160: Box, Sphere, Capsule, Cylinder */
+    int32_t type;               /* CPHB_PRIM_* */
+    float transform[16];        /* row-major 4x4; a Capsule's axis is its third column */
+    float lengths[3];           /* Box */
+    float radius;               /* Sphere, Capsule, Cylinder */
+    float height;               /* Capsule, Cylinder */
+} cphb_primitive;
+enum { /* CollisionResult::CollisionType */
+    CPHB_COLL_PRIMITIVES = 1,
+    CPHB_COLL_VOXEL_GRID = 2,
+    CPHB_COLL_OCCUPANCY_GRID = 3
+};
+typedef struct cphb_coll_operand {
+    int32_t kind;                      /* CPHB_COLL_* */
+    const int32_t *keys;               /* VOXEL_GRID: device [n][3] voxels_keys_ (any order, duplicates allowed) */
+    size_t n;                          /* VOXEL_GRID: keys; PRIMITIVES: primitives */
+    float voxel_size, origin[3];       /* VOXEL_GRID */
+    const cphb_occgrid *occ;           /* OCCUPANCY_GRID (its own voxel size, origin and threshold) */
+    const cphb_primitive *primitives;  /* PRIMITIVES: device [n] */
+} cphb_coll_operand;
+/* ComputeIntersection(a, b, margin): a is the target, b the query.  Every query element that collides with some
+ * target element gives one pair (smallest colliding index in a, index in b), in ascending query order, written to
+ * pairs_out (device [capacity][2] int32); *h_count = the number of pairs (capacity 0 sizes the output).  Grid
+ * against grid: the query box widened by margin overlaps the target box (inclusive).  Primitive against grid element
+ * (centre (k + 0.5) * vs + origin, half size vs / 2): Box = separating axes with margin added to the half size,
+ * Sphere and Capsule with radius + margin.  An empty operand gives no pairs.  CPHB_ERR_INVALID: a pair the reference
+ * does not offer (OccupancyGrid x OccupancyGrid, primitives x primitives), a non-finite margin, a VoxelGrid with keys
+ * or any OccupancyGrid whose voxel size is not positive and finite, or VoxelGrid target keys spanning 2^21 or more
+ * on an axis.  Synchronises. */
+int cphb_compute_intersection(const cphb_coll_operand *a, const cphb_coll_operand *b, float margin, int32_t *pairs_out,
+                              size_t capacity, size_t *h_count, void *stream);
+
 /* registration::EvaluateRegistration (registration.cu:106-119). */
 int cphb_evaluate_registration(const cphb_cloud *source, const cphb_cloud *target,
                                float max_correspondence_distance, const float h_T[16],

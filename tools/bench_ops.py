@@ -38,7 +38,12 @@ def main():
     ap.add_argument("--out", default=None, help="--shot, --crop: also write the JSON object to this file")
     ap.add_argument("--edt", action="store_true",
                     help="instead: time geometry::DistanceTransform::ComputeEDT at 256^3 and 512^3 and GetDistances of 10 M points")
+    ap.add_argument("--collision", action="store_true",
+                    help="instead: time collision::ComputeIntersection on the config-3 VoxelGrid, a 512^3 OccupancyGrid and "
+                         "1 / 1e4 primitives")
     args = ap.parse_args()
+    if args.collision:
+        return collision(args.reps, args.out)
     if args.edt:
         return edt(args.reps)
     if args.segment_plane:
@@ -700,6 +705,114 @@ def crop(reps, n, out=None):
                      "share_of_3.35TBps_over_call_time": nbytes / (float(np.median(ts)) * 1e-3) / H100_HBM_BYTES_PER_S})
     obj = {"op": "bounding-box selection and cleanup on the config-3 cloud (uniform_cube(N, 21) in [0,4)x[0,4)x[0,1), "
                  "normals and colours)", "gpu": gpu, "reps": reps, "rows": rows}
+    line = json.dumps(obj)
+    print(line)
+    if out:
+        with open(out, "w") as f:
+            f.write(line + "\n")
+
+
+def collision_bytes_model(kind_t, n_t, kind_q, n_q, m, box_cells=0):
+    """HBM bytes one compute_intersection call must move at least (a model, not a measurement): a VoxelGrid target's
+    keys read twice (bounds, pack) and sorted (12-byte key + index pairs, read and written by each of 8 radix passes);
+    the query's elements read once (keys, 88-byte primitives, or the bound box of an OccupancyGrid query flagged and
+    compacted); per query element its best index, flag and compaction slot (9 B); 8 B per pair.  Lookups into the
+    target are not counted: they mostly hit L2."""
+    b = 0
+    if kind_t == "vg":
+        b += 24 * n_t + 2 * 12 * n_t * 9
+    b += {"vg": 12, "prim": 88 + 32, "occ": 0}[kind_q] * n_q
+    b += 5 * box_cells + 4 * n_q if kind_q == "occ" else 0
+    return b + 9 * n_q + 8 * m
+
+
+def collision(reps, out=None):
+    """compute_intersection on the config-3 cloud (uniform_cube(10 M, 21) in [0,4)x[0,4)x[0,1)) voxelised at 0.02
+    (about 2 M voxels): against itself moved by (0.3, 0.2, 0.1) voxels at margins 0 and 2 voxels; a 512^3
+    OccupancyGrid (voxel 0.02) after inserting a 1 M-point scan, in both orders against that grid; 1 and 1e4 mixed
+    primitives in both orders; one box whose region covers about 1e6 cells.  CUDA-event median and minimum of `reps`
+    calls after a warm-up call, the kernel time of one further call from torch.profiler, the bytes model beside it."""
+    import subprocess
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    import cupoch_b200 as cph
+    from cupoch_b200 import _lib
+    from cupoch_b200.testing import datagen
+    L = _lib.lib()
+    K = cph.collision
+    gpu = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                         capture_output=True, text=True).stdout.strip()
+    ev = [L.cphb_event_create() for _ in range(2)]
+
+    def timed(fn):
+        times = []
+        for r in range(reps + 1):
+            L.cphb_event_record(ev[0], None)
+            fn()
+            L.cphb_event_record(ev[1], None)
+            ms = C.c_float(0)
+            _lib.check(L.cphb_event_elapsed_ms(ev[0], ev[1], C.byref(ms)))
+            if r:
+                times.append(ms.value)
+        return times
+
+    vs = 0.02
+    pc = cph.geometry.PointCloud(datagen.uniform_cube(10_000_000, 21, hi=(4, 4, 1)))
+    tgt = cph.geometry.VoxelGrid.create_from_point_cloud(pc, vs)
+    del pc
+    qry = cph.geometry.VoxelGrid()
+    qry.voxel_size, qry.voxels_keys = tgt.voxel_size, tgt.voxels_keys
+    qry.origin = tgt.origin + np.float32(vs) * np.array([0.3, 0.2, 0.1], np.float32)
+    scan = datagen.surface(1_000_000, 11, extent=4.0)[0] + np.array([0, 0, 0.5], np.float32)
+    occ = cph.geometry.OccupancyGrid(vs, 512, (2.0, 2.0, 0.5))
+    occ.insert(cph.geometry.PointCloud(scan.astype(np.float32)), (2.0, 2.0, 3.0))
+    lo, hi = occ._bounds()
+    box_cells = int(np.prod((hi - lo + 1).astype(np.int64)))
+    rng = np.random.default_rng(3)
+    prims = K.PrimitiveArray()
+    for i in range(10_000):
+        c = rng.uniform((0, 0, 0), (4, 4, 1))
+        T = np.eye(4, dtype=np.float32)
+        T[:3, 3] = c
+        a = rng.uniform(0, np.pi)
+        T[:2, :2] = [[np.cos(a), -np.sin(a)], [np.sin(a), np.cos(a)]]
+        s = rng.uniform(1, 5) * vs
+        prims.append([K.Box([s, s, s], T), K.Sphere(s, c), K.Capsule(s / 2, 2 * s, T)][i % 3])
+    one = K.PrimitiveArray([prims[0]])
+    big = K.PrimitiveArray([K.Box([2.0, 2.0, 2.0], np.array([[1, 0, 0, 2], [0, 1, 0, 2], [0, 0, 1, 0.5], [0, 0, 0, 1]], np.float32))])
+    n_vg = len(tgt)
+    work = [("vg x vg, margin 0", tgt, qry, 0.0, ("vg", n_vg, "vg", n_vg)),
+            ("vg x vg, margin 2 vs", tgt, qry, 2 * vs, ("vg", n_vg, "vg", n_vg)),
+            ("occ x vg", occ, qry, 0.0, ("occ", 0, "vg", n_vg)),
+            ("vg x occ", tgt, occ, 0.0, ("vg", n_vg, "occ", None)),
+            ("vg x 1 primitive", tgt, one, 0.0, ("vg", n_vg, "prim", 1)),
+            ("1 primitive x vg", one, tgt, 0.0, ("prim", 1, "vg", n_vg)),
+            ("vg x 1e4 primitives", tgt, prims, 0.0, ("vg", n_vg, "prim", 10_000)),
+            ("1e4 primitives x vg", prims, tgt, 0.0, ("prim", 10_000, "vg", n_vg)),
+            ("vg x one box over ~1e6 cells", tgt, big, 0.0, ("vg", n_vg, "prim", 1))]
+    rows = []
+    for name, a, b, margin, shape in work:
+        ts = timed(lambda: K.compute_intersection(a, b, margin))
+        res = K.compute_intersection(a, b, margin)
+        m = len(res.collision_index_pairs)
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            K.compute_intersection(a, b, margin)
+            torch.cuda.synchronize()
+        kernels = {}
+        for e in prof.key_averages():
+            t = getattr(e, "device_time_total", getattr(e, "cuda_time_total", 0.0)) * 1e-3
+            if t > 0 and "Memset" not in e.key and "Memcpy" not in e.key:
+                kernels[e.key[:60]] = kernels.get(e.key[:60], 0.0) + t
+        kern_ms = float(sum(kernels.values()))
+        kt, nt, kq, nq = shape
+        nq = m if nq is None else nq  # an OccupancyGrid query: its occupied cells are not known up front
+        nbytes = collision_bytes_model(kt, nt, kq, nq, m, box_cells if kq == "occ" else 0)
+        rows.append({"workload": name, "pairs": m, "call_ms_median": float(np.median(ts)), "call_ms_min": float(np.min(ts)),
+                     "kernel_ms_profiled": kernels, "kernel_ms_sum": kern_ms, "bytes_model": nbytes,
+                     "share_of_3.35TBps_over_kernel_time": nbytes / (kern_ms * 1e-3) / HBM_BYTES_PER_S if kern_ms else None})
+    obj = {"op": "collision::ComputeIntersection on the config-3 cloud voxelised at 0.02 (%d voxels), a 512^3 "
+                 "OccupancyGrid after a 1 M-point scan (%d cells in its bound box) and 1 / 1e4 mixed primitives" % (n_vg, box_cells),
+           "gpu": gpu, "reps": reps, "rows": rows}
     line = json.dumps(obj)
     print(line)
     if out:

@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
-"""Generate tests/golden/reference_vectors.json (and segment_plane_known.json, pointcloud_crop_known.json) from the
-reference's own unit tests.
+"""Generate tests/golden/reference_vectors.json (and segment_plane_known.json, pointcloud_crop_known.json,
+collision_known.json) from the reference's own unit tests.  `make_golden.py collision` writes collision_known.json only.
 
 Run in the development container only (needs /root/reference, which does not
 exist on the GPU box).  It reads
@@ -224,5 +224,33 @@ def crop_known(table, pc, source):
     print("wrote", os.path.normpath(OUT_CROP), os.path.getsize(OUT_CROP), "bytes")
 
 
+def collision_known():
+    """TEST(Collision, VoxelVoxel) (src/tests/collision/collision.cpp) -> OUT_COLL: its three steps, each with the
+    voxel keys the test has added by then (voxel size 1, origin 0) and what it asserts"""
+    b = test_body(read("src/tests/collision/collision.cpp"), "Collision", "VoxelVoxel")
+    adds = re.findall(r"(voxel[12])\.AddVoxel\(geometry::Voxel\(Eigen::Vector3i\((-?\d+),\s*(-?\d+),\s*(-?\d+)\)\)\)", b)
+    assert len(adds) == 4 and "voxel_size_ = 1.0" in b and "Eigen::Vector2i(0, 0)" in b, adds
+    keys = {"voxel1": [], "voxel2": []}
+    steps = []
+    for i, (v, x, y, z) in enumerate(adds):
+        keys[v].append([int(x), int(y), int(z)])
+        if i % 2 == 1:
+            steps.append({"keys1": [list(k) for k in keys["voxel1"]], "keys2": [list(k) for k in keys["voxel2"]]})
+    out = {"voxel_size": 1.0, "origin": [0.0, 0.0, 0.0],
+           "steps": [{"keys1": [], "keys2": [], "collided": False}] +
+                    [dict(steps[0], collided=True), dict(steps[1], collided=True, pairs=[[0, 0]])],
+           "cite": "src/tests/collision/collision.cpp TEST(Collision, VoxelVoxel): empty grids do not collide; one "
+                   "shared voxel collides; with (5,0,0) and (10,0,0) added there is exactly one pair, (0, 0)"}
+    with open(OUT_COLL, "w") as f:
+        json.dump(out, f)
+    print("wrote", os.path.normpath(OUT_COLL), os.path.getsize(OUT_COLL), "bytes")
+
+
+OUT_COLL = os.path.join(os.path.dirname(OUT), "collision_known.json")
+
 if __name__ == "__main__":
-    sys.exit(main())
+    if sys.argv[1:] == ["collision"]:  # only the collision known answer; the other files stay as they are
+        sys.exit(collision_known())
+    rc = main()
+    collision_known()
+    sys.exit(rc)

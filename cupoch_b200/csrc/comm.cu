@@ -9,6 +9,8 @@
 #include <dlfcn.h>
 #include <string.h>
 
+#include <memory>
+
 #include "cphb_internal.cuh"
 
 typedef struct { char internal[128]; } nccl_uid;
@@ -86,7 +88,6 @@ extern "C" int cphb_comm_nccl_create(const char h_id[128], int world_size, int r
     nccl_comm_t c = nullptr;
     NCCL_TRY(g_nccl.init_rank(&c, world_size, u, rank));
     cphb_comm *cm = new cphb_comm();
-    memset(cm, 0, sizeof(*cm));
     cm->kind = CPHB_COMM_NCCL;
     cm->rank = rank;
     cm->world = world_size;
@@ -101,8 +102,7 @@ extern "C" int cphb_comm_p2p_create(int world_size, int rank, char h_handle[64],
         return CPHB_ERR_INVALID;
     }
     static_assert(sizeof(cudaIpcMemHandle_t) == 64, "IPC handle size");
-    cphb_comm *cm = new cphb_comm();
-    memset(cm, 0, sizeof(*cm));
+    std::unique_ptr<cphb_comm> cm(new cphb_comm());
     cm->kind = CPHB_COMM_P2P;
     cm->rank = rank;
     cm->world = world_size;
@@ -112,7 +112,7 @@ extern "C" int cphb_comm_p2p_create(int world_size, int rank, char h_handle[64],
     cudaIpcMemHandle_t h;
     CPHB_CUDA(cudaIpcGetMemHandle(&h, cm->box_local));
     memcpy(h_handle, &h, 64);
-    *out = cm;
+    *out = cm.release();
     return CPHB_OK;
 }
 
@@ -138,16 +138,18 @@ extern "C" int cphb_comm_p2p_connect(cphb_comm *cm, const char *h_handles) {
     return CPHB_OK;
 }
 
-extern "C" int cphb_comm_destroy(cphb_comm *cm) {
-    if (!cm) return CPHB_OK;
-    if (cm->kind == CPHB_COMM_NCCL && cm->nccl) {
-        if (nccl_load() == CPHB_OK) g_nccl.destroy((nccl_comm_t)cm->nccl);
-    } else if (cm->kind == CPHB_COMM_P2P) {
+cphb_comm::~cphb_comm() {
+    if (kind == CPHB_COMM_NCCL && nccl) {
+        if (nccl_load() == CPHB_OK) g_nccl.destroy((nccl_comm_t)nccl);
+    } else if (kind == CPHB_COMM_P2P) {
         cudaDeviceSynchronize();
-        for (int q = 0; q < cm->world; ++q)
-            if (q != cm->rank && cm->view.box[q]) cudaIpcCloseMemHandle(cm->view.box[q]);
-        if (cm->box_local) cudaFree(cm->box_local);
+        for (int q = 0; q < world; ++q)
+            if (q != rank && view.box[q]) cudaIpcCloseMemHandle(view.box[q]);
+        if (box_local) cudaFree(box_local);
     }
+}
+
+extern "C" int cphb_comm_destroy(cphb_comm *cm) {
     delete cm;
     return CPHB_OK;
 }

@@ -5,6 +5,9 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include <utility>
+#include <vector>
+
 #include "cupoch_b200.h"
 
 // ---------------------------------------------------------------------------
@@ -37,15 +40,6 @@ struct IndexView {
     unsigned long long n;
     unsigned n_leaves;
     int top; /* smallest level with <= 32 nodes */
-};
-
-struct cphb_index {
-    IndexView v;
-    void *arena;
-    size_t arena_bytes;
-    float *bounds; /* device: 6 ordered-uint encoded floats (min xyz, max xyz) */
-    int device;
-    cudaStream_t stream; /* stream the arena was allocated on */
 };
 
 // ---------------------------------------------------------------------------
@@ -115,6 +109,55 @@ class cphb_scratch {
     cudaStream_t s_;
     void *p_[CPHB_SCRATCH_SLOTS];
     int n_ = 0;
+};
+
+// One device block cut into typed slices, for a handle's storage or a call's fixed layout.  slice() records a slice of
+// `count` elements at the running offset (an absent slice takes no space and its pointer stays null); the offset then
+// moves to the next multiple of 256.  alloc() makes one allocation of the total and points every recorded slice into
+// it, or on failure allocates nothing and leaves every pointer null.  The block goes back to the pool, on the stream
+// it was allocated on, when the owner is destroyed.
+class cphb_arena {
+  public:
+    cphb_arena() = default;
+    ~cphb_arena() {
+        if (base_) cphb_free_async(base_, s_);
+    }
+    cphb_arena(cphb_arena &&o) noexcept : slices_(std::move(o.slices_)), bytes_(o.bytes_), base_(o.base_), s_(o.s_) {
+        o.base_ = nullptr;
+    }
+    cphb_arena(const cphb_arena &) = delete;
+    cphb_arena &operator=(const cphb_arena &) = delete;
+    template <class T>
+    void slice(T **p, size_t count, bool present = true) {
+        *p = nullptr;
+        if (!present) return;
+        slices_.push_back({(void **)p, bytes_});
+        bytes_ = cphb_align(bytes_ + sizeof(T) * count, 256);
+    }
+    int alloc(cudaStream_t s) {
+        const int rc = cphb_alloc_async(&base_, bytes_, s);
+        if (rc) {
+            base_ = nullptr;
+            return rc;
+        }
+        s_ = s;
+        for (const auto &sl : slices_) *sl.first = (char *)base_ + sl.second;
+        return CPHB_OK;
+    }
+    size_t bytes() const { return bytes_; }
+
+  private:
+    std::vector<std::pair<void **, size_t>> slices_;  // (pointer to fill, offset)
+    size_t bytes_ = 0;
+    void *base_ = nullptr;
+    cudaStream_t s_ = nullptr;
+};
+
+struct cphb_index {
+    IndexView v = {};
+    cphb_arena arena;     // points, boxes, bounds, permutation and inverse (index.cu)
+    float *bounds = nullptr; /* device: 6 ordered-uint encoded floats (min xyz, max xyz) */
+    int device = 0;
 };
 
 // pending launch error, then `bytes` from d to h (0: none), then a synchronise of s; the first failure is reported as
@@ -192,10 +235,11 @@ struct P2pView {
     int rank, world;
 };
 struct cphb_comm {
-    int kind, rank, world, connected;
-    void *nccl;
-    void *box_local;
-    P2pView view;
+    int kind = 0, rank = 0, world = 0, connected = 0;
+    void *nccl = nullptr;
+    void *box_local = nullptr;
+    P2pView view = {};
+    ~cphb_comm();  // releases the NCCL communicator, or the peers' mapped mailboxes and this rank's own (comm.cu)
 };
 int cphb_nccl_allreduce_f64(void *nccl_comm, const double *send, double *recv, size_t count, cudaStream_t s);
 

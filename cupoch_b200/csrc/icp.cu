@@ -25,6 +25,7 @@
 #include <string.h>
 
 #include "cphb_internal.cuh"
+#include <memory>
 #include <type_traits>
 #include <vector>
 #include "cphb_eigen3.cuh"
@@ -41,35 +42,34 @@
 // ===========================================================================
 
 struct cphb_icp {
-    cphb_index *index;
-    cphb_icp_params prm;
-    cphb_cloud tgt;
-    unsigned n_src, n_pad;
-    unsigned n_full;   // size of the source as passed (== n_src unless the library shards it)
-    void *arena;
-    size_t arena_bytes;
-    float4 *pristine_xyz, *pristine_nrm, *pristine_cov;  // Hilbert-ordered source as given
-    float4 *work_xyz, *work_nrm, *work_cov;
-    float4 *src_col;
-    float4 *tix_nrm, *tix_grad, *tix_cov;  // target attributes in index order (icp_types.cuh)
-    IcpState *st;
-    IcpState *h_st;  // pinned
-    bool owns_host;
-    cudaEvent_t ev0, ev1;
-    double *partials;
-    int32_t *corr_index;
-    unsigned *cmp_counts;
-    unsigned *cmp_total;
-    double *tile_sums;
-    unsigned *flag_bits;
-    unsigned flag_words;
-    int2 *prev;
+    cphb_arena arena;  // every device buffer below but dbg
+    cphb_index *index = nullptr;
+    cphb_icp_params prm = {};
+    cphb_cloud tgt = {};
+    unsigned n_src = 0, n_pad = 0;
+    unsigned n_full = 0;  // size of the source as passed (== n_src unless the library shards it)
+    float4 *pristine_xyz = nullptr, *pristine_nrm = nullptr, *pristine_cov = nullptr;  // Hilbert-ordered source as given
+    float4 *work_xyz = nullptr, *work_nrm = nullptr, *work_cov = nullptr;
+    float4 *src_col = nullptr;
+    float4 *tix_nrm = nullptr, *tix_grad = nullptr, *tix_cov = nullptr;  // target attributes in index order (icp_types.cuh)
+    IcpState *st = nullptr;
+    IcpState *h_st = nullptr;  // pinned
+    bool owns_host = false;
+    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+    double *partials = nullptr;
+    int32_t *corr_index = nullptr;
+    unsigned *cmp_counts = nullptr;
+    unsigned *cmp_total = nullptr;
+    double *tile_sums = nullptr;
+    unsigned *flag_bits = nullptr;
+    unsigned flag_words = 0;
+    int2 *prev = nullptr;
     unsigned *dbg = nullptr;  // CPHB_DEBUG_CERT statistics
     cudaEvent_t *dbg_ev = nullptr;  // CPHB_DEBUG_EVENTS: 3 events per launch (before, between, after)
-    unsigned grid_search;  // ROLE 0 launch (searching regime)
-    unsigned grid;         // ROLE 1 launch (certified regime / sum of a searching launch's tile sums + solve)
-    unsigned reduce_grid;  // blocks of the ROLE 1 launch that take part in that sum
-    cudaStream_t stream;
+    unsigned grid_search = 0;  // ROLE 0 launch (searching regime)
+    unsigned grid = 0;         // ROLE 1 launch (certified regime / sum of a searching launch's tile sums + solve)
+    unsigned reduce_grid = 0;  // blocks of the ROLE 1 launch that take part in that sum
+    ~cphb_icp();
 };
 
 // per-thread cached pinned staging buffer + events: cudaMallocHost / cudaEventCreate cost milliseconds,
@@ -80,6 +80,28 @@ struct HostCache {
     bool in_use = false;
 };
 static thread_local HostCache t_cache;
+
+cphb_icp::~cphb_icp() {
+    if (dbg) cudaFree(dbg);
+    if (owns_host) {
+        if (h_st) cudaFreeHost(h_st);
+        if (ev0) cudaEventDestroy(ev0);
+        if (ev1) cudaEventDestroy(ev1);
+    } else if (h_st == t_cache.h_st) {
+        t_cache.in_use = false;
+    }
+    cphb_index_destroy(index);
+}
+
+// runs f when it leaves scope
+template <class F>
+struct scope_exit {
+    F f;
+    ~scope_exit() { f(); }
+};
+template <class F>
+scope_exit(F) -> scope_exit<F>;
+
 // cphb_registration_icp_host: the source arrays are still being uploaded on another stream while the target index is
 // built; cphb_icp_create waits for this event right before it first reads them
 static thread_local cudaEvent_t t_source_ready = nullptr;
@@ -201,23 +223,13 @@ extern "C" int cphb_icp_create(const cphb_cloud *source, const cphb_cloud *targe
         cphb_set_error("cphb_icp_create: cloud exceeds int32 indices");
         return CPHB_ERR_INVALID;
     }
-    cphb_icp *icp = new cphb_icp();
-    memset(icp, 0, sizeof(*icp));
-    uint32_t *perm_side = nullptr;
-    // one exit for CUDA errors after this point: the half-built context (index, arena, host staging) is released
-#define CREATE_TRY(call)                                                                                 \
-    do {                                                                                                 \
-        cudaError_t e__ = (call);                                                                        \
-        if (e__ != cudaSuccess) {                                                                        \
-            cphb_set_error("%s:%d %s: %s", __FILE__, __LINE__, #call, cudaGetErrorString(e__));          \
-            if (perm_side) cphb_free_async(perm_side, t_side.stream);                                    \
-            cphb_icp_destroy(icp);                                                                       \
-            return CPHB_ERR_CUDA;                                                                        \
-        }                                                                                                \
-    } while (0)
+    if (params->shard_world > 1 && (params->shard_rank < 0 || params->shard_rank >= params->shard_world)) {
+        cphb_set_error("cphb_icp_create: shard_rank %d outside [0,%d)", params->shard_rank, params->shard_world);
+        return CPHB_ERR_INVALID;
+    }
+    std::unique_ptr<cphb_icp> icp(new cphb_icp());
     icp->prm = *params;
     icp->tgt = *target;
-    icp->stream = s;
     const unsigned n_full = (unsigned)source->n;
     // The source's Hilbert ordering (bounds, keys, radix sort) does not depend on the target index: it runs on a side
     // stream, concurrently with the index build (both are short chains of small kernels), and joins right before the
@@ -226,37 +238,36 @@ extern "C" int cphb_icp_create(const cphb_cloud *source, const cphb_cloud *targe
     cudaGetDevice(&cur_dev);
     if (!t_side.stream || t_side.device != cur_dev) {  // (a thread that moved to another device gets a new one)
         t_side.device = cur_dev;
-        CREATE_TRY(cudaStreamCreateWithFlags(&t_side.stream, cudaStreamNonBlocking));
-        CREATE_TRY(cudaEventCreateWithFlags(&t_side.fork, cudaEventDisableTiming));
-        CREATE_TRY(cudaEventCreateWithFlags(&t_side.join, cudaEventDisableTiming));
+        CPHB_CUDA(cudaStreamCreateWithFlags(&t_side.stream, cudaStreamNonBlocking));
+        CPHB_CUDA(cudaEventCreateWithFlags(&t_side.fork, cudaEventDisableTiming));
+        CPHB_CUDA(cudaEventCreateWithFlags(&t_side.join, cudaEventDisableTiming));
     }
+    cphb_arena side;  // the source permutation, allocated on the side stream
+    uint32_t *perm_side = nullptr;
+    // it goes back to the pool on the side stream, which first waits for s: the gather on s reads it
+    scope_exit side_waits{[&] {
+        if (!perm_side) return;
+        cudaEventRecord(t_side.fork, s);
+        cudaStreamWaitEvent(t_side.stream, t_side.fork, 0);
+    }};
     int rc = CPHB_OK;
     if (n_full) {
-        CREATE_TRY(cudaEventRecord(t_side.fork, s));
-        CREATE_TRY(cudaStreamWaitEvent(t_side.stream, t_side.fork, 0));
+        CPHB_CUDA(cudaEventRecord(t_side.fork, s));
+        CPHB_CUDA(cudaStreamWaitEvent(t_side.stream, t_side.fork, 0));
         if (t_source_ready) {  // (host-buffer call: the source upload is still in flight on the copy stream)
             cudaStreamWaitEvent(t_side.stream, t_source_ready, 0);
             t_source_ready = nullptr;
         }
-        rc = cphb_alloc_async((void **)&perm_side, sizeof(uint32_t) * n_full, t_side.stream);
+        side.slice(&perm_side, n_full);
+        rc = side.alloc(t_side.stream);
         if (!rc) rc = cphb_hilbert_order(source->points, n_full, perm_side, nullptr, 0, t_side.stream);
-        if (rc) { cphb_free_async(perm_side, t_side.stream); delete icp; return rc; }
-        CREATE_TRY(cudaEventRecord(t_side.join, t_side.stream));
+        if (rc) return rc;
+        CPHB_CUDA(cudaEventRecord(t_side.join, t_side.stream));
     }
     rc = cphb_index_create(target->points, target->n, s, &icp->index);
-    if (rc) {
-        if (perm_side) { cudaStreamWaitEvent(s, t_side.join, 0); cphb_free_async(perm_side, s); }
-        delete icp;
-        return rc;
-    }
+    if (rc) return rc;
     unsigned lo = 0, n = n_full;
     if (params->shard_world > 1) {
-        if (params->shard_rank < 0 || params->shard_rank >= params->shard_world) {
-            cphb_set_error("cphb_icp_create: shard_rank %d outside [0,%d)", params->shard_rank, params->shard_world);
-            cphb_index_destroy(icp->index);
-            delete icp;
-            return CPHB_ERR_INVALID;
-        }
         lo = (unsigned)(((unsigned long long)n_full * params->shard_rank) / params->shard_world);
         unsigned hi = (unsigned)(((unsigned long long)n_full * (params->shard_rank + 1)) / params->shard_world);
         n = hi - lo;
@@ -288,70 +299,48 @@ extern "C" int cphb_icp_create(const cphb_cloud *source, const cphb_cloud *targe
     const bool want_nrm = params->estimation == CPHB_EST_SYMMETRIC && source->normals;
     const bool want_col = params->estimation == CPHB_EST_COLORED_ICP && source->colors;
     const bool want_cov = params->estimation == CPHB_EST_GENERALIZED_ICP && source->covariances;
-    size_t off = 0;
-    auto take = [&](size_t bytes) { size_t o = off; off = cphb_align(off + bytes, 256); return o; };
-    size_t o_pxyz = take(sizeof(float4) * n_pad), o_wxyz = take(sizeof(float4) * n_pad);
-    size_t o_pnrm = want_nrm ? take(sizeof(float4) * n_pad) : 0, o_wnrm = want_nrm ? take(sizeof(float4) * n_pad) : 0;
-    size_t o_pcov = want_cov ? take(sizeof(float4) * 3 * n_pad) : 0, o_wcov = want_cov ? take(sizeof(float4) * 3 * n_pad) : 0;
-    size_t o_col = want_col ? take(sizeof(float4) * n_pad) : 0;
-    size_t o_st = take(sizeof(IcpState));
-    size_t o_part = take(sizeof(double) * 32 * (icp->reduce_grid > icp->grid ? icp->reduce_grid : icp->grid));
     // private copies of the target attributes in index order (nothing of the caller's target is retained)
-    const size_t nt_pad = (size_t)icp->index->v.n_leaves * CPHB_LEAF;
+    const size_t nt_pad = (size_t)icp->index->v.n_leaves * CPHB_LEAF, nt_slice = nt_pad ? nt_pad : 1;
     const int est = params->estimation;
     const bool t_nrm = target->normals && (est == CPHB_EST_POINT_TO_PLANE || est == CPHB_EST_SYMMETRIC || est == CPHB_EST_COLORED_ICP);
     const bool t_grad = target->color_gradient && est == CPHB_EST_COLORED_ICP;
     const bool t_cov = target->covariances && est == CPHB_EST_GENERALIZED_ICP;
-    size_t o_tn = t_nrm ? take(sizeof(float4) * (nt_pad ? nt_pad : 1)) : 0, o_tg = t_grad ? take(sizeof(float4) * (nt_pad ? nt_pad : 1)) : 0;
-    size_t o_tc = t_cov ? take(sizeof(float4) * 3 * (nt_pad ? nt_pad : 1)) : 0;
-    size_t o_ts = take(sizeof(double) * n_pad);
-    const unsigned flag_words = n_pad / 1024 + 1;
-    size_t o_fb = take(sizeof(unsigned) * 2 * flag_words);
-    size_t o_prev = take(sizeof(int2) * n_pad);
     const unsigned nf_pad = (unsigned)cphb_align(n_full ? n_full : 1, ICP_BLOCK);
-    size_t o_ci = take(sizeof(int32_t) * nf_pad);
-    unsigned cmp_blocks = (nf_pad + CMP_BLOCK - 1) / CMP_BLOCK;
-    size_t o_cc = take(sizeof(unsigned) * (cmp_blocks + 1));
-    size_t o_ct = take(16);
-    icp->arena_bytes = off;
-    rc = cphb_alloc_async(&icp->arena, off, s);
-    if (rc) { cphb_index_destroy(icp->index); delete icp; return rc; }
-    char *b = (char *)icp->arena;
-    icp->pristine_xyz = (float4 *)(b + o_pxyz);
-    icp->work_xyz = (float4 *)(b + o_wxyz);
-    icp->pristine_nrm = want_nrm ? (float4 *)(b + o_pnrm) : nullptr;
-    icp->work_nrm = want_nrm ? (float4 *)(b + o_wnrm) : nullptr;
-    icp->pristine_cov = want_cov ? (float4 *)(b + o_pcov) : nullptr;
-    icp->work_cov = want_cov ? (float4 *)(b + o_wcov) : nullptr;
-    icp->src_col = want_col ? (float4 *)(b + o_col) : nullptr;
-    icp->st = (IcpState *)(b + o_st);
-    icp->partials = (double *)(b + o_part);
-    icp->tix_nrm = t_nrm ? (float4 *)(b + o_tn) : nullptr;
-    icp->tix_grad = t_grad ? (float4 *)(b + o_tg) : nullptr;
-    icp->tix_cov = t_cov ? (float4 *)(b + o_tc) : nullptr;
-    icp->tile_sums = (double *)(b + o_ts);
-    icp->flag_bits = (unsigned *)(b + o_fb);
-    icp->flag_words = flag_words;
-    icp->prev = (int2 *)(b + o_prev);
-    icp->corr_index = (int32_t *)(b + o_ci);
-    icp->cmp_counts = (unsigned *)(b + o_cc);
-    icp->cmp_total = (unsigned *)(b + o_ct);
+    icp->flag_words = n_pad / 1024 + 1;
+    cphb_arena &ar = icp->arena;
+    ar.slice(&icp->pristine_xyz, n_pad);
+    ar.slice(&icp->work_xyz, n_pad);
+    ar.slice(&icp->pristine_nrm, n_pad, want_nrm);
+    ar.slice(&icp->work_nrm, n_pad, want_nrm);
+    ar.slice(&icp->pristine_cov, 3 * n_pad, want_cov);
+    ar.slice(&icp->work_cov, 3 * n_pad, want_cov);
+    ar.slice(&icp->src_col, n_pad, want_col);
+    ar.slice(&icp->st, 1);
+    ar.slice(&icp->partials, 32 * (icp->reduce_grid > icp->grid ? icp->reduce_grid : icp->grid));
+    ar.slice(&icp->tix_nrm, nt_slice, t_nrm);
+    ar.slice(&icp->tix_grad, nt_slice, t_grad);
+    ar.slice(&icp->tix_cov, 3 * nt_slice, t_cov);
+    ar.slice(&icp->tile_sums, n_pad);
+    ar.slice(&icp->flag_bits, 2 * icp->flag_words);
+    ar.slice(&icp->prev, n_pad);
+    ar.slice(&icp->corr_index, nf_pad);
+    ar.slice(&icp->cmp_counts, (nf_pad + CMP_BLOCK - 1) / CMP_BLOCK + 1);
+    ar.slice(&icp->cmp_total, 4);
+    rc = ar.alloc(s);
+    if (rc) return rc;
     if (!t_cache.in_use) {
-        if (!t_cache.h_st) {
-            CREATE_TRY(cudaMallocHost((void **)&t_cache.h_st, sizeof(IcpState)));
-            CREATE_TRY(cudaEventCreate(&t_cache.ev0));
-            CREATE_TRY(cudaEventCreate(&t_cache.ev1));
-        }
+        if (!t_cache.h_st) CPHB_CUDA(cudaMallocHost((void **)&t_cache.h_st, sizeof(IcpState)));
+        if (!t_cache.ev0) CPHB_CUDA(cudaEventCreate(&t_cache.ev0));
+        if (!t_cache.ev1) CPHB_CUDA(cudaEventCreate(&t_cache.ev1));
         t_cache.in_use = true;
-        icp->owns_host = false;
         icp->h_st = t_cache.h_st;
         icp->ev0 = t_cache.ev0;
         icp->ev1 = t_cache.ev1;
     } else {  // a second live context on this thread gets its own
         icp->owns_host = true;
-        CREATE_TRY(cudaMallocHost((void **)&icp->h_st, sizeof(IcpState)));
-        CREATE_TRY(cudaEventCreate(&icp->ev0));
-        CREATE_TRY(cudaEventCreate(&icp->ev1));
+        CPHB_CUDA(cudaMallocHost((void **)&icp->h_st, sizeof(IcpState)));
+        CPHB_CUDA(cudaEventCreate(&icp->ev0));
+        CPHB_CUDA(cudaEventCreate(&icp->ev1));
     }
     if (t_source_ready) {  // (n_full == 0)
         cudaStreamWaitEvent(s, t_source_ready, 0);
@@ -361,32 +350,16 @@ extern "C" int cphb_icp_create(const cphb_cloud *source, const cphb_cloud *targe
     CPHB_LAUNCH(gather_source_kernel, n_pad / 256, 256, 0, s, source->points, source->normals, source->colors,
                 source->covariances, source->cov_col_major, perm_side, lo, n, n_pad, icp->pristine_xyz, icp->pristine_nrm,
                 icp->src_col, icp->pristine_cov);
-    cphb_free_async(perm_side, s);
-    perm_side = nullptr;
     if ((t_nrm || t_grad || t_cov) && nt_pad)
         CPHB_LAUNCH(gather_target_kernel, (unsigned)((nt_pad + 255) / 256), 256, 0, s, icp->index->v.pts, nt_pad, target->normals,
                     (est == CPHB_EST_COLORED_ICP) ? target->colors : nullptr, target->color_gradient, target->covariances,
                     target->cov_col_major, icp->tix_nrm, icp->tix_grad, icp->tix_cov);
-    CREATE_TRY(cudaGetLastError());
-    *out = icp;
+    CPHB_CUDA(cudaGetLastError());
+    *out = icp.release();
     return CPHB_OK;
 }
 
-#undef CREATE_TRY
-extern "C" void cphb_icp_destroy(cphb_icp *icp) {
-    if (!icp) return;
-    if (icp->arena) cudaFreeAsync(icp->arena, icp->stream);
-    if (icp->dbg) cudaFree(icp->dbg);
-    if (icp->owns_host) {
-        if (icp->h_st) cudaFreeHost(icp->h_st);
-        if (icp->ev0) cudaEventDestroy(icp->ev0);
-        if (icp->ev1) cudaEventDestroy(icp->ev1);
-    } else if (icp->h_st == t_cache.h_st) {
-        t_cache.in_use = false;
-    }
-    cphb_index_destroy(icp->index);
-    delete icp;
-}
+extern "C" void cphb_icp_destroy(cphb_icp *icp) { delete icp; }
 
 static void fill_args(const cphb_icp *icp, IcpArgs &a) {
     memset(&a, 0, sizeof(a));
@@ -438,7 +411,9 @@ static void fill_args(const cphb_icp *icp, IcpArgs &a) {
     a.tmax = CPHB_TRANSPOSE_MAX;
 }
 
-static int reset_working_copy(cphb_icp *icp, cudaStream_t s) {
+// the opening of a run or a step: the working copy back to the pristine source, and a fresh state at pose T (U = T) on
+// the device
+static int reset_state(cphb_icp *icp, const float T[16], int apply_u, cudaStream_t s) {
     CPHB_CUDA(cudaMemsetAsync(icp->flag_bits, 0, sizeof(unsigned) * 2 * icp->flag_words, s));
     CPHB_CUDA(cudaMemsetAsync(icp->prev, 0xff, sizeof(int2) * icp->n_pad, s));  // no warm start at launch 0
     CPHB_CUDA(cudaMemcpyAsync(icp->work_xyz, icp->pristine_xyz, sizeof(float4) * icp->n_pad, cudaMemcpyDeviceToDevice, s));
@@ -446,6 +421,12 @@ static int reset_working_copy(cphb_icp *icp, cudaStream_t s) {
         CPHB_CUDA(cudaMemcpyAsync(icp->work_nrm, icp->pristine_nrm, sizeof(float4) * icp->n_pad, cudaMemcpyDeviceToDevice, s));
     if (icp->work_cov)
         CPHB_CUDA(cudaMemcpyAsync(icp->work_cov, icp->pristine_cov, sizeof(float4) * 3 * icp->n_pad, cudaMemcpyDeviceToDevice, s));
+    IcpState *h = icp->h_st;
+    memset(h, 0, sizeof(*h));
+    memcpy(h->T, T, 64);
+    memcpy(h->U, T, 64);
+    h->apply_u = apply_u;
+    CPHB_CUDA(cudaMemcpyAsync(icp->st, h, sizeof(IcpState), cudaMemcpyHostToDevice, s));
     return CPHB_OK;
 }
 
@@ -467,14 +448,9 @@ extern "C" int cphb_icp_run(cphb_icp *icp, const float h_init[16], cphb_comm *co
         cphb_set_error("cphb_icp_run: null argument");
         return CPHB_ERR_INVALID;
     }
-    int rc = reset_working_copy(icp, s);
+    int rc = reset_state(icp, h_init, is_identity4(h_init) ? 0 : 1, s);
     if (rc) return rc;
     IcpState *h = icp->h_st;
-    memset(h, 0, sizeof(*h));
-    memcpy(h->T, h_init, 64);
-    memcpy(h->U, h_init, 64);
-    h->apply_u = is_identity4(h_init) ? 0 : 1;
-    CPHB_CUDA(cudaMemcpyAsync(icp->st, h, sizeof(IcpState), cudaMemcpyHostToDevice, s));
     static const bool dbg_cert = getenv("CPHB_DEBUG_CERT") != nullptr;
     if (dbg_cert) {
         if (!icp->dbg) CPHB_CUDA(cudaMalloc(&icp->dbg, sizeof(unsigned) * 256 + 128));
@@ -505,25 +481,17 @@ extern "C" int cphb_icp_run(cphb_icp *icp, const float h_init[16], cphb_comm *co
                            comm->world, icp->prm.shard_rank, icp->prm.shard_world);
             return CPHB_ERR_INVALID;
         }
-    }
-    if (comm && comm->world > 1 && lib_sharded) {
-        if (comm->kind == CPHB_COMM_NCCL) {
-            nccl_comm = comm->nccl;
-            a.defer_finalize = 1;
-        } else {
-            a.use_p2p = 1;
-            a.p2p = comm->view;
+        if (!lib_sharded) {
+            // caller-sharded source: global source size by one tiny exchange before the loop
+            double *tmp = icp->partials;  // scratch
+            double hn = (double)icp->n_src;
+            CPHB_CUDA(cudaMemcpyAsync(tmp, &hn, 8, cudaMemcpyHostToDevice, s));
+            rc = cphb_comm_allreduce_f64(comm, tmp, 1, s);
+            if (rc) return rc;
+            CPHB_CUDA(cudaMemcpyAsync(&hn, tmp, 8, cudaMemcpyDeviceToHost, s));
+            CPHB_CUDA(cudaStreamSynchronize(s));
+            n_total = (unsigned long long)hn;
         }
-    } else if (comm && comm->world > 1) {
-        // caller-sharded source: global source size by one tiny exchange before the loop
-        double *tmp = icp->partials;  // scratch
-        double hn = (double)icp->n_src;
-        CPHB_CUDA(cudaMemcpyAsync(tmp, &hn, 8, cudaMemcpyHostToDevice, s));
-        rc = cphb_comm_allreduce_f64(comm, tmp, 1, s);
-        if (rc) return rc;
-        CPHB_CUDA(cudaMemcpyAsync(&hn, tmp, 8, cudaMemcpyDeviceToHost, s));
-        CPHB_CUDA(cudaStreamSynchronize(s));
-        n_total = (unsigned long long)hn;
         if (comm->kind == CPHB_COMM_NCCL) {
             nccl_comm = comm->nccl;
             a.defer_finalize = 1;
@@ -626,14 +594,9 @@ extern "C" int cphb_icp_step(cphb_icp *icp, const float h_T[16], double h_sums[3
         cphb_set_error("cphb_icp_step: null argument");
         return CPHB_ERR_INVALID;
     }
-    int rc = reset_working_copy(icp, s);
+    int rc = reset_state(icp, h_T, 1, s);
     if (rc) return rc;
     IcpState *h = icp->h_st;
-    memset(h, 0, sizeof(*h));
-    memcpy(h->T, h_T, 64);
-    memcpy(h->U, h_T, 64);
-    h->apply_u = 1;
-    CPHB_CUDA(cudaMemcpyAsync(icp->st, h, sizeof(IcpState), cudaMemcpyHostToDevice, s));
     IcpArgs a;
     fill_args(icp, a);
     a.step_mode = 1;
@@ -694,73 +657,62 @@ extern "C" int cphb_registration_icp_host(const cphb_cloud *h_source, const cphb
         for (auto &e : t_up.ev) CPHB_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
     }
     const size_t ns = h_source->n, nt = h_target->n;
-    // device arena: [tgt points | src points, normals, colors, covariances | tgt normals, colors, covariances, gradient | pairs]
-    size_t off = 0;
-    auto take = [&](const void *hp, size_t bytes) { size_t o = off; if (hp) off = cphb_align(off + bytes, 256); return hp ? o : (size_t)-1; };
-    const size_t o_tp = take(h_target->points, 12 * nt);
-    const size_t o_sp = take(h_source->points, 12 * ns), o_sn = take(h_source->normals, 12 * ns), o_sc = take(h_source->colors, 12 * ns),
-                 o_sv = take(h_source->covariances, 36 * ns);
-    const size_t o_tn = take(h_target->normals, 12 * nt), o_tc = take(h_target->colors, 12 * nt),
-                 o_tv = take(h_target->covariances, 36 * nt), o_tg = take(h_target->color_gradient, 12 * nt);
-    const size_t o_pairs = take(h_corr_out, 8 * ns);
-    char *base = nullptr;
-    int rc = cphb_alloc_async((void **)&base, off ? off : 256, s);
-    if (rc) return rc;
-    auto dp = [&](size_t o) { return o == (size_t)-1 ? (float *)nullptr : (float *)(base + o); };
     cudaStream_t c = t_up.copy;
-    // one exit for CUDA errors: no upload may still be reading the caller's buffers, and the arena goes back to the pool
-#define HOST_TRY(call)                                                                                   \
-    do {                                                                                                 \
-        cudaError_t e__ = (call);                                                                        \
-        if (e__ != cudaSuccess) {                                                                        \
-            cphb_set_error("%s:%d %s: %s", __FILE__, __LINE__, #call, cudaGetErrorString(e__));          \
-            cudaStreamSynchronize(c);                                                                    \
-            cphb_free_async(base, s);                                                                    \
-            return CPHB_ERR_CUDA;                                                                        \
-        }                                                                                                \
-    } while (0)
-    HOST_TRY(cudaEventRecord(t_up.ev[0], s));            // the arena exists from here on in stream order
-    HOST_TRY(cudaStreamWaitEvent(c, t_up.ev[0], 0));
-    auto up = [&](size_t o, const void *hp, size_t bytes) {
-        if (hp && bytes) cudaMemcpyAsync(base + o, hp, bytes, cudaMemcpyHostToDevice, c);
-    };
-    up(o_tp, h_target->points, 12 * nt);
-    HOST_TRY(cudaEventRecord(t_up.ev[1], c));            // target points: all the index build needs
-    up(o_sp, h_source->points, 12 * ns);
-    up(o_sn, h_source->normals, 12 * ns);
-    up(o_sc, h_source->colors, 12 * ns);
-    up(o_sv, h_source->covariances, 36 * ns);
-    HOST_TRY(cudaEventRecord(t_up.ev[2], c));            // source: first read by the Hilbert ordering
-    up(o_tn, h_target->normals, 12 * nt);
-    up(o_tc, h_target->colors, 12 * nt);
-    up(o_tv, h_target->covariances, 36 * nt);
-    up(o_tg, h_target->color_gradient, 12 * nt);
-    HOST_TRY(cudaEventRecord(t_up.ev[3], c));            // target attributes: first read by the first iteration
+    scope_exit all_done{[&] { cudaStreamSynchronize(s); }};  // everything is complete on return, the arena's release included
+    // the clouds on the device, in one arena: [tgt points | src points, normals, colors, covariances | tgt normals, colors,
+    // covariances, gradient | pairs]
     cphb_cloud ds = *h_source, dt = *h_target;
-    ds.points = dp(o_sp); ds.normals = dp(o_sn); ds.colors = dp(o_sc); ds.covariances = dp(o_sv); ds.color_gradient = nullptr;
-    dt.points = dp(o_tp); dt.normals = dp(o_tn); dt.colors = dp(o_tc); dt.covariances = dp(o_tv); dt.color_gradient = dp(o_tg);
-    HOST_TRY(cudaStreamWaitEvent(s, t_up.ev[1], 0));
-#undef HOST_TRY
+    int32_t *d_pairs = nullptr;
+    cphb_arena arena;
+    arena.slice(&dt.points, 3 * nt, h_target->points);
+    arena.slice(&ds.points, 3 * ns, h_source->points);
+    arena.slice(&ds.normals, 3 * ns, h_source->normals);
+    arena.slice(&ds.colors, 3 * ns, h_source->colors);
+    arena.slice(&ds.covariances, 9 * ns, h_source->covariances);
+    arena.slice(&dt.normals, 3 * nt, h_target->normals);
+    arena.slice(&dt.colors, 3 * nt, h_target->colors);
+    arena.slice(&dt.covariances, 9 * nt, h_target->covariances);
+    arena.slice(&dt.color_gradient, 3 * nt, h_target->color_gradient);
+    arena.slice(&d_pairs, 2 * ns, h_corr_out);
+    ds.color_gradient = nullptr;
+    int rc = arena.alloc(s);
+    if (rc) return rc;
+    // declared after the arena, so it runs first: no upload may still be reading the caller's buffers, or writing into
+    // the arena, when the arena is freed
+    scope_exit uploads_done{[&] { cudaStreamSynchronize(c); }};
+    CPHB_CUDA(cudaEventRecord(t_up.ev[0], s));            // the arena exists from here on in stream order
+    CPHB_CUDA(cudaStreamWaitEvent(c, t_up.ev[0], 0));
+    auto up = [&](const float *d, const float *h, size_t floats) {
+        return h && floats ? cudaMemcpyAsync((void *)d, h, sizeof(float) * floats, cudaMemcpyHostToDevice, c) : cudaSuccess;
+    };
+    CPHB_CUDA(up(dt.points, h_target->points, 3 * nt));
+    CPHB_CUDA(cudaEventRecord(t_up.ev[1], c));            // target points: all the index build needs
+    CPHB_CUDA(up(ds.points, h_source->points, 3 * ns));
+    CPHB_CUDA(up(ds.normals, h_source->normals, 3 * ns));
+    CPHB_CUDA(up(ds.colors, h_source->colors, 3 * ns));
+    CPHB_CUDA(up(ds.covariances, h_source->covariances, 9 * ns));
+    CPHB_CUDA(cudaEventRecord(t_up.ev[2], c));            // source: first read by the Hilbert ordering
+    CPHB_CUDA(up(dt.normals, h_target->normals, 3 * nt));
+    CPHB_CUDA(up(dt.colors, h_target->colors, 3 * nt));
+    CPHB_CUDA(up(dt.covariances, h_target->covariances, 9 * nt));
+    CPHB_CUDA(up(dt.color_gradient, h_target->color_gradient, 3 * nt));
+    CPHB_CUDA(cudaEventRecord(t_up.ev[3], c));            // target attributes: first read by the first iteration
+    CPHB_CUDA(cudaStreamWaitEvent(s, t_up.ev[1], 0));
     t_source_ready = t_up.ev[2];
     cphb_icp *icp = nullptr;
     rc = cphb_icp_create(&ds, &dt, params, stream, &icp);
     t_source_ready = nullptr;
-    if (!rc) {
-        cudaStreamWaitEvent(s, t_up.ev[2], 0);            // (already waited inside create; harmless if it returned early)
-        cudaStreamWaitEvent(s, t_up.ev[3], 0);
-        int32_t *d_pairs = (int32_t *)dp(o_pairs);
-        rc = cphb_icp_run(icp, h_init, comm, h_result, d_pairs, stream);
-        if (!rc && h_corr_out && h_result->n_local_correspondences > 0) {
-            cudaError_t e = cudaMemcpyAsync(h_corr_out, d_pairs, sizeof(int32_t) * 2 * (size_t)h_result->n_local_correspondences,
-                                            cudaMemcpyDeviceToHost, s);
-            if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-            if (e != cudaSuccess) { cphb_set_error("cphb_registration_icp_host: %s", cudaGetErrorString(e)); rc = CPHB_ERR_CUDA; }
-        }
-        cphb_icp_destroy(icp);
+    if (rc) return rc;
+    cudaStreamWaitEvent(s, t_up.ev[2], 0);            // (already waited inside create; harmless if it returned early)
+    cudaStreamWaitEvent(s, t_up.ev[3], 0);
+    rc = cphb_icp_run(icp, h_init, comm, h_result, d_pairs, stream);
+    if (!rc && h_corr_out && h_result->n_local_correspondences > 0) {
+        cudaError_t e = cudaMemcpyAsync(h_corr_out, d_pairs, sizeof(int32_t) * 2 * (size_t)h_result->n_local_correspondences,
+                                        cudaMemcpyDeviceToHost, s);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+        if (e != cudaSuccess) { cphb_set_error("cphb_registration_icp_host: %s", cudaGetErrorString(e)); rc = CPHB_ERR_CUDA; }
     }
-    cudaStreamSynchronize(c);                              // no upload may outlive the host buffers or the arena
-    cphb_free_async(base, s);
-    cudaStreamSynchronize(s);
+    cphb_icp_destroy(icp);
     return rc;
 }
 
@@ -824,15 +776,14 @@ static int run_estimate(int estimation, const cphb_cloud *source, const cphb_clo
     a.corr = corr;
     a.n_corr = (unsigned)n_corr;
     unsigned grid = (unsigned)((n_corr + ICP_BLOCK - 1) / ICP_BLOCK);
-    cphb_scratch sc(s);
-    char *buf = nullptr;
-    size_t bytes = cphb_align(sizeof(double) * 32 * grid, 256) + 256 + 256 + 64;
-    int rc = sc.alloc(&buf, bytes);
+    cphb_arena arena;
+    float *Td;
+    arena.slice(&a.partials, 32 * (size_t)grid);
+    arena.slice(&a.total, 32);
+    arena.slice(&a.ticket, 1);
+    arena.slice(&Td, 16);
+    int rc = arena.alloc(s);
     if (rc) return rc;
-    a.partials = (double *)buf;
-    a.total = (double *)(buf + cphb_align(sizeof(double) * 32 * grid, 256));
-    a.ticket = (unsigned *)((char *)a.total + 256);
-    float *Td = (float *)((char *)a.total + 512);
     CPHB_CUDA(cudaMemsetAsync(a.ticket, 0, 4, s));
     // the inputs the estimator needs are present (otherwise the solve leaves the identity)
     const bool have = estimation == CPHB_EST_POINT_TO_PLANE ? target->normals != nullptr

@@ -12,6 +12,8 @@
 
 #include <stdlib.h>
 
+#include <memory>
+
 #include "cphb_internal.cuh"
 
 // ---------------------------------------------------------------------------
@@ -511,10 +513,9 @@ int cphb_hilbert_order_n(const float *xyz, size_t n, uint32_t *perm_out, float *
     return cphb_sort_pairs_u32(keys, keys2, vals, perm_out, n, 3 * levels, s);
 }
 
-// fills the zeroed handle ix; on failure the caller destroys it (with its arena, if one was allocated)
+// fills the new handle ix; on failure the caller destroys it (with its arena, if one was allocated)
 static int index_build(cphb_index *ix, const float *xyz, size_t n, cudaStream_t s) {
     CPHB_CUDA(cudaGetDevice(&ix->device));
-    ix->stream = s;
     size_t count[CPHB_LEVELS], pad[CPHB_LEVELS];
     count[0] = (n + CPHB_LEAF - 1) / CPHB_LEAF;
     for (int l = 0; l < CPHB_LEVELS; ++l) {
@@ -526,30 +527,16 @@ static int index_build(cphb_index *ix, const float *xyz, size_t n, cudaStream_t 
         return CPHB_ERR_INVALID;
     }
     size_t n_pad = (count[0] ? count[0] : 1) * CPHB_LEAF;
-    size_t off_pts = 0;
-    size_t off = cphb_align(n_pad * sizeof(float4), 256);
-    size_t off_box[CPHB_LEVELS];
-    for (int l = 0; l < CPHB_LEVELS; ++l) {
-        off_box[l] = off;
-        off = cphb_align(off + pad[l] * sizeof(Box), 256);
-    }
-    size_t off_bounds = off;
-    off += 256;
-    size_t off_perm = off;
-    off = cphb_align(off + sizeof(uint32_t) * (n ? n : 1), 256);
-    size_t off_inv = off;
-    off = cphb_align(off + sizeof(uint32_t) * (n ? n : 1), 256);
-    ix->arena_bytes = off;
-    char *base = nullptr;
-    int rc = cphb_alloc_async((void **)&base, off, s);
-    if (rc) return rc;
-    ix->arena = base;
-    float4 *pts = (float4 *)(base + off_pts);
+    float4 *pts;
     Box *boxes[CPHB_LEVELS];
-    for (int l = 0; l < CPHB_LEVELS; ++l) boxes[l] = (Box *)(base + off_box[l]);
-    ix->bounds = (float *)(base + off_bounds);
-    uint32_t *perm = (uint32_t *)(base + off_perm);
-    uint32_t *inv = (uint32_t *)(base + off_inv);
+    uint32_t *perm, *inv;
+    ix->arena.slice(&pts, n_pad);
+    for (int l = 0; l < CPHB_LEVELS; ++l) ix->arena.slice(&boxes[l], pad[l]);
+    ix->arena.slice(&ix->bounds, 6);
+    ix->arena.slice(&perm, n ? n : 1);
+    ix->arena.slice(&inv, n ? n : 1);
+    int rc = ix->arena.alloc(s);
+    if (rc) return rc;
 
     if (n) {
         rc = cphb_hilbert_order(xyz, n, perm, ix->bounds, 0, s);
@@ -589,22 +576,14 @@ extern "C" int cphb_index_create(const float *xyz, size_t n, void *stream, cphb_
         cphb_set_error("cphb_index_create: n=%zu exceeds int32 indices", n);
         return CPHB_ERR_INVALID;
     }
-    cphb_index *ix = new cphb_index();
-    memset(ix, 0, sizeof(*ix));
-    const int rc = index_build(ix, xyz, n, (cudaStream_t)stream);
-    if (rc) {
-        cphb_index_destroy(ix);
-        return rc;
-    }
-    *out = ix;
+    std::unique_ptr<cphb_index> ix(new cphb_index());
+    const int rc = index_build(ix.get(), xyz, n, (cudaStream_t)stream);
+    if (rc) return rc;
+    *out = ix.release();
     return CPHB_OK;
 }
 
-extern "C" void cphb_index_destroy(cphb_index *ix) {
-    if (!ix) return;
-    if (ix->arena) cudaFreeAsync(ix->arena, ix->stream);
-    delete ix;
-}
+extern "C" void cphb_index_destroy(cphb_index *ix) { delete ix; }
 extern "C" size_t cphb_index_size(const cphb_index *ix) { return ix ? (size_t)ix->v.n : 0; }
 
 extern "C" int cphb_min_max_bound(const float *points, size_t n, float h_min[3], float h_max[3], void *stream) {

@@ -1,6 +1,7 @@
-// Host-only check of cphb_scratch (cupoch_b200/csrc/cphb_internal.cuh) against recording stubs of the allocator:
-// every buffer it hands out is freed exactly once, on its stream, whichever way the scope is left.  Launches nothing
-// and needs no device.  Exit code 0 = all checks passed.
+// Host-only check of cphb_scratch and cphb_arena (cupoch_b200/csrc/cphb_internal.cuh) against recording stubs of the
+// allocator: every buffer they hand out is freed exactly once, on its stream, whichever way the scope is left, and an
+// arena lays its slices out at 256-byte-aligned running offsets.  Launches nothing and needs no device.  Exit code 0 =
+// all checks passed.
 #include <stdarg.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -138,6 +139,56 @@ int main() {
         EXPECT(extra == nullptr && g_allocs == CPHB_SCRATCH_SLOTS && g_err[0] != 0);
     }
     EXPECT(count(true) == CPHB_SCRATCH_SLOTS && count(false) == CPHB_SCRATCH_SLOTS && balanced());
+
+    // cphb_arena: each slice starts at the running offset, which then moves to the next multiple of 256; an absent
+    // slice is null and takes no bytes; one allocation of the total on the given stream, freed once on it at the end
+    reset();
+    {
+        cphb_arena ar;
+        float *a = nullptr;
+        double *b = (double *)&ar;
+        int32_t *c = nullptr;
+        char *d = nullptr;
+        uint8_t *e = nullptr;
+        ar.slice(&a, 10);           // [0, 40)
+        ar.slice(&b, 1000, false);  // absent
+        ar.slice(&c, 64);           // [256, 512)
+        ar.slice(&d, 0);            // empty, at 512
+        ar.slice(&e, 257);          // [512, 769)
+        EXPECT(ar.bytes() == 1024 && g_calls.empty() && !a && !b && !c);
+        EXPECT(ar.alloc(S) == CPHB_OK);
+        EXPECT(g_calls.size() == 1 && g_calls[0].alloc && g_calls[0].bytes == 1024 && g_calls[0].s == S);
+        char *base = (char *)g_calls[0].p;
+        EXPECT((char *)a == base && !b && (char *)c == base + 256 && d == base + 512 && (char *)e == base + 512);
+    }
+    EXPECT(count(true) == 1 && count(false) == 1 && balanced());
+
+    // a failed allocation leaves every pointer null and frees nothing
+    reset(0);
+    {
+        cphb_arena ar;
+        float *a = nullptr, *b = nullptr;
+        ar.slice(&a, 4);
+        ar.slice(&b, 4);
+        EXPECT(ar.alloc(S) == CPHB_ERR_CUDA && !a && !b);
+    }
+    EXPECT(g_calls.empty());
+
+    // a move hands the block over: the moved-from arena frees nothing, the new owner frees it once
+    reset();
+    {
+        cphb_arena *owner = nullptr;
+        {
+            cphb_arena ar;
+            float *a = nullptr;
+            ar.slice(&a, 4);
+            EXPECT(ar.alloc(S) == CPHB_OK && a);
+            owner = new cphb_arena(std::move(ar));
+        }
+        EXPECT(count(false) == 0);
+        delete owner;
+    }
+    EXPECT(count(true) == 1 && count(false) == 1 && balanced());
 
     if (g_failed) {
         fprintf(stderr, "scratch_check: %d failed\n", g_failed);

@@ -296,3 +296,56 @@ def test_user_defined_estimator_generic_loop(orc):
     # host-buffer entry point takes the same route
     res_h = R.registration_icp_host(src, tgt, 0.03, init, Mine(), crit, target_normals=tn, return_correspondences=True)
     np.testing.assert_array_equal(res_h.transformation, res.transformation)
+
+
+def test_create_checks_shard_rank_before_any_work():
+    """an out-of-range shard rank is refused with the other argument checks: no source ordering, no index build, no
+    launch"""
+    import ctypes as C
+    L = cph._lib.lib()
+    src, sn, tgt, tn = small_pair(2000)
+    s, t = cloud(src), cloud(tgt)
+    p = R._params(R.TransformationEstimationPointToPoint(), 0.03, R.ICPConvergenceCriteria(), shard=(5, 2))
+    sc, tc = s._cloud(), t._cloud()
+    h = C.c_void_p()
+    before = L.cphb_launch_count()
+    rc = L.cphb_icp_create(C.byref(sc), C.byref(tc), C.byref(p), None, C.byref(h))
+    assert rc == cph._lib.CPHB_ERR_INVALID
+    assert "shard_rank 5 outside [0,2)" in L.cphb_last_error().decode()
+    assert L.cphb_launch_count() == before and not h.value
+
+
+@pytest.mark.parametrize("close_first", [0, 1])
+def test_two_live_contexts_match_a_lone_one(close_first):
+    """the second live context on a thread has its own pinned staging: both give a lone context's bits, whichever
+    is closed first"""
+    src, sn, tgt, tn = small_pair()
+    init = datagen.gt_transform((-0.3, 0.2, 0.4), (0.002, 0.0, -0.001)).astype(np.float32)
+    crit = R.ICPConvergenceCriteria(0, 0, 12)
+    make = lambda: R.IcpContext(cloud(src), cloud(tgt, tn), 0.03, R.TransformationEstimationPointToPlane(), crit)
+    lone = make()
+    ref = lone.run(init)
+    ref_step = lone.step(init)
+    lone.close()
+    ctx = [make(), make()]
+    try:
+        for c in ctx:
+            r = c.run(init)
+            np.testing.assert_array_equal(r.transformation, ref.transformation)
+            np.testing.assert_array_equal(r.correspondence_set, ref.correspondence_set)
+            assert (r.iterations, r.fitness, r.inlier_rmse) == (ref.iterations, ref.fitness, ref.inlier_rmse)
+        ctx[close_first].close()
+        other = ctx[1 - close_first]
+        sums, ci = other.step(init)
+        np.testing.assert_array_equal(sums, ref_step[0])
+        np.testing.assert_array_equal(ci, ref_step[1])
+        r = other.run(init)
+        np.testing.assert_array_equal(r.transformation, ref.transformation)
+        again = make()  # takes over whatever staging the closed context released
+        try:
+            np.testing.assert_array_equal(again.run(init).transformation, ref.transformation)
+        finally:
+            again.close()
+    finally:
+        for c in ctx:
+            c.close()

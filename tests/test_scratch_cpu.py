@@ -1,5 +1,6 @@
-"""cphb_scratch, the owner of an entry point's device scratch (cupoch_b200/csrc/cphb_internal.cuh): the type checked on
-the host against recording stubs of the allocator, and a source check that no hand-written free list comes back."""
+"""cphb_scratch and cphb_arena, the owners of an entry point's device scratch and of a handle's device block
+(cupoch_b200/csrc/cphb_internal.cuh): the types checked on the host against recording stubs of the allocator, and a
+source check that no hand-written free list comes back."""
 import os
 import re
 import subprocess
@@ -9,14 +10,13 @@ import pytest
 from conftest import ROOT
 from cupoch_b200.build import FLAGS, NVCC, SRC
 
-# the only places that may call cphb_free_async: the allocator and the owner themselves (None: the whole file), the ICP
-# context, and the storage that outlives a call -- the distance transform's grid, the occupancy grid, the neighbour table
+# the only places that may call cphb_free_async or cudaFreeAsync: the owners themselves (None: the whole file), the
+# allocator, and the storage that outlives a call -- the distance transform's grid, the occupancy grid, the neighbour table
 FREE_ALLOWED = {
     "cphb_internal.cuh": None,
-    "index.cu": None,
-    "icp.cu": None,
-    "edt.cu": {"edt_alloc_grid", "cphb_dt_reconstruct"},
-    "occgrid.cu": {"cphb_occgrid_create"},
+    "index.cu": {"cphb_free_async", "cphb_reserve_pool", "cphb_free"},
+    "edt.cu": {"edt_alloc_grid", "cphb_dt_reconstruct", "cphb_dt_destroy"},
+    "occgrid.cu": {"cphb_occgrid_create", "cphb_occgrid_destroy"},
     "search.cu": {"cphb_nbr_table_release"},
 }
 # a function definition starts in column 0: [extern "C"] [static] <type> <name>(
@@ -45,6 +45,6 @@ def test_no_hand_written_free_lists():
                 m = _DEF.match(line)
                 if m:
                     func = m.group(1)
-                if "cphb_free_async(" in line and allowed is not None and func not in allowed:
+                if ("cphb_free_async(" in line or "cudaFreeAsync(" in line) and allowed is not None and func not in allowed:
                     stray.append("%s:%d in %s" % (name, no, func))
-    assert not stray, "call-scoped device scratch belongs to a cphb_scratch: " + ", ".join(stray)
+    assert not stray, "device storage belongs to a cphb_scratch or a cphb_arena: " + ", ".join(stray)

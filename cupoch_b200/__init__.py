@@ -15,7 +15,7 @@ cph.utility.{Vector3fVector, compute_jtj_jtr, compute_weighted_jtj_jtr}; cupoch_
 multi-GPU orchestration (torch.distributed).  All computation runs in libcupoch_b200.so (hand-written sm_90a CUDA);
 there is no CPU fallback.
 """
-from . import _lib, collision, geometry, registration, utility  # noqa: F401
+from . import _lib, camera, collision, geometry, registration, utility  # noqa: F401
 
 __version__ = "0.1.0"
 

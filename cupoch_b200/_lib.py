@@ -60,6 +60,17 @@ _I3 = C.POINTER(C.c_int32)
 _SIGNATURES = {
     "cphb_compute_intersection": (C.c_int, [C.POINTER(CollOperand), C.POINTER(CollOperand), C.c_float, _P, C.c_size_t,
                                             C.POINTER(C.c_size_t), _P]),
+    "cphb_voxel_grid_create_dense": (C.c_int, [C.c_float, C.c_float, C.c_float, C.c_float, _P, _P, C.c_size_t,
+                                               C.POINTER(C.c_size_t), _P]),
+    "cphb_voxel_grid_check_if_included": (C.c_int, [_P, C.c_size_t, C.c_float, _F3, _P, C.c_size_t, _P, _P]),
+    "cphb_voxel_grid_has_key": (C.c_int, [_P, C.c_size_t, _I3, C.POINTER(C.c_int), _P]),
+    "cphb_voxel_grid_carve": (C.c_int, [_P, _P, C.c_size_t, C.c_float, _F3, _P, C.c_int, C.c_int, C.c_int, C.c_int, _F3, _F3,
+                                        C.c_int, _P, _P, C.POINTER(C.c_size_t), _P]),
+    "cphb_voxel_grid_merge": (C.c_int, [_P, _P, C.c_size_t, _P, _P, C.c_size_t, C.c_int, _P, _P, C.POINTER(C.c_size_t), _P]),
+    "cphb_voxel_grid_paint": (C.c_int, [_P, C.c_size_t, _P, C.c_size_t, _F3, _P]),
+    "cphb_voxel_grid_select_by_index": (C.c_int, [_P, _P, C.c_size_t, _P, C.c_size_t, C.c_int, _P, _P, C.POINTER(C.c_size_t), _P]),
+    "cphb_voxel_grid_from_occgrid": (C.c_int, [_P, _P, _P, C.c_size_t, C.POINTER(C.c_size_t), _F3, _P]),
+    "cphb_point_cloud_from_occgrid": (C.c_int, [_P, _P, _P, C.c_size_t, C.POINTER(C.c_size_t), _P]),
     "cphb_occgrid_default_params": (None, [C.POINTER(OccGridParams)]),
     "cphb_occgrid_create": (C.c_int, [C.c_float, C.c_int, _F3, _P, C.POINTER(_P)]),
     "cphb_occgrid_destroy": (None, [_P]),

@@ -28,10 +28,9 @@
 #include <math.h>
 #include <string.h>
 
-#include "cphb_internal.cuh"
+#include "voxelkey.cuh"
 
 #define COLL_BLOCK 256
-#define COLL_AXIS_BITS 21
 
 // A grid as the kernels see it.  Element key k covers [k * vs + o, (k + 1) * vs + o]; every element's key lies in
 // [lo, hi].  VoxelGrid: element i is keys[i], its index i.  OccupancyGrid: cell = k + half, index = linear cell index.
@@ -51,10 +50,6 @@ struct CollGrid {
     float thres;
 };
 
-__device__ __forceinline__ uint64_t coll_pack(const CollGrid &g, int x, int y, int z) {
-    return ((uint64_t)(uint32_t)(x - g.lo[0]) << (2 * COLL_AXIS_BITS)) | ((uint64_t)(uint32_t)(y - g.lo[1]) << COLL_AXIS_BITS) |
-           (uint64_t)(uint32_t)(z - g.lo[2]);
-}
 __device__ __forceinline__ int occ_linear(const CollGrid &g, int x, int y, int z) {
     return ((x + g.half) * g.res + (y + g.half)) * g.res + (z + g.half);
 }
@@ -99,17 +94,11 @@ __device__ __forceinline__ bool key_range(const CollGrid &g, const float blo[3],
 // lookups: f(key, index) for every element of g in the row (x, y, z0..z1), or in a cell
 template <class F>
 __device__ __forceinline__ void vg_row(const CollGrid &g, int x, int y, int z0, int z1, F &f) {
-    const uint64_t kl = coll_pack(g, x, y, z0), kh = coll_pack(g, x, y, z1);
-    size_t a = 0, b = g.n;
-    while (a < b) {
-        const size_t m = (a + b) >> 1;
-        if (g.skeys[m] < kl) a = m + 1;
-        else b = m;
-    }
-    for (; a < g.n; ++a) {
+    const uint64_t kl = cphb_key_pack(g.lo, x, y, z0), kh = cphb_key_pack(g.lo, x, y, z1);
+    for (size_t a = cphb_key_lower_bound(g.skeys, g.n, kl); a < g.n; ++a) {
         const uint64_t k = g.skeys[a];
         if (k > kh) break;
-        const int key[3] = {x, y, g.lo[2] + (int)(k & ((1ull << COLL_AXIS_BITS) - 1))};
+        const int key[3] = {x, y, g.lo[2] + (int)(k & ((1ull << CPHB_KEY_AXIS_BITS) - 1))};
         f(key, (int)g.sidx[a]);
     }
 }
@@ -300,10 +289,12 @@ __global__ void __launch_bounds__(COLL_BLOCK) coll_key_bounds_kernel(const int32
     if (threadIdx.x < 3) atomicMin(&b[threadIdx.x], s[threadIdx.x]);
     else if (threadIdx.x < 6) atomicMax(&b[threadIdx.x], s[threadIdx.x]);
 }
-__global__ void __launch_bounds__(COLL_BLOCK) coll_pack_kernel(const CollGrid g, uint64_t *packed, uint32_t *idx) {
+__global__ void __launch_bounds__(COLL_BLOCK) coll_pack_kernel(const int32_t *__restrict__ keys, size_t n, int3 lo3, uint64_t *packed,
+                                                                uint32_t *idx) {
     const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
-    if (i >= g.n) return;
-    packed[i] = coll_pack(g, g.keys[3 * i], g.keys[3 * i + 1], g.keys[3 * i + 2]);
+    if (i >= n) return;
+    const int lo[3] = {lo3.x, lo3.y, lo3.z};
+    packed[i] = cphb_key_pack(lo, keys[3 * i], keys[3 * i + 1], keys[3 * i + 2]);
     idx[i] = (uint32_t)i;
 }
 // the occupied cells of an OccupancyGrid query's bound box (box order = ascending linear index)
@@ -565,6 +556,39 @@ __global__ void __launch_bounds__(COLL_BLOCK) coll_gather_kernel(const int32_t *
 // ---------------------------------------------------------------------------------------------------------------------
 // host
 // ---------------------------------------------------------------------------------------------------------------------
+int cphb_sort_voxel_keys(const int32_t *keys, size_t n, cphb_scratch &sc, cphb_sorted_keys *out, cudaStream_t s, const char *who) {
+    int *d_b = nullptr;
+    uint64_t *pk = nullptr, *pk2 = nullptr;
+    uint32_t *ix = nullptr, *ix2 = nullptr;
+    int rc = sc.alloc(&d_b, 6);
+    if (!rc) rc = sc.alloc(&pk, n);
+    if (!rc) rc = sc.alloc(&pk2, n);
+    if (!rc) rc = sc.alloc(&ix, n);
+    if (!rc) rc = sc.alloc(&ix2, n);
+    if (rc) return rc;
+    const int init[6] = {INT_MAX, INT_MAX, INT_MAX, INT_MIN, INT_MIN, INT_MIN};
+    CPHB_CUDA(cudaMemcpyAsync(d_b, init, sizeof(init), cudaMemcpyHostToDevice, s));
+    const unsigned grid = (unsigned)((n + COLL_BLOCK - 1) / COLL_BLOCK);
+    CPHB_LAUNCH(coll_key_bounds_kernel, grid < CPHB_SMS * 8 ? grid : CPHB_SMS * 8, COLL_BLOCK, 0, s, keys, n, d_b);
+    int hb[6];
+    rc = cphb_read_back(hb, d_b, sizeof(hb), s, who);
+    if (rc) return rc;
+    for (int x = 0; x < 3; ++x) {
+        if ((long long)hb[3 + x] - (long long)hb[x] >= (1ll << CPHB_KEY_AXIS_BITS)) {
+            cphb_set_error("%s: VoxelGrid keys span %lld >= 2^21 on axis %d", who, (long long)hb[3 + x] - (long long)hb[x] + 1, x);
+            return CPHB_ERR_INVALID;
+        }
+        out->lo[x] = hb[x];
+        out->hi[x] = hb[3 + x];
+    }
+    CPHB_LAUNCH(coll_pack_kernel, grid, COLL_BLOCK, 0, s, keys, n, make_int3(hb[0], hb[1], hb[2]), pk, ix);
+    rc = cphb_sort_pairs_u64(pk, pk2, ix, ix2, n, 3 * CPHB_KEY_AXIS_BITS, s);
+    if (rc) return rc;
+    out->skeys = pk2;
+    out->sidx = ix2;
+    return CPHB_OK;
+}
+
 static bool vs_ok(float vs) { return isfinite(vs) && vs > 0.f; }
 
 // grid operand -> CollGrid with its element count (VoxelGrid: keys; OccupancyGrid: the bound box volume, enumerated later)
@@ -659,36 +683,15 @@ extern "C" int cphb_compute_intersection(const cphb_coll_operand *a, const cphb_
     }
     // VoxelGrid target: key bounds, then the packed keys sorted with their indices
     if (!a_prim && !t.occ) {
-        int *d_b = nullptr;
-        uint64_t *pk = nullptr, *pk2 = nullptr;
-        uint32_t *ix = nullptr, *ix2 = nullptr;
-        rc = sc.alloc(&d_b, 6);
-        if (!rc) rc = sc.alloc(&pk, t.n);
-        if (!rc) rc = sc.alloc(&pk2, t.n);
-        if (!rc) rc = sc.alloc(&ix, t.n);
-        if (!rc) rc = sc.alloc(&ix2, t.n);
-        if (rc) return rc;
-        const int init[6] = {INT_MAX, INT_MAX, INT_MAX, INT_MIN, INT_MIN, INT_MIN};
-        CPHB_CUDA(cudaMemcpyAsync(d_b, init, sizeof(init), cudaMemcpyHostToDevice, s));
-        const unsigned grid = (unsigned)((t.n + COLL_BLOCK - 1) / COLL_BLOCK);
-        CPHB_LAUNCH(coll_key_bounds_kernel, grid < CPHB_SMS * 8 ? grid : CPHB_SMS * 8, COLL_BLOCK, 0, s, t.keys, t.n, d_b);
-        int hb[6];
-        rc = cphb_read_back(hb, d_b, sizeof(hb), s, "cphb_compute_intersection");
+        cphb_sorted_keys sk;
+        rc = cphb_sort_voxel_keys(t.keys, t.n, sc, &sk, s, "cphb_compute_intersection");
         if (rc) return rc;
         for (int x = 0; x < 3; ++x) {
-            if ((long long)hb[3 + x] - (long long)hb[x] >= (1ll << COLL_AXIS_BITS)) {
-                cphb_set_error("cphb_compute_intersection: VoxelGrid target keys span %lld >= 2^21 on axis %d",
-                               (long long)hb[3 + x] - (long long)hb[x] + 1, x);
-                return CPHB_ERR_INVALID;
-            }
-            t.lo[x] = hb[x];
-            t.hi[x] = hb[3 + x];
+            t.lo[x] = sk.lo[x];
+            t.hi[x] = sk.hi[x];
         }
-        CPHB_LAUNCH(coll_pack_kernel, grid, COLL_BLOCK, 0, s, t, pk, ix);
-        rc = cphb_sort_pairs_u64(pk, pk2, ix, ix2, t.n, 3 * COLL_AXIS_BITS, s);
-        if (rc) return rc;
-        t.skeys = pk2;
-        t.sidx = ix2;
+        t.skeys = sk.skeys;
+        t.sidx = sk.sidx;
     }
     // the query's elements
     size_t nq = b_prim ? b->n : q.n;

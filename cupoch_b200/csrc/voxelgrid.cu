@@ -9,7 +9,7 @@
 // bit-exact.
 #include <math.h>
 
-#include "cphb_internal.cuh"
+#include "voxelkey.cuh"
 
 struct VgParams {
     float org[3];
@@ -184,4 +184,484 @@ extern "C" int cphb_voxel_indices(const float *points, size_t n, float voxel_siz
                 out_indices);
     CPHB_CHECK_LAUNCH();
     return CPHB_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// The rest of VoxelGrid (voxelgrid.cu:235-475, voxelgrid_factory.cu:134-162,283-305; SURVEY 8f rank 12).  Every
+// operation is a fixed number of coalesced passes: CreateDense writes keys already in lexicographic order (no sort, no
+// unique); lookups and merges go through the packed-key sort of voxelkey.cuh (one sort per call, then a binary
+// search per query or a head-flag compaction); carving and the inverted selection are a flag kernel, the stable
+// compaction and a gather, so survivors keep their order.
+// ---------------------------------------------------------------------------------------------------------------------
+#define VGO_BLOCK 256
+static unsigned vgo_grid(size_t n) { return (unsigned)((n + VGO_BLOCK - 1) / VGO_BLOCK); }
+// at least one block: a launch whose work can be empty (no survivors) still happens, so the launch count of a call does
+// not depend on its data
+static unsigned vgo_grid1(size_t n) { return n ? vgo_grid(n) : 1u; }
+static unsigned vgo_capped(size_t n) {
+    const unsigned g = vgo_grid(n);
+    return g < CPHB_SMS * 32 ? g : CPHB_SMS * 32;
+}
+static int vgo_invalid(const char *who, const char *what) {
+    cphb_set_error("%s: %s", who, what);
+    return CPHB_ERR_INVALID;
+}
+
+// create_dense_functor (voxelgrid_factory.cu:42-55): voxel i is (i / (nh nd), (i / nd) % nh, i % nd)
+template <class I>
+__global__ void __launch_bounds__(VGO_BLOCK) vgo_dense_kernel(I total, I nh, I nd, int32_t *__restrict__ keys, float *__restrict__ colors) {
+    for (I i = blockIdx.x * (I)blockDim.x + threadIdx.x; i < total; i += (I)gridDim.x * blockDim.x) {
+        const I hd = nh * nd;
+        const I w = i / hd, r = i - w * hd, h = r / nd;
+        keys[3 * (size_t)i] = (int32_t)w;
+        keys[3 * (size_t)i + 1] = (int32_t)h;
+        keys[3 * (size_t)i + 2] = (int32_t)(r - h * nd);
+        colors[3 * (size_t)i] = 1.f;
+        colors[3 * (size_t)i + 1] = 1.f;
+        colors[3 * (size_t)i + 2] = 1.f;
+    }
+}
+
+extern "C" int cphb_voxel_grid_create_dense(float voxel_size, float width, float height, float depth, int32_t *out_keys,
+                                            float *out_colors, size_t capacity, size_t *h_n, void *stream) {
+    cudaStream_t s = (cudaStream_t)stream;
+    const char *who = "cphb_voxel_grid_create_dense";
+    if (!h_n) return vgo_invalid(who, "null argument");
+    *h_n = 0;
+    if (!(isfinite(voxel_size) && voxel_size > 0.f)) return vgo_invalid(who, "voxel_size is not positive and finite");
+    const float ext[3] = {width, height, depth};
+    unsigned long long cnt[3];
+    for (int a = 0; a < 3; ++a) {
+        const volatile float q = ext[a] / voxel_size;  // int(std::round(w / voxel_size)) in float
+        const float c = roundf(q);
+        if (!(c >= 0.f && c < 2147483648.f)) {
+            cphb_set_error("%s: axis %d count round(%g / %g) is negative, not finite or >= 2^31", who, a, (double)ext[a],
+                           (double)voxel_size);
+            return CPHB_ERR_INVALID;
+        }
+        cnt[a] = (unsigned long long)c;
+    }
+    // the total in 64 bits, with its keys and colours (24 bytes a voxel) addressable by size_t
+    const unsigned long long lim = (unsigned long long)(SIZE_MAX / 24);
+    unsigned long long total = cnt[0];
+    if (cnt[1] && total > lim / cnt[1]) return vgo_invalid(who, "voxel count overflows");
+    total *= cnt[1];
+    if (cnt[2] && total > lim / cnt[2]) return vgo_invalid(who, "voxel count overflows");
+    total *= cnt[2];
+    *h_n = (size_t)total;
+    if (total == 0 || capacity < total) return CPHB_OK;
+    if (!out_keys || !out_colors) return vgo_invalid(who, "null output");
+    // the 32-bit index path only when the grid-stride step cannot wrap past 2^32
+    if (total <= 0xffffffffull - (unsigned long long)vgo_capped(total) * VGO_BLOCK)
+        CPHB_LAUNCH(vgo_dense_kernel<uint32_t>, vgo_capped(total), VGO_BLOCK, 0, s, (uint32_t)total, (uint32_t)cnt[1], (uint32_t)cnt[2],
+                    out_keys, out_colors);
+    else
+        CPHB_LAUNCH(vgo_dense_kernel<unsigned long long>, vgo_capped(total), VGO_BLOCK, 0, s, total, cnt[1], cnt[2], out_keys, out_colors);
+    CPHB_CHECK_LAUNCH();
+    return CPHB_OK;
+}
+
+// CheckIfIncluded: the GetVoxel cell of each query, looked up among the sorted packed keys
+__global__ void __launch_bounds__(VGO_BLOCK) vgo_included_kernel(const uint64_t *__restrict__ skeys, size_t n, int3 lo3, int3 hi3,
+                                                                 float voxel, float ox, float oy, float oz,
+                                                                 const float *__restrict__ q, size_t nq, uint8_t *__restrict__ out) {
+    const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+    if (i >= nq) return;
+    const int lo[3] = {lo3.x, lo3.y, lo3.z}, hi[3] = {hi3.x, hi3.y, hi3.z};
+    const float o[3] = {ox, oy, oz};
+    int k[3];
+    bool in = true;
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+        // vg_index's expression; a NaN or out-of-range floor fails the test before the cast
+        const float f = floorf(__fdiv_rn(__fsub_rn(q[3 * i + a], o[a]), voxel));
+        in = in && (double)f >= (double)lo[a] && (double)f <= (double)hi[a];
+        k[a] = in ? (int)f : lo[a];
+    }
+    if (in) {
+        const uint64_t key = cphb_key_pack(lo, k[0], k[1], k[2]);
+        const size_t p = cphb_key_lower_bound(skeys, n, key);
+        in = p < n && skeys[p] == key;
+    }
+    out[i] = in ? 1 : 0;
+}
+
+extern "C" int cphb_voxel_grid_check_if_included(const int32_t *keys, size_t n, float voxel_size, const float h_origin[3],
+                                                 const float *queries, size_t nq, uint8_t *out, void *stream) {
+    cudaStream_t s = (cudaStream_t)stream;
+    const char *who = "cphb_voxel_grid_check_if_included";
+    if (!h_origin || (n && !keys) || (nq && (!queries || !out))) return vgo_invalid(who, "null argument");
+    if (n && !(isfinite(voxel_size) && voxel_size > 0.f)) return vgo_invalid(who, "voxel_size is not positive and finite");
+    if (n > (size_t)INT32_MAX) return vgo_invalid(who, "more than 2^31-1 voxels");
+    if (nq == 0) return CPHB_OK;
+    if (n == 0) {
+        CPHB_CUDA(cudaMemsetAsync(out, 0, nq, s));
+        return cphb_read_back(nullptr, nullptr, 0, s, who);
+    }
+    cphb_scratch sc(s);
+    cphb_sorted_keys sk;
+    int rc = cphb_sort_voxel_keys(keys, n, sc, &sk, s, who);
+    if (rc) return rc;
+    CPHB_LAUNCH(vgo_included_kernel, vgo_grid(nq), VGO_BLOCK, 0, s, sk.skeys, n, make_int3(sk.lo[0], sk.lo[1], sk.lo[2]),
+                make_int3(sk.hi[0], sk.hi[1], sk.hi[2]), voxel_size, h_origin[0], h_origin[1], h_origin[2], queries, nq, out);
+    return cphb_read_back(nullptr, nullptr, 0, s, who);
+}
+
+__global__ void __launch_bounds__(VGO_BLOCK) vgo_has_key_kernel(const int32_t *__restrict__ keys, size_t n, int x, int y, int z,
+                                                                int *found) {
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+        if (keys[3 * i] == x && keys[3 * i + 1] == y && keys[3 * i + 2] == z) *found = 1;
+}
+
+extern "C" int cphb_voxel_grid_has_key(const int32_t *keys, size_t n, const int32_t h_key[3], int *h_found, void *stream) {
+    cudaStream_t s = (cudaStream_t)stream;
+    const char *who = "cphb_voxel_grid_has_key";
+    if (!h_key || !h_found || (n && !keys)) return vgo_invalid(who, "null argument");
+    *h_found = 0;
+    if (n == 0) return CPHB_OK;
+    cphb_scratch sc(s);
+    int *d_found = nullptr;
+    int rc = sc.alloc(&d_found, 1);
+    if (rc) return rc;
+    CPHB_CUDA(cudaMemsetAsync(d_found, 0, sizeof(int), s));
+    CPHB_LAUNCH(vgo_has_key_kernel, vgo_capped(n), VGO_BLOCK, 0, s, keys, n, h_key[0], h_key[1], h_key[2], d_found);
+    return cphb_read_back(h_found, d_found, sizeof(int), s, who);
+}
+
+// ------------------------------------------------------------------------------------------------ carving
+struct VgoCamera {
+    float K[9], R[9], t[3];
+    float o[3], voxel;
+    int width, height;
+    int sampled;  // the image is 1-channel float32 (FloatValueAt's only readable kind)
+    int keep_outside;
+};
+
+// FloatValueAt (image.h:240-270) with the defined outside cases: z == 0 or a non-finite u / v is outside
+__device__ __forceinline__ bool vgo_sample(const float *__restrict__ img, const VgoCamera &c, float u, float v, float z, float &d) {
+    if (!c.sampled || z == 0.f || !isfinite(u) || !isfinite(v) || u < 0.f || u > (float)(c.width - 1) || v < 0.f ||
+        v > (float)(c.height - 1))
+        return false;
+    const int ui = max(min((int)u, c.width - 2), 0), vi = max(min((int)v, c.height - 2), 0);
+    const float pu = __fsub_rn(u, (float)ui), pv = __fsub_rn(v, (float)vi);
+    const float v0 = __ldg(img + (size_t)vi * c.width + ui), v1 = __ldg(img + (size_t)(vi + 1) * c.width + ui);
+    const float v2 = __ldg(img + (size_t)vi * c.width + ui + 1), v3 = __ldg(img + (size_t)(vi + 1) * c.width + ui + 1);
+    const float qv = __fsub_rn(1.f, pv), qu = __fsub_rn(1.f, pu);
+    const float a = __fadd_rn(__fmul_rn(v0, qv), __fmul_rn(v1, pv)), b = __fadd_rn(__fmul_rn(v2, qv), __fmul_rn(v3, pv));
+    d = __fadd_rn(__fmul_rn(a, qu), __fmul_rn(b, pu));
+    return true;
+}
+
+// compute_carve_functor (voxelgrid.cu:58-123), keep[i] = !carve.  The projection's expression order (oracle/voxelgrid_ops.c
+// restates it): centre c = ((float)k + 0.5f) * vs + o; corner p = c +- vs / 2 in GetVoxelBoundingPoints' order;
+// x = fma(R2, p2, fma(R1, p1, R0 * p0)) + t per row; (u', v', z) = fma(K2, x2, fma(K1, x1, K0 * x0)) per row;
+// u = u' / z, v = v' / z.
+__global__ void __launch_bounds__(VGO_BLOCK) vgo_carve_kernel(const int32_t *__restrict__ keys, size_t n, const float *__restrict__ img,
+                                                              const VgoCamera c, uint8_t *__restrict__ keep) {
+    const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const float r = __fmul_rn(c.voxel, 0.5f);
+    float ctr[3];
+#pragma unroll
+    for (int a = 0; a < 3; ++a) ctr[a] = __fadd_rn(__fmul_rn(__fadd_rn((float)keys[3 * i + a], 0.5f), c.voxel), c.o[a]);
+    bool kept = false;
+#pragma unroll 1
+    for (int j = 0; j < 8 && !kept; ++j) {
+        const float p[3] = {__fadd_rn(ctr[0], (j & 2) ? r : -r), __fadd_rn(ctr[1], (j & 4) ? r : -r), __fadd_rn(ctr[2], (j & 1) ? r : -r)};
+        float x[3], w[3];
+#pragma unroll
+        for (int a = 0; a < 3; ++a)
+            x[a] = __fadd_rn(__fmaf_rn(c.R[3 * a + 2], p[2], __fmaf_rn(c.R[3 * a + 1], p[1], __fmul_rn(c.R[3 * a], p[0]))), c.t[a]);
+#pragma unroll
+        for (int a = 0; a < 3; ++a) w[a] = __fmaf_rn(c.K[3 * a + 2], x[2], __fmaf_rn(c.K[3 * a + 1], x[1], __fmul_rn(c.K[3 * a], x[0])));
+        const float z = w[2], u = __fdiv_rn(w[0], z), v = __fdiv_rn(w[1], z);
+        float d = 0.f;
+        const bool within = vgo_sample(img, c, u, v, z, d);
+        kept = (!within && c.keep_outside) || (within && d > 0.f && z >= d);
+    }
+    keep[i] = kept ? 1 : 0;
+}
+
+template <class I>
+__global__ void __launch_bounds__(VGO_BLOCK) vgo_gather_kernel(const I *__restrict__ sel, size_t m, const int32_t *__restrict__ keys,
+                                                               const float *__restrict__ colors, int32_t *__restrict__ out_keys,
+                                                               float *__restrict__ out_colors) {
+    const size_t t = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+    if (t >= m) return;
+    const size_t i = (size_t)sel[t];
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+        out_keys[3 * t + a] = keys[3 * i + a];
+        out_colors[3 * t + a] = colors[3 * i + a];
+    }
+}
+
+extern "C" int cphb_voxel_grid_carve(const int32_t *keys, const float *colors, size_t n, float voxel_size, const float h_origin[3],
+                                     const void *image, int width, int height, int num_of_channels, int bytes_per_channel,
+                                     const float h_intrinsic[9], const float h_extrinsic[16], int keep_outside, int32_t *out_keys,
+                                     float *out_colors, size_t *h_n_out, void *stream) {
+    cudaStream_t s = (cudaStream_t)stream;
+    const char *who = "cphb_voxel_grid_carve";
+    if (!h_n_out || !h_origin || !h_intrinsic || !h_extrinsic) return vgo_invalid(who, "null argument");
+    *h_n_out = 0;
+    if (width < 2 || height < 2) return vgo_invalid(who, "the image is narrower or lower than 2 pixels");
+    VgoCamera c;
+    c.sampled = num_of_channels == 1 && bytes_per_channel == 4;
+    if (c.sampled && !image) return vgo_invalid(who, "null image");
+    if (n == 0) return CPHB_OK;
+    if (!keys || !colors || !out_keys || !out_colors) return vgo_invalid(who, "null argument");
+    if (n > (size_t)INT32_MAX) return vgo_invalid(who, "more than 2^31-1 voxels");
+    for (int a = 0; a < 9; ++a) c.K[a] = h_intrinsic[a];
+    for (int r = 0; r < 3; ++r) {
+        for (int q = 0; q < 3; ++q) c.R[3 * r + q] = h_extrinsic[4 * r + q];
+        c.t[r] = h_extrinsic[4 * r + 3];
+        c.o[r] = h_origin[r];
+    }
+    c.voxel = voxel_size;
+    c.width = width;
+    c.height = height;
+    c.keep_outside = keep_outside ? 1 : 0;
+    cphb_scratch sc(s);
+    uint8_t *keep = nullptr;
+    int32_t *sel = nullptr;
+    int rc = sc.alloc(&keep, n);
+    if (!rc) rc = sc.alloc(&sel, n);
+    if (rc) return rc;
+    CPHB_LAUNCH(vgo_carve_kernel, vgo_grid(n), VGO_BLOCK, 0, s, keys, n, c.sampled ? (const float *)image : nullptr, c, keep);
+    size_t m = 0;
+    rc = cphb_compact_flags(keep, n, sel, &m, s);
+    if (rc) return rc;
+    CPHB_LAUNCH(vgo_gather_kernel<int32_t>, vgo_grid1(m), VGO_BLOCK, 0, s, sel, m, keys, colors, out_keys, out_colors);
+    rc = cphb_read_back(nullptr, nullptr, 0, s, who);
+    if (!rc) *h_n_out = m;
+    return rc;
+}
+
+// ------------------------------------------------------------------------------------------------ += and AddVoxels
+// one thread per run of equal keys: a's voxels precede b's in the concatenation and the stable sort keeps that order
+__global__ void __launch_bounds__(VGO_BLOCK) vgo_merge_kernel(const uint32_t *__restrict__ sidx, const int32_t *__restrict__ starts,
+                                                              size_t n_out, size_t n, const int32_t *__restrict__ keys,
+                                                              const float *__restrict__ colors, int average,
+                                                              int32_t *__restrict__ out_keys, float *__restrict__ out_colors) {
+    const size_t v = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+    if (v >= n_out) return;
+    const size_t b = (size_t)starts[v], e = (v + 1 < n_out) ? (size_t)starts[v + 1] : n;
+    const size_t f = sidx[b];
+    float c[3] = {colors[3 * f], colors[3 * f + 1], colors[3 * f + 2]};
+    if (average) {
+        for (size_t t = b + 1; t < e; ++t) {  // add_voxel_color_functor, left to right
+            const size_t i = sidx[t];
+#pragma unroll
+            for (int a = 0; a < 3; ++a) c[a] = __fadd_rn(c[a], colors[3 * i + a]);
+        }
+        const float cnt = (float)(int)(e - b);  // divide_voxel_color_functor (voxelgrid.h:75-82)
+#pragma unroll
+        for (int a = 0; a < 3; ++a) c[a] = __fdiv_rn(c[a], cnt);
+    }
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+        out_keys[3 * v + a] = keys[3 * f + a];
+        out_colors[3 * v + a] = c[a];
+    }
+}
+
+extern "C" int cphb_voxel_grid_merge(const int32_t *keys_a, const float *colors_a, size_t na, const int32_t *keys_b,
+                                     const float *colors_b, size_t nb, int average, int32_t *out_keys, float *out_colors,
+                                     size_t *h_n_out, void *stream) {
+    cudaStream_t s = (cudaStream_t)stream;
+    const char *who = "cphb_voxel_grid_merge";
+    if (!h_n_out || (na && (!keys_a || !colors_a)) || (nb && (!keys_b || !colors_b))) return vgo_invalid(who, "null argument");
+    *h_n_out = 0;
+    const size_t n = na + nb;
+    if (n == 0) return CPHB_OK;
+    if (!out_keys || !out_colors) return vgo_invalid(who, "null output");
+    if (na > (size_t)INT32_MAX || nb > (size_t)INT32_MAX || n > (size_t)INT32_MAX) return vgo_invalid(who, "more than 2^31-1 voxels");
+    cphb_scratch sc(s);
+    int32_t *keys = nullptr, *starts = nullptr;
+    float *colors = nullptr;
+    uint8_t *head = nullptr;
+    int rc = sc.alloc(&keys, 3 * n);
+    if (!rc) rc = sc.alloc(&colors, 3 * n);
+    if (!rc) rc = sc.alloc(&head, n);
+    if (!rc) rc = sc.alloc(&starts, n);
+    if (rc) return rc;
+    if (na) {
+        CPHB_CUDA(cudaMemcpyAsync(keys, keys_a, 12 * na, cudaMemcpyDeviceToDevice, s));
+        CPHB_CUDA(cudaMemcpyAsync(colors, colors_a, 12 * na, cudaMemcpyDeviceToDevice, s));
+    }
+    if (nb) {
+        CPHB_CUDA(cudaMemcpyAsync(keys + 3 * na, keys_b, 12 * nb, cudaMemcpyDeviceToDevice, s));
+        CPHB_CUDA(cudaMemcpyAsync(colors + 3 * na, colors_b, 12 * nb, cudaMemcpyDeviceToDevice, s));
+    }
+    cphb_sorted_keys sk;
+    rc = cphb_sort_voxel_keys(keys, n, sc, &sk, s, who);
+    if (rc) return rc;
+    CPHB_LAUNCH(vg_head_kernel, vgo_grid(n), VGO_BLOCK, 0, s, (const unsigned long long *)sk.skeys, n, head);
+    size_t n_out = 0;
+    rc = cphb_compact_flags(head, n, starts, &n_out, s);
+    if (rc) return rc;
+    CPHB_LAUNCH(vgo_merge_kernel, vgo_grid(n_out), VGO_BLOCK, 0, s, sk.sidx, starts, n_out, n, keys, colors, average ? 1 : 0, out_keys,
+                out_colors);
+    rc = cphb_read_back(nullptr, nullptr, 0, s, who);
+    if (!rc) *h_n_out = n_out;
+    return rc;
+}
+
+// ------------------------------------------------------------------------------------------------ paint and select
+__global__ void __launch_bounds__(VGO_BLOCK) vgo_bad_index_kernel(const int64_t *__restrict__ idx, size_t m, long long n, int *bad) {
+    for (size_t t = blockIdx.x * (size_t)blockDim.x + threadIdx.x; t < m; t += (size_t)gridDim.x * blockDim.x)
+        if (idx[t] < 0 || idx[t] >= n) *bad = 1;
+}
+__global__ void __launch_bounds__(VGO_BLOCK) vgo_paint_kernel(float *__restrict__ colors, const int64_t *__restrict__ idx, size_t m,
+                                                              float c0, float c1, float c2) {
+    for (size_t t = blockIdx.x * (size_t)blockDim.x + threadIdx.x; t < m; t += (size_t)gridDim.x * blockDim.x) {
+        const size_t i = idx ? (size_t)idx[t] : t;
+        colors[3 * i] = c0;
+        colors[3 * i + 1] = c1;
+        colors[3 * i + 2] = c2;
+    }
+}
+__global__ void __launch_bounds__(VGO_BLOCK) vgo_unmark_kernel(const int64_t *__restrict__ idx, size_t m, uint8_t *keep) {
+    const size_t t = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+    if (t < m) keep[idx[t]] = 0;
+}
+
+// CPHB_ERR_INVALID when an index is outside [0, n); synchronises
+static int vgo_check_indices(const int64_t *idx, size_t m, size_t n, cphb_scratch &sc, cudaStream_t s, const char *who) {
+    int *d_bad = nullptr;
+    int rc = sc.alloc(&d_bad, 1);
+    if (rc) return rc;
+    CPHB_CUDA(cudaMemsetAsync(d_bad, 0, sizeof(int), s));
+    CPHB_LAUNCH(vgo_bad_index_kernel, m ? vgo_capped(m) : 1u, VGO_BLOCK, 0, s, idx, m, (long long)n, d_bad);
+    int bad = 0;
+    rc = cphb_read_back(&bad, d_bad, sizeof(int), s, who);
+    if (rc) return rc;
+    if (bad) {
+        cphb_set_error("%s: an index is outside [0, %zu)", who, n);
+        return CPHB_ERR_INVALID;
+    }
+    return CPHB_OK;
+}
+
+extern "C" int cphb_voxel_grid_paint(float *colors, size_t n, const int64_t *indices, size_t m, const float h_color[3], void *stream) {
+    cudaStream_t s = (cudaStream_t)stream;
+    const char *who = "cphb_voxel_grid_paint";
+    if (!h_color || (n && !colors) || (indices == nullptr && m != 0) || (m && !indices)) return vgo_invalid(who, "null argument");
+    const size_t cnt = indices ? m : n;
+    if (cnt == 0) return CPHB_OK;
+    cphb_scratch sc(s);
+    if (indices) {
+        const int rc = vgo_check_indices(indices, m, n, sc, s, who);
+        if (rc) return rc;
+    }
+    CPHB_LAUNCH(vgo_paint_kernel, vgo_capped(cnt), VGO_BLOCK, 0, s, colors, indices, cnt, h_color[0], h_color[1], h_color[2]);
+    CPHB_CHECK_LAUNCH();
+    return CPHB_OK;
+}
+
+extern "C" int cphb_voxel_grid_select_by_index(const int32_t *keys, const float *colors, size_t n, const int64_t *indices, size_t m,
+                                               int invert, int32_t *out_keys, float *out_colors, size_t *h_n_out, void *stream) {
+    cudaStream_t s = (cudaStream_t)stream;
+    const char *who = "cphb_voxel_grid_select_by_index";
+    if (!h_n_out || (n && (!keys || !colors)) || (m && !indices)) return vgo_invalid(who, "null argument");
+    *h_n_out = 0;
+    if (n > (size_t)INT32_MAX) return vgo_invalid(who, "more than 2^31-1 voxels");
+    const size_t rows = invert ? n : m;
+    if (rows && (!out_keys || !out_colors)) return vgo_invalid(who, "null output");
+    cphb_scratch sc(s);
+    if (rows == 0) return CPHB_OK;
+    int rc = vgo_check_indices(indices, m, n, sc, s, who);
+    if (rc) return rc;
+    size_t w = m;
+    if (!invert) {
+        CPHB_LAUNCH(vgo_gather_kernel<int64_t>, vgo_grid(m), VGO_BLOCK, 0, s, indices, m, keys, colors, out_keys, out_colors);
+    } else {
+        uint8_t *keep = nullptr;
+        int32_t *sel = nullptr;
+        rc = sc.alloc(&keep, n);
+        if (!rc) rc = sc.alloc(&sel, n);
+        if (rc) return rc;
+        CPHB_CUDA(cudaMemsetAsync(keep, 1, n, s));
+        CPHB_LAUNCH(vgo_unmark_kernel, vgo_grid1(m), VGO_BLOCK, 0, s, indices, m, keep);
+        rc = cphb_compact_flags(keep, n, sel, &w, s);
+        if (rc) return rc;
+        CPHB_LAUNCH(vgo_gather_kernel<int32_t>, vgo_grid1(w), VGO_BLOCK, 0, s, sel, w, keys, colors, out_keys, out_colors);
+    }
+    rc = cphb_read_back(nullptr, nullptr, 0, s, who);
+    if (!rc) *h_n_out = w;
+    return rc;
+}
+
+// ------------------------------------------------------------------------------------------------ from an OccupancyGrid
+// compute_points_from_occvoxels_functor (pointcloud_factory.cu:239-256): (cell + c) * vs + o, c = (float)(-res / 2 + 0.5)
+__global__ void __launch_bounds__(VGO_BLOCK) vgo_occ_points_kernel(const int32_t *__restrict__ cells, size_t m, float c, float voxel,
+                                                                   float ox, float oy, float oz, float *__restrict__ pts,
+                                                                   float *__restrict__ colors) {
+    const size_t t = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+    if (t >= m) return;
+    const float o[3] = {ox, oy, oz};
+#pragma unroll
+    for (int a = 0; a < 3; ++a) pts[3 * t + a] = __fadd_rn(__fmul_rn(__fadd_rn((float)cells[3 * t + a], c), voxel), o[a]);
+    colors[3 * t] = 0.f;  // OccupancyVoxel's colour (occupancygrid.h:33-72)
+    colors[3 * t + 1] = 0.f;
+    colors[3 * t + 2] = 1.f;
+}
+
+static int vgo_occ_check(const cphb_occgrid *grid, float *vs, float o[3], int *res, const char *who) {
+    if (!grid) return vgo_invalid(who, "null OccupancyGrid");
+    cphb_occgrid_geometry(grid, vs, o);
+    cphb_occgrid_view v;
+    cphb_occgrid_view_of(grid, &v);
+    *res = v.res;
+    if (!(*vs > 0.f)) return vgo_invalid(who, "occupancy grid voxel_size <= 0");  // voxelgrid_factory.cu:287-290
+    return CPHB_OK;
+}
+
+extern "C" int cphb_voxel_grid_from_occgrid(const cphb_occgrid *grid, int32_t *out_keys, float *out_colors, size_t capacity,
+                                            size_t *h_count, float h_origin[3], void *stream) {
+    cudaStream_t s = (cudaStream_t)stream;
+    const char *who = "cphb_voxel_grid_from_occgrid";
+    if (!h_count || !h_origin) return vgo_invalid(who, "null argument");
+    *h_count = 0;
+    float vs, o[3];
+    int res;
+    int rc = vgo_occ_check(grid, &vs, o, &res, who);
+    if (rc) return rc;
+    const float half = (float)(res / 2);
+    for (int a = 0; a < 3; ++a) h_origin[a] = o[a] - half * vs;
+    if (capacity && (!out_keys || !out_colors)) return vgo_invalid(who, "null output");
+    size_t cnt = 0;
+    rc = cphb_occgrid_extract(grid, 2, capacity ? out_keys : nullptr, nullptr, capacity, &cnt, stream);
+    if (rc) return rc;
+    *h_count = cnt;
+    if (cnt == 0 || capacity < cnt) return cphb_read_back(nullptr, nullptr, 0, s, who);
+    CPHB_LAUNCH(vgo_paint_kernel, vgo_capped(cnt), VGO_BLOCK, 0, s, out_colors, nullptr, cnt, 0.f, 0.f, 1.f);
+    return cphb_read_back(nullptr, nullptr, 0, s, who);
+}
+
+extern "C" int cphb_point_cloud_from_occgrid(const cphb_occgrid *grid, float *out_points, float *out_colors, size_t capacity,
+                                             size_t *h_count, void *stream) {
+    cudaStream_t s = (cudaStream_t)stream;
+    const char *who = "cphb_point_cloud_from_occgrid";
+    if (!h_count) return vgo_invalid(who, "null argument");
+    *h_count = 0;
+    float vs, o[3];
+    int res;
+    int rc = vgo_occ_check(grid, &vs, o, &res, who);
+    if (rc) return rc;
+    if (capacity && (!out_points || !out_colors)) return vgo_invalid(who, "null output");
+    cphb_scratch sc(s);
+    int32_t *cells = nullptr;
+    if (capacity) {
+        rc = sc.alloc(&cells, 3 * capacity);
+        if (rc) return rc;
+    }
+    size_t cnt = 0;
+    rc = cphb_occgrid_extract(grid, 2, cells, nullptr, capacity, &cnt, stream);
+    if (rc) return rc;
+    *h_count = cnt;
+    if (cnt == 0 || capacity < cnt) return cphb_read_back(nullptr, nullptr, 0, s, who);
+    const float c = (float)(-(res / 2) + 0.5);
+    CPHB_LAUNCH(vgo_occ_points_kernel, vgo_grid(cnt), VGO_BLOCK, 0, s, cells, cnt, c, vs, o[0], o[1], o[2], out_points, out_colors);
+    return cphb_read_back(nullptr, nullptr, 0, s, who);
 }

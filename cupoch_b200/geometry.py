@@ -416,6 +416,21 @@ class PointCloud:
         out._points, out._normals, out._colors = op, on, oc
         return out
 
+    @staticmethod
+    def create_from_occupancy_grid(occupancy_grid):
+        """PointCloud::CreateFromOccupancyGrid (pointcloud_factory.cu:418-430): one point per occupied cell, at
+        (cell + (-(resolution / 2) + 0.5)) * voxel_size + origin, colour (0, 0, 1), in ExtractOccupiedVoxels order"""
+        occupancy_grid._sync_params()
+        L, h, n = _lib.lib(), occupancy_grid._h, C.c_size_t(0)
+        _lib.check(L.cphb_point_cloud_from_occgrid(h, None, None, 0, C.byref(n), None))
+        out = PointCloud()
+        m = n.value
+        if m:
+            pts, cols = DeviceArray((m, 3), np.float32), DeviceArray((m, 3), np.float32)
+            _lib.check(L.cphb_point_cloud_from_occgrid(h, pts.ptr, cols.ptr, m, C.byref(n), None))
+            out._points, out._colors = pts, cols
+        return out
+
     def normalize_normals(self):
         """NormalizeNormals (pointcloud.cu:282-285), in place: every non-zero normal divided by its length"""
         if self._normals is not None and len(self._normals):
@@ -577,9 +592,10 @@ def _point_indices(points, fn, *args):
 
 
 class VoxelGrid:
-    """geometry::VoxelGrid (voxelgrid.h:84-160), the part SURVEY 8f ranks next: creation from a point cloud
-    (voxelgrid_factory.cu:164-228) and the accessors that need nothing else.  voxels_keys / voxels_colors are
-    device arrays ([m, 3] int32 grid indices in lexicographic order, [m, 3] float32 mean colours)."""
+    """geometry::VoxelGrid (voxelgrid.h:84-210; pybind voxelgrid.cpp:96-157).  voxels_keys / voxels_colors are device
+    arrays ([m, 3] int32 grid indices, [m, 3] float32 colours).  The factories, +=, add_voxels and carving leave the
+    keys in lexicographic order and unique; select_by_index and direct assignment may leave them in any order, with
+    repeats, and every lookup accepts that."""
 
     def __init__(self):
         self.voxel_size = 0.0
@@ -655,6 +671,239 @@ class VoxelGrid:
         mn, mx = input._bounds()
         return VoxelGrid.create_from_point_cloud_within_bounds(input, voxel_size, mn - v * np.float32(0.5),
                                                                mx + v * np.float32(0.5))
+
+    # -- the rest of the reference's VoxelGrid (voxelgrid.cu:235-475) ------------------------------------------------
+    def _like(self, keys=None, colors=None, m=0):
+        """a grid with this one's geometry holding the first m rows of keys / colors; when that is fewer rows than the
+        buffers hold (carving, merging) the rows are copied out, so the result does not keep the larger buffers alive"""
+        out = VoxelGrid()
+        out.voxel_size, out.origin = self.voxel_size, self.origin.copy()
+        if m and m == keys.shape[0]:
+            out.voxels_keys, out.voxels_colors = keys, colors
+        elif m:
+            out.voxels_keys, out.voxels_colors = DeviceArray((m, 3), np.int32), DeviceArray((m, 3), np.float32)
+            L = _lib.lib()
+            _lib.check(L.cphb_memcpy_d2d(out.voxels_keys.ptr, keys.ptr, 12 * m, None))
+            _lib.check(L.cphb_memcpy_d2d(out.voxels_colors.ptr, colors.ptr, 12 * m, None))
+            _lib.check(L.cphb_stream_synchronize(None))
+        return out
+
+    def _set(self, other):
+        self.voxels_keys, self.voxels_colors = other.voxels_keys, other.voxels_colors
+        return self
+
+    def _f3(self, v=None):
+        return (C.c_float * 3)(*np.asarray(self.origin if v is None else v, np.float32).reshape(3).tolist())
+
+    def _device(self):
+        """voxels_keys / voxels_colors as device arrays (assigned host keys are uploaded, missing colours are (1, 1, 1))"""
+        if len(self):
+            if not isinstance(self.voxels_keys, DeviceArray):
+                self.voxels_keys = DeviceArray.wrap(self.voxels_keys, np.int32)
+            if self.voxels_colors is None:
+                self.voxels_colors = DeviceArray.from_numpy(np.ones((len(self), 3), np.float32), np.float32)
+            elif not isinstance(self.voxels_colors, DeviceArray):
+                self.voxels_colors = DeviceArray.wrap(self.voxels_colors, np.float32)
+        return self
+
+    def _keys_ptr(self):
+        return self._device().voxels_keys.ptr if len(self) else None
+
+    def _colors_ptr(self):
+        return self._device().voxels_colors.ptr if len(self) else None
+
+    @staticmethod
+    def create_dense(origin, voxel_size, width, height, depth):
+        """VoxelGrid::CreateDense (voxelgrid_factory.cu:134-162): int(round(extent / voxel_size)) voxels per axis, keys in
+        lexicographic order, colours (1, 1, 1).  A bad voxel size, a negative count or an overflowing total raise."""
+        out = VoxelGrid()
+        out.voxel_size = float(np.float32(voxel_size))
+        out.origin = np.asarray(origin, np.float32).reshape(3).copy()
+        args = [float(np.float32(x)) for x in (voxel_size, width, height, depth)]
+        n = C.c_size_t(0)
+        _lib.check(_lib.lib().cphb_voxel_grid_create_dense(*args, None, None, 0, C.byref(n), None))
+        m = n.value
+        if m:
+            keys, cols = DeviceArray((m, 3), np.int32), DeviceArray((m, 3), np.float32)
+            _lib.check(_lib.lib().cphb_voxel_grid_create_dense(*args, keys.ptr, cols.ptr, m, C.byref(n), None))
+            out.voxels_keys, out.voxels_colors = keys, cols
+        return out
+
+    @staticmethod
+    def create_from_occupancy_grid(occupancy_grid):
+        """VoxelGrid::CreateFromOccupancyGrid (voxelgrid_factory.cu:283-305): one voxel per occupied cell, key = its grid
+        index, colour (0, 0, 1).  origin = grid origin - (resolution / 2) * voxel_size (the reference keeps the grid's
+        origin, which puts every voxel resolution / 2 cells away from its cell)."""
+        occupancy_grid._sync_params()
+        L, h = _lib.lib(), occupancy_grid._h
+        n, o = C.c_size_t(0), (C.c_float * 3)()
+        _lib.check(L.cphb_voxel_grid_from_occgrid(h, None, None, 0, C.byref(n), o, None))
+        out = VoxelGrid()
+        out.voxel_size, out.origin = float(np.float32(occupancy_grid.voxel_size)), np.array(o, np.float32)
+        m = n.value
+        if m:
+            keys, cols = DeviceArray((m, 3), np.int32), DeviceArray((m, 3), np.float32)
+            _lib.check(L.cphb_voxel_grid_from_occgrid(h, keys.ptr, cols.ptr, m, C.byref(n), o, None))
+            out.voxels_keys, out.voxels_colors = keys, cols
+        return out
+
+    def check_if_included(self, queries):
+        """CheckIfIncluded (voxelgrid.cu:365-376): host [n, 3] queries -> [n] bool, whether each query's GetVoxel cell is
+        a voxel.  Non-finite queries and cells outside the int range are False."""
+        q = np.ascontiguousarray(np.asarray(queries, np.float32).reshape(-1, 3))
+        if len(q) == 0:
+            return np.zeros(0, bool)
+        d = DeviceArray.from_numpy(q, np.float32)
+        out = DeviceArray((len(q),), np.uint8)
+        _lib.check(_lib.lib().cphb_voxel_grid_check_if_included(self._keys_ptr(), len(self), float(self.voxel_size), self._f3(),
+                                                                d.ptr, len(q), out.ptr, None))
+        return out.cpu().astype(bool)
+
+    def get_voxel_center_coordinate(self, idx):
+        """GetVoxelCenterCoordinate (voxelgrid.cu:343-354): ((idx + 0.5) * voxel_size) + origin, or the zero vector when
+        idx is not a voxel (the reference's answer)."""
+        k = np.asarray(idx, np.int32).reshape(3)
+        found = C.c_int(0)
+        _lib.check(_lib.lib().cphb_voxel_grid_has_key(self._keys_ptr(), len(self), (C.c_int32 * 3)(*k.tolist()), C.byref(found), None))
+        if not found.value:
+            return np.zeros(3, np.float32)
+        return ((k.astype(np.float32) + np.float32(0.5)) * np.float32(self.voxel_size) + self.origin).astype(np.float32)
+
+    def get_voxel_bounding_points(self, idx):
+        """GetVoxelBoundingPoints (voxelgrid.cu:356-363): the 8 corners around GetVoxelCenterCoordinate(idx), in the
+        order carving projects them (bit 0: +z, bit 1: +x, bit 2: +y)"""
+        x = self.get_voxel_center_coordinate(idx)
+        r = np.float32(self.voxel_size) * np.float32(0.5)
+        sgn = np.array([[(j >> 1) & 1, (j >> 2) & 1, j & 1] for j in range(8)], np.float32) * 2 - 1
+        return (x[None, :] + sgn * r).astype(np.float32)
+
+    def _carve(self, image, camera_params, keep_voxels_outside_image, what):
+        intr = camera_params.intrinsic
+        if image.height != intr.height or image.width != intr.width:
+            raise ValueError("[VoxelGrid] provided %s dimensions are not compatible with the provided camera_parameters" % what)
+        n = len(self)
+        sampled = image.num_of_channels == 1 and image.bytes_per_channel == 4
+        img = DeviceArray.from_numpy(image._data, image._data.dtype) if sampled else None
+        K = (C.c_float * 9)(*np.asarray(intr.intrinsic_matrix, np.float32).reshape(9).tolist())
+        E = (C.c_float * 16)(*np.asarray(camera_params.extrinsic, np.float32).reshape(16).tolist())
+        keys, cols = (DeviceArray((n, 3), np.int32), DeviceArray((n, 3), np.float32)) if n else (None, None)
+        m = C.c_size_t(0)
+        _lib.check(_lib.lib().cphb_voxel_grid_carve(self._keys_ptr(), self._colors_ptr(), n, float(self.voxel_size), self._f3(),
+                                                    img.ptr if img is not None else None, image.width, image.height,
+                                                    image.num_of_channels, image.bytes_per_channel, K, E,
+                                                    int(bool(keep_voxels_outside_image)), keys.ptr if n else None,
+                                                    cols.ptr if n else None, C.byref(m), None))
+        return self._set(self._like(keys, cols, m.value))
+
+    def carve_depth_map(self, depth_map, camera_params, keep_voxels_outside_image=False):
+        """CarveDepthMap (voxelgrid.cu:378-403): removes every voxel none of whose corners projects to a pixel with
+        depth d > 0 and z >= d (or outside the image, with keep_voxels_outside_image).  Only a 1-channel float32 image
+        is sampled; any other image is outside everywhere, as in the reference."""
+        return self._carve(depth_map, camera_params, keep_voxels_outside_image, "depth_map")
+
+    def carve_silhouette(self, silhouette_mask, camera_params, keep_voxels_outside_image=False):
+        """CarveSilhouette (voxelgrid.cu:405-430): the reference's test is the depth map's (d > 0 and z >= d), so a uint8
+        mask is outside everywhere: every voxel is removed, or with keep_voxels_outside_image every voxel is kept."""
+        return self._carve(silhouette_mask, camera_params, keep_voxels_outside_image, "silhouette_mask")
+
+    def _merge(self, other, average):
+        if float(np.float32(self.voxel_size)) != float(np.float32(other.voxel_size)):
+            raise ValueError("[VoxelGrid] Could not combine VoxelGrid because voxel_size differs (this=%f, other=%f)"
+                             % (self.voxel_size, other.voxel_size))
+        if not np.array_equal(np.asarray(self.origin, np.float32), np.asarray(other.origin, np.float32)):
+            raise ValueError("[VoxelGrid] Could not combine VoxelGrid because origin differs")
+        n = len(self) + len(other)
+        keys, cols = (DeviceArray((n, 3), np.int32), DeviceArray((n, 3), np.float32)) if n else (None, None)
+        m = C.c_size_t(0)
+        _lib.check(_lib.lib().cphb_voxel_grid_merge(self._keys_ptr(), self._colors_ptr(), len(self), other._keys_ptr(),
+                                                    other._colors_ptr(), len(other), int(average), keys.ptr if n else None,
+                                                    cols.ptr if n else None, C.byref(m), None))
+        return self._like(keys, cols, m.value)
+
+    def __iadd__(self, other):
+        """operator+= (voxelgrid.cu:235-281): both grids' voxels, one per key, colours averaged over equal keys (summed
+        in this grid's order, then the other's).  Different voxel sizes or origins raise."""
+        return self._set(self._merge(other, True))
+
+    def __add__(self, other):
+        return self._merge(other, True)
+
+    def add_voxels(self, keys, colors=None):
+        """AddVoxels (voxelgrid.cu:299-319): voxels [m, 3] int32 keys (and [m, 3] colours, (1, 1, 1) by default); a key
+        already present keeps its voxel"""
+        other = self._like()
+        k = np.ascontiguousarray(np.asarray(keys, np.int32).reshape(-1, 3))
+        if len(k):
+            c = np.ones((len(k), 3), np.float32) if colors is None else np.asarray(colors, np.float32).reshape(-1, 3)
+            other.voxels_keys, other.voxels_colors = DeviceArray.from_numpy(k, np.int32), DeviceArray.from_numpy(c, np.float32)
+        return self._set(self._merge(other, False))
+
+    def add_voxel(self, key, color=(1.0, 1.0, 1.0)):
+        """AddVoxel (voxelgrid.cu:288-297)"""
+        return self.add_voxels(np.asarray(key).reshape(1, 3), np.asarray(color).reshape(1, 3))
+
+    @staticmethod
+    def _indices(indices):
+        if isinstance(indices, DeviceArray) or hasattr(indices, "is_cuda"):
+            return DeviceArray.wrap(indices, np.int64)
+        return DeviceArray.from_numpy(np.ascontiguousarray(np.asarray(indices, np.int64).reshape(-1)), np.int64)
+
+    def paint_uniform_color(self, color):
+        """PaintUniformColor (voxelgrid.cu:321-325)"""
+        _lib.check(_lib.lib().cphb_voxel_grid_paint(self._colors_ptr(), len(self), None, 0, self._f3(color), None))
+        _lib.check(_lib.lib().cphb_stream_synchronize(None))
+        return self
+
+    def paint_indexed_color(self, indices, color):
+        """PaintIndexedColor (voxelgrid.cu:327-336); an index outside [0, len) raises and nothing is painted"""
+        d = self._indices(indices)
+        if len(d):
+            _lib.check(_lib.lib().cphb_voxel_grid_paint(self._colors_ptr(), len(self), d.ptr, len(d), self._f3(color), None))
+            _lib.check(_lib.lib().cphb_stream_synchronize(None))
+        return self
+
+    def select_by_index(self, indices, invert=False):
+        """SelectByIndex (voxelgrid.cu:432-475): the voxels at indices, in index order, or with invert the others in
+        ascending order (repeated indices allowed).  An index outside [0, len) raises."""
+        d = self._indices(indices)
+        rows = len(self) if invert else len(d)
+        keys, cols = (DeviceArray((rows, 3), np.int32), DeviceArray((rows, 3), np.float32)) if rows else (None, None)
+        m = C.c_size_t(0)
+        _lib.check(_lib.lib().cphb_voxel_grid_select_by_index(self._keys_ptr(), self._colors_ptr(), len(self),
+                                                              d.ptr if len(d) else None, len(d), int(bool(invert)),
+                                                              keys.ptr if rows else None, cols.ptr if rows else None,
+                                                              C.byref(m), None))
+        return self._like(keys, cols, m.value)
+
+
+class Image:
+    """geometry::Image as a data holder (image.h; pybind image.cpp:80-100): a C-contiguous uint8, uint16 or float32
+    buffer of shape (height, width) or (height, width, channels) with 1, 3 or 4 channels.  Filters, pyramids and IO
+    are not part of this project."""
+
+    def __init__(self, data=None):
+        if data is None:
+            data = np.zeros((0, 0), np.uint8)
+        a = np.asarray(data)
+        if a.dtype not in (np.uint8, np.uint16, np.float32):
+            raise ValueError("Image can only be initialized from buffer of uint8, uint16, or float!")
+        if a.ndim not in (2, 3) or (a.ndim == 3 and a.shape[2] not in (1, 3, 4)):
+            raise ValueError("Image can only be initialized from a (height, width) or (height, width, 1 | 3 | 4) buffer")
+        self._data = np.ascontiguousarray(a)
+
+    height = property(lambda s: int(s._data.shape[0]))
+    width = property(lambda s: int(s._data.shape[1]))
+    num_of_channels = property(lambda s: 1 if s._data.ndim == 2 else int(s._data.shape[2]))
+    bytes_per_channel = property(lambda s: int(s._data.dtype.itemsize))
+
+    def is_empty(self):
+        return self._data.size == 0
+
+    def __array__(self, dtype=None, copy=None):
+        return self._data if dtype is None else self._data.astype(dtype)
+
+    def __repr__(self):
+        return "geometry::Image of size %dx%d, with %d channels." % (self.width, self.height, self.num_of_channels)
 
 
 class OccupancyVoxel:

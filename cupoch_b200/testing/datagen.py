@@ -83,3 +83,40 @@ def make_source(target, T_gt, perm_seed, noise_seed, sigma, attrs=()):
             b = (b.astype(np.float64) @ Ti[:3, :3].T)
         out.append(np.ascontiguousarray(b, np.float32))
     return out if len(out) > 1 else out[0]
+
+
+def ring_cameras(views, w, h, radius=2.5, f=None):
+    """carving views: cameras on a tilted ring of the given radius around the origin, each looking at it.  -> a list of
+    (K [3, 3], world-to-camera E [4, 4]) float32 pairs; f defaults to 0.9 w"""
+    f = f or 0.9 * w
+    K = np.array([[f, 0, (w - 1) / 2], [0, f, (h - 1) / 2], [0, 0, 1]], np.float32)
+    out = []
+    for i in range(views):
+        a = 2 * np.pi * i / views
+        eye = np.array([radius * np.cos(a), radius * np.sin(a), 0.6 * np.sin(3 * a)])
+        zc = -eye / np.linalg.norm(eye)
+        xc = np.cross(zc, [0, 0, 1.0])
+        xc /= np.linalg.norm(xc)
+        R = np.stack([xc, np.cross(zc, xc), zc])
+        E = np.eye(4, dtype=np.float32)
+        E[:3, :3] = R
+        E[:3, 3] = -R @ eye
+        out.append((K, E))
+    return out
+
+
+def sphere_depth(K, E, w, h, radius):
+    """analytic depth map (camera z, float32 [h, w]) of a sphere of the given radius at the world origin seen through
+    K and the world-to-camera E; 0 where the ray misses"""
+    Ki = np.linalg.inv(np.asarray(K, np.float64))
+    uu, vv = np.meshgrid(np.arange(w), np.arange(h))
+    rays = np.stack([uu, vv, np.ones_like(uu)], -1).reshape(-1, 3) @ Ki.T  # camera rays with z = 1
+    R, t = np.asarray(E, np.float64)[:3, :3], np.asarray(E, np.float64)[:3, 3]
+    c = -R.T @ t  # camera centre in the world
+    dw = rays @ R  # world directions (R^T d)
+    a = np.sum(dw * dw, 1)
+    b = 2 * dw @ c
+    cc = c @ c - radius * radius
+    disc = b * b - 4 * a * cc
+    s = (-b - np.sqrt(np.maximum(disc, 0))) / (2 * a)
+    return np.where(disc > 0, s, 0).reshape(h, w).astype(np.float32)

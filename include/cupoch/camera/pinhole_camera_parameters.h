@@ -1,0 +1,4 @@
+// Path-compatible with cupoch/camera/pinhole_camera_parameters.h: camera::PinholeCameraParameters as plain data.
+// See cupoch/cupoch_b200_facade.h.
+#pragma once
+#include "cupoch/cupoch_b200_facade.h"

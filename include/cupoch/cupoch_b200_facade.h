@@ -295,6 +295,39 @@ private:
 };
 }  // namespace knn
 
+// --------------------------------------------------------------------------- camera
+namespace camera {
+/// camera::PinholeCameraIntrinsic (pinhole_camera_intrinsic.h): width_, height_ and the 3x3 intrinsic_matrix_
+class PinholeCameraIntrinsic {
+public:
+    PinholeCameraIntrinsic() {}
+    PinholeCameraIntrinsic(int width, int height, float fx, float fy, float cx, float cy) { SetIntrinsics(width, height, fx, fy, cx, cy); }
+    void SetIntrinsics(int width, int height, float fx, float fy, float cx, float cy) {
+        width_ = width;
+        height_ = height;
+        intrinsic_matrix_ = Eigen::Matrix3f::Identity();
+        intrinsic_matrix_(0, 0) = fx;
+        intrinsic_matrix_(1, 1) = fy;
+        intrinsic_matrix_(0, 2) = cx;
+        intrinsic_matrix_(1, 2) = cy;
+    }
+    std::pair<float, float> GetFocalLength() const { return std::make_pair(intrinsic_matrix_(0, 0), intrinsic_matrix_(1, 1)); }
+    std::pair<float, float> GetPrincipalPoint() const { return std::make_pair(intrinsic_matrix_(0, 2), intrinsic_matrix_(1, 2)); }
+    bool IsValid() const { return width_ > 0 && height_ > 0; }
+
+public:
+    int width_ = -1;
+    int height_ = -1;
+    Eigen::Matrix3f intrinsic_matrix_;
+};
+/// camera::PinholeCameraParameters (pinhole_camera_parameters.h): intrinsic_ and the world-to-camera extrinsic_
+class PinholeCameraParameters {
+public:
+    PinholeCameraIntrinsic intrinsic_;
+    Eigen::Matrix4f extrinsic_ = Eigen::Matrix4f::Identity();
+};
+}  // namespace camera
+
 // --------------------------------------------------------------------------- geometry
 namespace geometry {
 namespace detail {
@@ -446,9 +479,12 @@ inline OrientedBoundingBox OrientedBoundingBox::CreateFromAxisAlignedBoundingBox
 }
 
 /// geometry::PointCloud (pointcloud.h:43-263), hot-path subset.
+class OccupancyGrid;
 class PointCloud {
 public:
     PointCloud() {}
+    /// PointCloud::CreateFromOccupancyGrid (pointcloud_factory.cu:418-430), defined after OccupancyGrid
+    static std::shared_ptr<PointCloud> CreateFromOccupancyGrid(const OccupancyGrid &occgrid);
     PointCloud(const std::vector<Eigen::Vector3f> &points) : points_(points) {}
     virtual ~PointCloud() {}
     bool IsEmpty() const { return points_.empty(); }
@@ -763,9 +799,33 @@ public:
     Eigen::Vector3f color_ = Eigen::Vector3f(1.0f, 1.0f, 1.0f);
 };
 
+/// geometry::Image (image.h) as a holder of pixels: width_ x height_ x num_of_channels_ channels of bytes_per_channel_
+/// bytes each, row-major in data_ (device).  Carving samples a 1-channel float32 image; filters, pyramids and IO are not
+/// part of this engine.
+class Image {
+public:
+    Image &Prepare(int width, int height, int num_of_channels, int bytes_per_channel) {
+        width_ = width;
+        height_ = height;
+        num_of_channels_ = num_of_channels;
+        bytes_per_channel_ = bytes_per_channel;
+        data_.resize((size_t)width * height * num_of_channels * bytes_per_channel);
+        return *this;
+    }
+    bool IsEmpty() const { return data_.size() == 0; }
+
+public:
+    int width_ = 0;
+    int height_ = 0;
+    int num_of_channels_ = 0;
+    int bytes_per_channel_ = 0;
+    utility::device_vector<uint8_t> data_;
+};
+
 /// geometry::VoxelGrid (voxelgrid.h:84-160): creation from a point cloud (voxelgrid_factory.cu:164-228) and the
-/// accessors that need nothing else.  Keys and colours are kept as two device vectors (the reference zips keys
-/// with Voxel{grid_index, color}); GetVoxels() hands back the reference's pair.
+/// accessors, CreateDense, CheckIfIncluded, carving, += / AddVoxels, painting, SelectByIndex and CreateFromOccupancyGrid
+/// (voxelgrid.cu:235-475).  Keys and colours are kept as two device vectors (the reference zips keys with
+/// Voxel{grid_index, color}); GetVoxels() hands back the reference's pair.
 class VoxelGrid {
 public:
     bool HasVoxels() const { return voxels_keys_.size() > 0; }
@@ -810,12 +870,174 @@ public:
         return CreateFromPointCloudWithinBounds(input, voxel_size, Eigen::Vector3f(lo[0] - h, lo[1] - h, lo[2] - h),
                                                 Eigen::Vector3f(hi[0] + h, hi[1] + h, hi[2] + h));
     }
+    /// CreateDense (voxelgrid_factory.cu:134-162): int(round(extent / voxel_size)) voxels per axis in lexicographic order
+    static std::shared_ptr<VoxelGrid> CreateDense(const Eigen::Vector3f &origin, float voxel_size, float width, float height, float depth) {
+        auto out = std::make_shared<VoxelGrid>();
+        out->voxel_size_ = voxel_size;
+        out->origin_ = origin;
+        size_t n = 0;
+        utility::check(cphb_voxel_grid_create_dense(voxel_size, width, height, depth, nullptr, nullptr, 0, &n, nullptr));
+        out->voxels_keys_.resize(n);
+        out->voxels_colors_.resize(n);
+        if (n)
+            utility::check(cphb_voxel_grid_create_dense(voxel_size, width, height, depth, out->keys(), out->colors(), n, &n, nullptr));
+        return out;
+    }
+    /// CreateFromOccupancyGrid (voxelgrid_factory.cu:283-305), defined after OccupancyGrid
+    static std::shared_ptr<VoxelGrid> CreateFromOccupancyGrid(const OccupancyGrid &input);
+    /// CheckIfIncluded (voxelgrid.cu:365-376): whether each query's GetVoxel cell is a voxel (false for non-finite queries)
+    std::vector<bool> CheckIfIncluded(const std::vector<Eigen::Vector3f> &queries) const {
+        std::vector<bool> out(queries.size(), false);
+        if (queries.empty()) return out;
+        utility::device_vector<Eigen::Vector3f> q(queries);
+        utility::device_vector<uint8_t> d(queries.size());
+        const float o[3] = {origin_[0], origin_[1], origin_[2]};
+        utility::check(cphb_voxel_grid_check_if_included(keys(), voxels_keys_.size(), voxel_size_, o,
+                                                         reinterpret_cast<const float *>(q.data()), q.size(), d.data(), nullptr));
+        const auto h = d.to_host();
+        for (size_t i = 0; i < h.size(); ++i) out[i] = h[i] != 0;
+        return out;
+    }
+    /// GetVoxelCenterCoordinate (voxelgrid.cu:343-354): the zero vector when idx is not a voxel, as in the reference
+    Eigen::Vector3f GetVoxelCenterCoordinate(const Eigen::Vector3i &idx) const {
+        const int32_t k[3] = {idx[0], idx[1], idx[2]};
+        int found = 0;
+        utility::check(cphb_voxel_grid_has_key(keys(), voxels_keys_.size(), k, &found, nullptr));
+        if (!found) return Eigen::Vector3f(0.f, 0.f, 0.f);
+        return Eigen::Vector3f(((float)idx[0] + 0.5f) * voxel_size_ + origin_[0], ((float)idx[1] + 0.5f) * voxel_size_ + origin_[1],
+                               ((float)idx[2] + 0.5f) * voxel_size_ + origin_[2]);
+    }
+    /// GetVoxelBoundingPoints (voxelgrid.cu:356-363): corner j is the centre + r * (bit 1: x, bit 2: y, bit 0: z ? +1 : -1)
+    std::array<Eigen::Vector3f, 8> GetVoxelBoundingPoints(const Eigen::Vector3i &index) const {
+        const float r = voxel_size_ * 0.5f;
+        const Eigen::Vector3f x = GetVoxelCenterCoordinate(index);
+        std::array<Eigen::Vector3f, 8> p;
+        for (int j = 0; j < 8; ++j)
+            p[j] = Eigen::Vector3f(x[0] + ((j & 2) ? r : -r), x[1] + ((j & 4) ? r : -r), x[2] + ((j & 1) ? r : -r));
+        return p;
+    }
+    /// CarveDepthMap (voxelgrid.cu:378-403)
+    VoxelGrid &CarveDepthMap(const Image &depth_map, const camera::PinholeCameraParameters &camera_parameter,
+                             bool keep_voxels_outside_image = false) {
+        return carve(depth_map, camera_parameter, keep_voxels_outside_image, "depth_map");
+    }
+    /// CarveSilhouette (voxelgrid.cu:405-430): the reference applies the depth map's test (d > 0 and z >= d)
+    VoxelGrid &CarveSilhouette(const Image &silhouette_mask, const camera::PinholeCameraParameters &camera_parameter,
+                               bool keep_voxels_outside_image = false) {
+        return carve(silhouette_mask, camera_parameter, keep_voxels_outside_image, "silhouette_mask");
+    }
+    /// operator+= (voxelgrid.cu:235-286): one voxel per key, colours of equal keys averaged (this grid's, then the other's)
+    VoxelGrid &operator+=(const VoxelGrid &voxelgrid) {
+        merge(voxelgrid, true);
+        return *this;
+    }
+    VoxelGrid operator+(const VoxelGrid &voxelgrid) const { return (VoxelGrid(*this) += voxelgrid); }
+    /// AddVoxel / AddVoxels (voxelgrid.cu:288-319): a key already present keeps its voxel
+    void AddVoxel(const Voxel &voxel) { AddVoxels(std::vector<Voxel>{voxel}); }
+    void AddVoxels(const std::vector<Voxel> &voxels) {
+        VoxelGrid other;
+        other.voxel_size_ = voxel_size_;
+        other.origin_ = origin_;
+        std::vector<Eigen::Vector3i> k(voxels.size());
+        std::vector<Eigen::Vector3f> c(voxels.size());
+        for (size_t i = 0; i < voxels.size(); ++i) {
+            k[i] = voxels[i].grid_index_;
+            c[i] = voxels[i].color_;
+        }
+        other.voxels_keys_ = k;
+        other.voxels_colors_ = c;
+        merge(other, false);
+    }
+    /// PaintUniformColor / PaintIndexedColor (voxelgrid.cu:321-336); an index outside [0, size) throws, nothing painted
+    VoxelGrid &PaintUniformColor(const Eigen::Vector3f &color) {
+        const float c[3] = {color[0], color[1], color[2]};
+        utility::check(cphb_voxel_grid_paint(colors(), voxels_colors_.size(), nullptr, 0, c, nullptr));
+        utility::check(cphb_stream_synchronize(nullptr));
+        return *this;
+    }
+    VoxelGrid &PaintIndexedColor(const utility::device_vector<size_t> &indices, const Eigen::Vector3f &color) {
+        const float c[3] = {color[0], color[1], color[2]};
+        if (indices.size())
+            utility::check(cphb_voxel_grid_paint(colors(), voxels_colors_.size(), reinterpret_cast<const int64_t *>(indices.data()),
+                                                 indices.size(), c, nullptr));
+        utility::check(cphb_stream_synchronize(nullptr));
+        return *this;
+    }
+    /// SelectByIndex (voxelgrid.cu:432-475): invert gives the voxels not among indices, ascending (repeats allowed);
+    /// an index outside [0, size) throws
+    std::shared_ptr<VoxelGrid> SelectByIndex(const utility::device_vector<size_t> &indices, bool invert = false) const {
+        auto out = std::make_shared<VoxelGrid>();
+        out->voxel_size_ = voxel_size_;
+        out->origin_ = origin_;
+        const size_t rows = invert ? voxels_keys_.size() : indices.size();
+        out->voxels_keys_.resize(rows);
+        out->voxels_colors_.resize(rows);
+        size_t m = 0;
+        utility::check(cphb_voxel_grid_select_by_index(keys(), colors(), voxels_keys_.size(),
+                                                       reinterpret_cast<const int64_t *>(indices.data()), indices.size(),
+                                                       invert ? 1 : 0, out->keys(), out->colors(), &m, nullptr));
+        out->voxels_keys_.resize(m);
+        out->voxels_colors_.resize(m);
+        return out;
+    }
 
 public:
     float voxel_size_ = 0.0f;
     Eigen::Vector3f origin_ = Eigen::Vector3f(0.f, 0.f, 0.f);
     utility::device_vector<Eigen::Vector3i> voxels_keys_;
     utility::device_vector<Eigen::Vector3f> voxels_colors_;
+
+private:
+    int32_t *keys() { return reinterpret_cast<int32_t *>(voxels_keys_.data()); }
+    const int32_t *keys() const { return reinterpret_cast<const int32_t *>(voxels_keys_.data()); }
+    float *colors() { return reinterpret_cast<float *>(voxels_colors_.data()); }
+    // keys assigned without colours get the default (1, 1, 1)
+    const float *colors() const {
+        if (voxels_colors_.size() != voxels_keys_.size()) {
+            auto &c = const_cast<utility::device_vector<Eigen::Vector3f> &>(voxels_colors_);
+            c = std::vector<Eigen::Vector3f>(voxels_keys_.size(), Eigen::Vector3f(1.f, 1.f, 1.f));
+        }
+        return reinterpret_cast<const float *>(voxels_colors_.data());
+    }
+    VoxelGrid &carve(const Image &image, const camera::PinholeCameraParameters &cam, bool keep_outside, const char *what) {
+        if (image.height_ != cam.intrinsic_.height_ || image.width_ != cam.intrinsic_.width_)
+            throw std::runtime_error(std::string("[VoxelGrid] provided ") + what +
+                                     " dimensions are not compatible with the provided camera_parameters");
+        float K[9], E[16];
+        for (int r = 0; r < 3; ++r)
+            for (int c = 0; c < 3; ++c) K[3 * r + c] = cam.intrinsic_.intrinsic_matrix_(r, c);
+        utility::to_row_major(cam.extrinsic_, E);
+        const float o[3] = {origin_[0], origin_[1], origin_[2]};
+        const size_t n = voxels_keys_.size();
+        utility::device_vector<Eigen::Vector3i> k(n);
+        utility::device_vector<Eigen::Vector3f> c(n);
+        size_t m = 0;
+        utility::check(cphb_voxel_grid_carve(keys(), static_cast<const VoxelGrid *>(this)->colors(), n, voxel_size_, o,
+                                             image.data_.data(), image.width_, image.height_, image.num_of_channels_,
+                                             image.bytes_per_channel_, K, E, keep_outside ? 1 : 0,
+                                             reinterpret_cast<int32_t *>(k.data()), reinterpret_cast<float *>(c.data()), &m, nullptr));
+        k.resize(m);
+        c.resize(m);
+        voxels_keys_ = k;  // a copy of the m survivors, so a carved grid holds no more than it needs
+        voxels_colors_ = c;
+        return *this;
+    }
+    void merge(const VoxelGrid &other, bool average) {
+        if (voxel_size_ != other.voxel_size_) throw std::runtime_error("[VoxelGrid] Could not combine VoxelGrid because voxel_size differs");
+        if (origin_[0] != other.origin_[0] || origin_[1] != other.origin_[1] || origin_[2] != other.origin_[2])
+            throw std::runtime_error("[VoxelGrid] Could not combine VoxelGrid because origin differs");
+        const size_t n = voxels_keys_.size() + other.voxels_keys_.size();
+        utility::device_vector<Eigen::Vector3i> k(n);
+        utility::device_vector<Eigen::Vector3f> c(n);
+        size_t m = 0;
+        utility::check(cphb_voxel_grid_merge(keys(), static_cast<const VoxelGrid *>(this)->colors(), voxels_keys_.size(), other.keys(),
+                                             other.colors(), other.voxels_keys_.size(), average ? 1 : 0,
+                                             reinterpret_cast<int32_t *>(k.data()), reinterpret_cast<float *>(c.data()), &m, nullptr));
+        k.resize(m);
+        c.resize(m);
+        voxels_keys_ = std::move(k);
+        voxels_colors_ = std::move(c);
+    }
 };
 
 /// geometry::OccupancyVoxel (occupancygrid.h:33-72)
@@ -919,6 +1141,8 @@ public:
 
 private:
     friend class DistanceTransform;  // CreateFromOccupancyGrid reads the dense grid
+    friend class VoxelGrid;          // and so do VoxelGrid's and PointCloud's
+    friend class PointCloud;
     friend struct collision::detail::Operand;  // ComputeIntersection reads it too
     void sync() const {  // the public members are the source of truth, like the reference's
         const float o[3] = {origin_[0], origin_[1], origin_[2]};
@@ -942,6 +1166,35 @@ private:
     }
     cphb_occgrid *h_ = nullptr;
 };
+
+/// keys = the occupied cells' grid indices (ExtractOccupiedVoxels order), colours (0, 0, 1); origin_ = the grid's origin
+/// - (resolution / 2) * voxel_size, so each voxel covers the cell it came from (the reference keeps the grid's origin)
+inline std::shared_ptr<VoxelGrid> VoxelGrid::CreateFromOccupancyGrid(const OccupancyGrid &input) {
+    auto out = std::make_shared<VoxelGrid>();
+    input.sync();
+    size_t n = 0;
+    float o[3];
+    utility::check(cphb_voxel_grid_from_occgrid(input.h_, nullptr, nullptr, 0, &n, o, nullptr));
+    out->voxel_size_ = input.voxel_size_;
+    out->origin_ = Eigen::Vector3f(o[0], o[1], o[2]);
+    out->voxels_keys_.resize(n);
+    out->voxels_colors_.resize(n);
+    if (n) utility::check(cphb_voxel_grid_from_occgrid(input.h_, out->keys(), out->colors(), n, &n, o, nullptr));
+    return out;
+}
+/// a point per occupied cell at (cell + (float)(-(resolution / 2) + 0.5)) * voxel_size + origin, colour (0, 0, 1)
+inline std::shared_ptr<PointCloud> PointCloud::CreateFromOccupancyGrid(const OccupancyGrid &occgrid) {
+    auto out = std::make_shared<PointCloud>();
+    occgrid.sync();
+    size_t n = 0;
+    utility::check(cphb_point_cloud_from_occgrid(occgrid.h_, nullptr, nullptr, 0, &n, nullptr));
+    out->points_.resize(n);
+    out->colors_.resize(n);
+    if (n)
+        utility::check(cphb_point_cloud_from_occgrid(occgrid.h_, reinterpret_cast<float *>(out->points_.data()),
+                                                     reinterpret_cast<float *>(out->colors_.data()), n, &n, nullptr));
+    return out;
+}
 
 /// geometry::DistanceVoxel (distancetransform.h:30-49)
 class DistanceVoxel {

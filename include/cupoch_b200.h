@@ -438,6 +438,61 @@ int cphb_occgrid_get_voxel(const cphb_occgrid *grid, const float point[3], int *
 int cphb_occgrid_get_params(const cphb_occgrid *grid, cphb_occgrid_params *p);
 
 /* ------------------------------------------------------------------------ *
+ * geometry::VoxelGrid operations (voxelgrid.cu, voxelgrid_factory.cu).  A grid is
+ * keys [n][3] int32 + colors [n][3] float32 (device) with voxel_size and origin.
+ * CreateDense, merge and carving leave keys lexicographically sorted and unique
+ * when their inputs are; every lookup also accepts unsorted, repeated keys.
+ * Lookups and merges need a key span below 2^21 on each axis (CPHB_ERR_INVALID).
+ * ------------------------------------------------------------------------ */
+/* VoxelGrid::CreateDense (voxelgrid_factory.cu:134-162): counts int(roundf(extent / voxel_size)) per axis, keys
+ * (w, h, d) in lexicographic order, every colour (1, 1, 1).  *h_n = the voxel count; the keys and colours are written
+ * only when capacity >= it (call with capacity 0 to size).  voxel_size <= 0 or non-finite, a negative, non-finite or
+ * >= 2^31 count, or a total whose keys and colours do not fit a size_t byte count: CPHB_ERR_INVALID. */
+int cphb_voxel_grid_create_dense(float voxel_size, float width, float height, float depth, int32_t *out_keys,
+                                 float *out_colors, size_t capacity, size_t *h_n, void *stream);
+/* VoxelGrid::CheckIfIncluded (voxelgrid.cu:365-376): out[i] = 1 when the cell floor((q_i - origin) / voxel_size) of
+ * query i is one of the keys.  Non-finite queries and cells outside the int range give 0.  queries [nq][3] float32,
+ * out [nq] uint8 (device).  Synchronises. */
+int cphb_voxel_grid_check_if_included(const int32_t *keys, size_t n, float voxel_size, const float h_origin[3],
+                                      const float *queries, size_t nq, uint8_t *out, void *stream);
+/* whether key h_key is one of the keys (GetVoxelCenterCoordinate's find, voxelgrid.cu:343-354).  Synchronises. */
+int cphb_voxel_grid_has_key(const int32_t *keys, size_t n, const int32_t h_key[3], int *h_found, void *stream);
+/* VoxelGrid::CarveDepthMap / CarveSilhouette (voxelgrid.cu:45-123,378-430): a voxel is kept when one of its 8
+ * corners projects, through h_extrinsic (4x4 row-major) and h_intrinsic (3x3 row-major), inside the image with
+ * sampled value d > 0 and z >= d, or outside the image while keep_outside is set.  Only a 1-channel float32 image is
+ * sampled (bilinear, FloatValueAt of image.h:240-270); any other kind is outside everywhere, and image may then be
+ * NULL.  A corner with z == 0 or a non-finite u or v is outside.  The survivors keep their order in out_keys /
+ * out_colors (n rows); *h_n_out = their number (synchronises).  width or height < 2: CPHB_ERR_INVALID. */
+int cphb_voxel_grid_carve(const int32_t *keys, const float *colors, size_t n, float voxel_size, const float h_origin[3],
+                          const void *image, int width, int height, int num_of_channels, int bytes_per_channel,
+                          const float h_intrinsic[9], const float h_extrinsic[16], int keep_outside, int32_t *out_keys,
+                          float *out_colors, size_t *h_n_out, void *stream);
+/* VoxelGrid::operator+= (average = 1, voxelgrid.cu:235-286) and AddVoxels (average = 0, :288-319): a's voxels then
+ * b's, stable-sorted by key; each run of equal keys becomes one voxel whose colour is the run's colours summed left to
+ * right in float and divided by the run length (average = 1), or the run's first colour (average = 0).  Outputs hold
+ * na + nb rows; *h_n_out = the voxel count (synchronises).  na + nb > 2^31-1: CPHB_ERR_INVALID. */
+int cphb_voxel_grid_merge(const int32_t *keys_a, const float *colors_a, size_t na, const int32_t *keys_b,
+                          const float *colors_b, size_t nb, int average, int32_t *out_keys, float *out_colors,
+                          size_t *h_n_out, void *stream);
+/* PaintUniformColor (indices NULL) and PaintIndexedColor (voxelgrid.cu:321-336): colors[i] = h_color for every i, or
+ * for every i in indices [m] int64.  An index outside [0, n) is CPHB_ERR_INVALID and nothing is painted. */
+int cphb_voxel_grid_paint(float *colors, size_t n, const int64_t *indices, size_t m, const float h_color[3], void *stream);
+/* VoxelGrid::SelectByIndex (voxelgrid.cu:432-475): invert = 0: out row t = row indices[t] (m rows); invert = 1: the
+ * rows not among indices, ascending (repeated indices are allowed).  An index outside [0, n) is CPHB_ERR_INVALID.
+ * Outputs hold m (invert = 0) or n (invert = 1) rows; *h_n_out = rows written (synchronises). */
+int cphb_voxel_grid_select_by_index(const int32_t *keys, const float *colors, size_t n, const int64_t *indices, size_t m,
+                                    int invert, int32_t *out_keys, float *out_colors, size_t *h_n_out, void *stream);
+/* VoxelGrid::CreateFromOccupancyGrid (voxelgrid_factory.cu:283-305): keys = the occupied cells' grid indices in
+ * ExtractOccupiedVoxels order, colours (0, 0, 1); h_origin = grid origin - (resolution / 2) * voxel_size, so every
+ * voxel covers the cell it came from.  PointCloud::CreateFromOccupancyGrid (pointcloud_factory.cu:239-256,418-430):
+ * point = (cell + (float)(-(resolution / 2) + 0.5)) * voxel_size + origin, colour (0, 0, 1).  *h_count = the occupied
+ * count; rows are written only when capacity >= it (capacity 0 sizes).  Synchronises. */
+int cphb_voxel_grid_from_occgrid(const cphb_occgrid *grid, int32_t *out_keys, float *out_colors, size_t capacity,
+                                 size_t *h_count, float h_origin[3], void *stream);
+int cphb_point_cloud_from_occgrid(const cphb_occgrid *grid, float *out_points, float *out_colors, size_t capacity,
+                                  size_t *h_count, void *stream);
+
+/* ------------------------------------------------------------------------ *
  * geometry::DistanceTransform (distancetransform.h, distancetransform.cu): a
  * dense resolution^3 grid, cell (x, y, z) at linear index (x * res + y) * res + z
  * and centred on origin like the OccupancyGrid.  Each cell holds its nearest

@@ -38,12 +38,17 @@ def main():
     ap.add_argument("--out", default=None, help="--shot, --crop: also write the JSON object to this file")
     ap.add_argument("--edt", action="store_true",
                     help="instead: time geometry::DistanceTransform::ComputeEDT at 256^3 and 512^3 and GetDistances of 10 M points")
+    ap.add_argument("--voxelgrid", action="store_true",
+                    help="instead: time the VoxelGrid operations (CreateDense, carving, CheckIfIncluded, +=, "
+                         "CreateFromOccupancyGrid) on the config-3 VoxelGrid and 512^3 grids")
     ap.add_argument("--collision", action="store_true",
                     help="instead: time collision::ComputeIntersection on the config-3 VoxelGrid, a 512^3 OccupancyGrid and "
                          "1 / 1e4 primitives")
     args = ap.parse_args()
     if args.collision:
         return collision(args.reps, args.out)
+    if args.voxelgrid:
+        return voxelgrid(args.reps, args.out)
     if args.edt:
         return edt(args.reps)
     if args.segment_plane:
@@ -812,6 +817,118 @@ def collision(reps, out=None):
                      "share_of_3.35TBps_over_kernel_time": nbytes / (kern_ms * 1e-3) / HBM_BYTES_PER_S if kern_ms else None})
     obj = {"op": "collision::ComputeIntersection on the config-3 cloud voxelised at 0.02 (%d voxels), a 512^3 "
                  "OccupancyGrid after a 1 M-point scan (%d cells in its bound box) and 1 / 1e4 mixed primitives" % (n_vg, box_cells),
+           "gpu": gpu, "reps": reps, "rows": rows}
+    line = json.dumps(obj)
+    print(line)
+    if out:
+        with open(out, "w") as f:
+            f.write(line + "\n")
+
+
+def voxelgrid_bytes_model(op, n, m=0):
+    """least HBM traffic of one call: keys and colours are 12 bytes each a voxel; a sort pass reads and writes 8-byte
+    packed keys and 4-byte indices (counted once), a query reads 12 bytes and writes 1"""
+    if op == "dense":
+        return 24 * n
+    if op == "carve":
+        return 12 * n + 24 * m
+    if op == "included":
+        return 12 * n + 24 * n + 13 * m
+    if op == "merge":
+        return 48 * n + 24 * n + 24 * m
+    if op in ("vg_from_occ", "pc_from_occ"):
+        return 4 * n + 24 * m  # the log-odds of the grid's bound box (n cells) read once, the rows written
+    raise ValueError(op)
+
+
+def voxelgrid(reps, out=None):
+    """CreateDense at 256^3 and 512^3; one carve of a dense 512^3 grid by a sphere's depth map; CheckIfIncluded of 10 M
+    queries against the config-3 cloud voxelised at 0.02 (about 2 M voxels); += of that grid and a shifted one; both
+    CreateFromOccupancyGrid calls on a 512^3 grid after a 1 M-point scan.  CUDA-event median and minimum of `reps` calls
+    after a warm-up call (host upload of queries and images included where the call takes host data), the kernel time
+    of one further call from torch.profiler, and the bytes model beside it."""
+    import subprocess
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    import cupoch_b200 as cph
+    from cupoch_b200 import _lib
+    from cupoch_b200.testing import datagen
+    from cupoch_b200.testing.datagen import ring_cameras, sphere_depth
+    L = _lib.lib()
+    G = cph.geometry
+    gpu = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                         capture_output=True, text=True).stdout.strip()
+    ev = [L.cphb_event_create() for _ in range(2)]
+
+    def timed(fn, prep=None):
+        times = []
+        for r in range(reps + 1):
+            arg = prep() if prep else None
+            L.cphb_event_record(ev[0], None)
+            fn(arg)
+            L.cphb_event_record(ev[1], None)
+            ms = C.c_float(0)
+            _lib.check(L.cphb_event_elapsed_ms(ev[0], ev[1], C.byref(ms)))
+            if r:
+                times.append(ms.value)
+        return times
+
+    vs = 0.02
+    pts = datagen.uniform_cube(10_000_000, 21, hi=(4, 4, 1))
+    a = G.VoxelGrid.create_from_point_cloud_within_bounds(G.PointCloud(pts), vs, (0, 0, 0), (6, 4, 1))
+    b = G.VoxelGrid.create_from_point_cloud_within_bounds(G.PointCloud((pts + np.float32([2, 0, 0])).astype(np.float32)), vs,
+                                                          (0, 0, 0), (6, 4, 1))
+    del pts
+    q = np.random.default_rng(1).uniform((0, 0, 0), (4, 4, 1), (10_000_000, 3)).astype(np.float32)
+    scan = datagen.surface(1_000_000, 11, extent=4.0)[0] + np.array([0, 0, 0.5], np.float32)
+    occ = G.OccupancyGrid(vs, 512, (2.0, 2.0, 0.5))
+    occ.insert(G.PointCloud(scan.astype(np.float32)), (2.0, 2.0, 3.0))
+    K, E = ring_cameras(1, 640, 480)[0]
+    img = G.Image(sphere_depth(K, E, 640, 480, 0.8))
+    cam = cph.camera.PinholeCameraParameters(cph.camera.PinholeCameraIntrinsic(640, 480, K[0, 0], K[1, 1], K[0, 2], K[1, 2]), E)
+    n_occ = len(occ.extract_occupied_voxels()[0])
+    lo, hi = occ._bounds()
+    box_cells = int(np.prod((hi - lo + 1).astype(np.int64)))
+
+    def dense(r):
+        return lambda _: G.VoxelGrid.create_dense((-1, -1, -1), 2.0 / r, 2, 2, 2)
+
+    def fresh512():
+        return G.VoxelGrid.create_dense((-1, -1, -1), 2.0 / 512, 2, 2, 2)
+
+    carved = len(fresh512().carve_depth_map(img, cam))
+    work = [("CreateDense 256^3", dense(256), None, ("dense", 256 ** 3, 0)),
+            ("CreateDense 512^3", dense(512), None, ("dense", 512 ** 3, 0)),
+            ("CarveDepthMap of a dense 512^3 grid, 640x480 depth map", lambda g: g.carve_depth_map(img, cam), fresh512,
+             ("carve", 512 ** 3, carved)),
+            ("CheckIfIncluded, 10 M queries, %d voxels" % len(a), lambda _: a.check_if_included(q), None,
+             ("included", len(a), len(q))),
+            ("+= of %d and %d voxels" % (len(a), len(b)), lambda _: a + b, None, ("merge", len(a) + len(b), len(a + b))),
+            ("VoxelGrid.create_from_occupancy_grid 512^3", lambda _: G.VoxelGrid.create_from_occupancy_grid(occ), None,
+             ("vg_from_occ", box_cells, n_occ)),
+            ("PointCloud.create_from_occupancy_grid 512^3", lambda _: G.PointCloud.create_from_occupancy_grid(occ), None,
+             ("pc_from_occ", box_cells, n_occ))]
+    rows = []
+    for name, fn, prep, (op, n, m) in work:
+        ts = timed(fn, prep)
+        arg = prep() if prep else None
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            fn(arg)
+            torch.cuda.synchronize()
+        kernels = {}
+        for e in prof.key_averages():
+            t = getattr(e, "device_time_total", getattr(e, "cuda_time_total", 0.0)) * 1e-3
+            if t > 0 and "Memset" not in e.key and "Memcpy" not in e.key:
+                kernels[e.key[:60]] = kernels.get(e.key[:60], 0.0) + t
+        kern_ms = float(sum(kernels.values()))
+        nbytes = voxelgrid_bytes_model(op, n, m)
+        rows.append({"workload": name, "n": n, "m": m, "call_ms_median": float(np.median(ts)), "call_ms_min": float(np.min(ts)),
+                     "kernel_ms_profiled": kernels, "kernel_ms_sum": kern_ms, "bytes_model": nbytes,
+                     "share_of_3.35TBps_over_kernel_time": nbytes / (kern_ms * 1e-3) / HBM_BYTES_PER_S if kern_ms else None})
+        del arg
+    obj = {"op": "VoxelGrid operations: dense grids, carving, CheckIfIncluded and += on the config-3 cloud voxelised at "
+                 "0.02, CreateFromOccupancyGrid on a 512^3 grid after a 1 M-point scan (%d occupied cells)" % n_occ,
            "gpu": gpu, "reps": reps, "rows": rows}
     line = json.dumps(obj)
     print(line)

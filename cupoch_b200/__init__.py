@@ -5,8 +5,10 @@
             cph.registration.TransformationEstimationPointToPlane())
 
 Mirrors `import cupoch as cph` for: cph.geometry.{PointCloud, KDTreeFlann, KDTreeSearchParamKNN,
-KDTreeSearchParamRadius, VoxelGrid, OccupancyGrid, OccupancyVoxel, DistanceTransform, DistanceVoxel,
+KDTreeSearchParamRadius, VoxelGrid, OccupancyGrid, OccupancyVoxel, DistanceTransform, DistanceVoxel, Image, RGBDImage,
 keypoint.compute_iss_keypoints},
+cph.camera.{PinholeCameraIntrinsic, PinholeCameraIntrinsicParameters, PinholeCameraParameters},
+cph.integration.{UniformTSDFVolume, TSDFVolumeColorType},
 cph.registration.{registration_icp,
 registration_generalized_icp, registration_colored_icp, ICPConvergenceCriteria, TransformationEstimation*
 (user subclasses run the generic loop), RegistrationResult, compute_fpfh_feature, compute_shot_feature, FeatureSHOT, kabsch, kabsch_weighted},
@@ -15,7 +17,7 @@ cph.utility.{Vector3fVector, compute_jtj_jtr, compute_weighted_jtj_jtr}; cupoch_
 multi-GPU orchestration (torch.distributed).  All computation runs in libcupoch_b200.so (hand-written sm_90a CUDA);
 there is no CPU fallback.
 """
-from . import _lib, camera, collision, geometry, registration, utility  # noqa: F401
+from . import _lib, camera, collision, geometry, integration, registration, utility  # noqa: F401
 
 __version__ = "0.1.0"
 

@@ -98,6 +98,17 @@ _SIGNATURES = {
     "cphb_dt_get_voxel": (C.c_int, [_P, _F3, C.POINTER(C.c_int), _I3, C.POINTER(C.c_int), C.POINTER(C.c_float), _P]),
     "cphb_dt_distance_data": (_P, [_P]),
     "cphb_dt_nearest_data": (_P, [_P]),
+    "cphb_rgbd_convert": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, _P, _P]),
+    "cphb_tsdf_create": (C.c_int, [C.c_float, C.c_int, C.c_float, C.c_int, _F3, _P, C.POINTER(_P)]),
+    "cphb_tsdf_destroy": (None, [_P]),
+    "cphb_tsdf_reset": (C.c_int, [_P, _P]),
+    "cphb_tsdf_data": (C.c_int, [_P, C.POINTER(_P), C.POINTER(_P)]),
+    "cphb_tsdf_integrate": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                      C.c_int, _F3, _F3, _P]),
+    "cphb_tsdf_extract_points": (C.c_int, [_P, _P, _P, _P, C.c_size_t, C.POINTER(C.c_size_t), _P]),
+    "cphb_tsdf_extract_voxels": (C.c_int, [_P, _P, _P, _P, C.c_size_t, C.POINTER(C.c_size_t), _P]),
+    "cphb_tsdf_raycast": (C.c_int, [_P, C.c_int, C.c_int, _F3, _F3, C.c_float, C.c_int, _P, _P, _P, C.c_size_t,
+                                    C.POINTER(C.c_size_t), _P]),
     # name: (restype, argtypes)
     "cphb_version": (C.c_int, []),
     "cphb_last_error": (C.c_char_p, []),

@@ -1,7 +1,15 @@
 """cupoch.camera mirror: the pinhole camera model as plain data (pinhole_camera_intrinsic.h,
 pinhole_camera_parameters.h; pybind camera/camera.cpp), what VoxelGrid.carve_depth_map / carve_silhouette project
 through.  Nothing here touches the device."""
+import enum
+
 import numpy as np
+
+
+class PinholeCameraIntrinsicParameters(enum.IntEnum):
+    """camera::PinholeCameraIntrinsicParameters (pinhole_camera_intrinsic.h:33-40): the defaults an intrinsic can be
+    built from.  Only PrimeSenseDefault (640 x 480, fx = fy = 525, cx = 319.5, cy = 239.5) is provided."""
+    PrimeSenseDefault = 0
 
 
 class PinholeCameraIntrinsic:
@@ -9,6 +17,8 @@ class PinholeCameraIntrinsic:
     [[fx, 0, cx], [0, fy, cy], [0, 0, 1]] (float32)."""
 
     def __init__(self, width=-1, height=-1, fx=0.0, fy=0.0, cx=0.0, cy=0.0):
+        if isinstance(width, PinholeCameraIntrinsicParameters):  # PrimeSenseDefault
+            width, height, fx, fy, cx, cy = 640, 480, 525.0, 525.0, 319.5, 239.5
         self.set_intrinsics(width, height, fx, fy, cx, cy)
 
     @property

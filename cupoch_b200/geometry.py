@@ -906,6 +906,96 @@ class Image:
         return "geometry::Image of size %dx%d, with %d channels." % (self.width, self.height, self.num_of_channels)
 
 
+class RGBDImage:
+    """geometry::RGBDImage (rgbdimage.h): a colour and a depth image of the same size, built by the create_from_*
+    factories.  The converted images live on the device, where UniformTSDFVolume.integrate reads them; `color` and
+    `depth` download them as geometry.Image on first access.  RGBDImage(color, depth) wraps two host Images as they
+    are (no conversion), as the reference's constructor does."""
+
+    def __init__(self, color=None, depth=None):
+        self._color, self._depth = (Image() if color is None else color), (Image() if depth is None else depth)
+        self._d_color = self._d_depth = None
+
+    @staticmethod
+    def _from_device(d_color, d_depth):
+        out = RGBDImage()
+        out._color = out._depth = None
+        out._d_color, out._d_depth = d_color, d_depth
+        return out
+
+    @property
+    def color(self):
+        if self._color is None:
+            self._color = Image(self._d_color.cpu())
+        return self._color
+
+    @property
+    def depth(self):
+        if self._depth is None:
+            self._depth = Image(self._d_depth.cpu())
+        return self._depth
+
+    def _device(self):
+        """(color, depth) as device arrays; host images are uploaded once"""
+        if self._d_depth is None:
+            self._d_depth = DeviceArray.from_numpy(self._depth._data, self._depth._data.dtype)
+        if self._d_color is None:
+            self._d_color = DeviceArray.from_numpy(self._color._data, self._color._data.dtype)
+        return self._d_color, self._d_depth
+
+    @staticmethod
+    def _info(d):
+        """(width, height, channels, bytes_per_channel) of a device image"""
+        return (d.shape[1], d.shape[0], 1 if len(d.shape) == 2 else d.shape[2], d.dtype.itemsize)
+
+    def _depth_info(self):
+        return self._info(self._device()[1])
+
+    def _color_info(self):
+        return self._info(self._device()[0])
+
+    def is_empty(self):
+        return self.depth.is_empty()
+
+    def __repr__(self):
+        return "geometry::RGBDImage of size %dx%d." % (self.depth.width, self.depth.height)
+
+    @staticmethod
+    def _convert(image, to_depth, depth_scale=1000.0, depth_trunc=3.0):
+        a = image._data
+        src = DeviceArray.from_numpy(a, a.dtype)
+        out = DeviceArray(a.shape[:2], np.float32)
+        _lib.check(_lib.lib().cphb_rgbd_convert(src.ptr, image.width, image.height, image.num_of_channels, image.bytes_per_channel,
+                                                int(to_depth), float(depth_scale), float(depth_trunc), out.ptr, None))
+        _lib.check(_lib.lib().cphb_stream_synchronize(None))
+        return out
+
+    @staticmethod
+    def create_from_color_and_depth(color, depth, depth_scale=1000.0, depth_trunc=3.0, convert_rgb_to_intensity=True):
+        """RGBDImage::CreateFromColorAndDepth (rgbdimage_factory.cu:56-72): depth -> float32 metres, the raw value /
+        int(depth_scale) and 0 where it is >= int(depth_trunc) (the reference converts both to int, so depth_trunc
+        = 2.5 cuts at 2 m); colour -> float32 weighted intensity (/ 255 for 8-bit) when convert_rgb_to_intensity, else
+        kept as it is.  Images of different sizes raise, as does a depth_scale below 1 (int 0 would divide by zero)."""
+        if color.height != depth.height or color.width != depth.width:
+            raise ValueError("[CreateFromColorAndDepth] Unsupported image format.")
+        d = RGBDImage._convert(depth, True, depth_scale, depth_trunc)
+        if convert_rgb_to_intensity:
+            c = RGBDImage._convert(color, False)
+        else:
+            c = DeviceArray.from_numpy(color._data, color._data.dtype)
+        return RGBDImage._from_device(c, d)
+
+    @staticmethod
+    def create_from_redwood_format(color, depth, convert_rgb_to_intensity=True):
+        """CreateFromRedwoodFormat: depth_scale 1000, depth_trunc 4"""
+        return RGBDImage.create_from_color_and_depth(color, depth, 1000.0, 4.0, convert_rgb_to_intensity)
+
+    @staticmethod
+    def create_from_tum_format(color, depth, convert_rgb_to_intensity=True):
+        """CreateFromTUMFormat: depth_scale 5000, depth_trunc 4"""
+        return RGBDImage.create_from_color_and_depth(color, depth, 5000.0, 4.0, convert_rgb_to_intensity)
+
+
 class OccupancyVoxel:
     """geometry::OccupancyVoxel (occupancygrid.h:33-72): grid_index (3 uint16), prob_log, color (the default (0, 0, 1):
     nothing on this path ever changes it)."""

@@ -297,10 +297,14 @@ private:
 
 // --------------------------------------------------------------------------- camera
 namespace camera {
+/// camera::PinholeCameraIntrinsicParameters (pinhole_camera_intrinsic.h:33-40): only PrimeSenseDefault is provided
+enum class PinholeCameraIntrinsicParameters { PrimeSenseDefault = 0 };
 /// camera::PinholeCameraIntrinsic (pinhole_camera_intrinsic.h): width_, height_ and the 3x3 intrinsic_matrix_
 class PinholeCameraIntrinsic {
 public:
     PinholeCameraIntrinsic() {}
+    /// PrimeSenseDefault: 640 x 480, fx = fy = 525, cx = 319.5, cy = 239.5
+    PinholeCameraIntrinsic(PinholeCameraIntrinsicParameters) { SetIntrinsics(640, 480, 525.0f, 525.0f, 319.5f, 239.5f); }
     PinholeCameraIntrinsic(int width, int height, float fx, float fy, float cx, float cy) { SetIntrinsics(width, height, fx, fy, cx, cy); }
     void SetIntrinsics(int width, int height, float fx, float fy, float cx, float cy) {
         width_ = width;
@@ -1862,4 +1866,181 @@ inline std::shared_ptr<CollisionResult> ComputeIntersection(const PrimitiveArray
     return detail::compute(detail::Operand(primitives), detail::Operand(occgrid), margin);
 }
 }  // namespace collision
+
+// --------------------------------------------------------------------------- RGBDImage and the TSDF volume
+namespace geometry {
+/// geometry::RGBDImage (rgbdimage.h): a colour and a depth image of the same size
+class RGBDImage {
+public:
+    RGBDImage() {}
+    RGBDImage(const Image &color, const Image &depth) : color_(color), depth_(depth) {}
+    bool IsEmpty() const { return depth_.IsEmpty(); }
+    /// CreateFromColorAndDepth (rgbdimage_factory.cu:56-72): depth -> float32 metres, raw / int(depth_scale), 0 where it
+    /// is >= int(depth_trunc); colour -> float32 weighted intensity when convert_rgb_to_intensity, else kept
+    static std::shared_ptr<RGBDImage> CreateFromColorAndDepth(const Image &color, const Image &depth, float depth_scale = 1000.0f,
+                                                              float depth_trunc = 3.0f, bool convert_rgb_to_intensity = true) {
+        if (color.height_ != depth.height_ || color.width_ != depth.width_)
+            throw std::runtime_error("[CreateFromColorAndDepth] Unsupported image format.");
+        auto out = std::make_shared<RGBDImage>();
+        convert(depth, true, depth_scale, depth_trunc, out->depth_);
+        if (convert_rgb_to_intensity)
+            convert(color, false, 0.f, 0.f, out->color_);
+        else
+            out->color_ = color;
+        return out;
+    }
+    static std::shared_ptr<RGBDImage> CreateFromRedwoodFormat(const Image &color, const Image &depth, bool convert_rgb_to_intensity = true) {
+        return CreateFromColorAndDepth(color, depth, 1000.0f, 4.0f, convert_rgb_to_intensity);
+    }
+    static std::shared_ptr<RGBDImage> CreateFromTUMFormat(const Image &color, const Image &depth, bool convert_rgb_to_intensity = true) {
+        return CreateFromColorAndDepth(color, depth, 5000.0f, 4.0f, convert_rgb_to_intensity);
+    }
+
+public:
+    Image color_;
+    Image depth_;
+
+private:
+    static void convert(const Image &in, bool to_depth, float scale, float trunc, Image &out) {
+        out.Prepare(in.width_, in.height_, 1, 4);
+        utility::check(cphb_rgbd_convert(in.data_.data(), in.width_, in.height_, in.num_of_channels_, in.bytes_per_channel_, to_depth ? 1 : 0,
+                                         scale, trunc, reinterpret_cast<float *>(out.data_.data()), nullptr));
+        utility::check(cphb_stream_synchronize(nullptr));
+    }
+};
+}  // namespace geometry
+
+namespace integration {
+/// integration::TSDFVolumeColorType (tsdfvolume.h)
+enum class TSDFVolumeColorType { NoColor = 0, RGB8 = 1, Gray32 = 2 };
+
+/// integration::TSDFVolume (tsdfvolume.h): the members the reference's base class holds
+class TSDFVolume {
+public:
+    TSDFVolume(float voxel_length, float sdf_trunc, TSDFVolumeColorType color_type)
+        : voxel_length_(voxel_length), sdf_trunc_(sdf_trunc), color_type_(color_type) {}
+    virtual ~TSDFVolume() {}
+
+public:
+    float voxel_length_;
+    float sdf_trunc_;
+    TSDFVolumeColorType color_type_;
+};
+
+/// integration::UniformTSDFVolume (uniform_tsdfvolume.h): a dense resolution^3 grid owned by a cphb_tsdf handle.
+/// Reset restores the initial voxels; a resolution outside [2, 1290] or a length or sdf_trunc that is not positive and
+/// finite throws.  Not copyable (the grid stays on the device).
+class UniformTSDFVolume : public TSDFVolume {
+public:
+    UniformTSDFVolume(float length, int resolution, float sdf_trunc, TSDFVolumeColorType color_type,
+                      const Eigen::Vector3f &origin = Eigen::Vector3f(0.f, 0.f, 0.f))
+        : TSDFVolume(length / (float)resolution, sdf_trunc, color_type), origin_(origin), length_(length), resolution_(resolution),
+          voxel_num_((size_t)(resolution > 0 ? resolution : 0) * (resolution > 0 ? resolution : 0) * (resolution > 0 ? resolution : 0)) {
+        const float o[3] = {origin[0], origin[1], origin[2]};
+        utility::check(cphb_tsdf_create(length, resolution, sdf_trunc, (int)color_type, o, nullptr, &h_));
+    }
+    UniformTSDFVolume(const UniformTSDFVolume &) = delete;
+    UniformTSDFVolume &operator=(const UniformTSDFVolume &) = delete;
+    ~UniformTSDFVolume() override {
+        if (h_) {
+            cphb_stream_synchronize(nullptr);
+            cphb_tsdf_destroy(h_);
+        }
+    }
+    void Reset() {
+        utility::check(cphb_tsdf_reset(h_, nullptr));
+        utility::check(cphb_stream_synchronize(nullptr));
+    }
+    /// Integrate (uniform_tsdfvolume.cu:670-701); extrinsic is world-to-camera
+    void Integrate(const geometry::RGBDImage &image, const camera::PinholeCameraIntrinsic &intrinsic, const Eigen::Matrix4f &extrinsic) {
+        float K[9], E[16];
+        intrinsic9(intrinsic, K);
+        utility::to_row_major(extrinsic, E);
+        const geometry::Image &d = image.depth_, &c = image.color_;
+        utility::check(cphb_tsdf_integrate(h_, reinterpret_cast<const float *>(d.data_.data()), d.width_, d.height_, d.num_of_channels_,
+                                           d.bytes_per_channel_, c.data_.data(), c.width_, c.height_, c.num_of_channels_,
+                                           c.bytes_per_channel_, intrinsic.width_, intrinsic.height_, K, E, nullptr));
+        utility::check(cphb_stream_synchronize(nullptr));
+    }
+    /// ExtractPointCloud (uniform_tsdfvolume.cu:703-737): points, normals and (with colour) colours of the crossings
+    std::shared_ptr<geometry::PointCloud> ExtractPointCloud() {
+        auto pc = std::make_shared<geometry::PointCloud>();
+        size_t n = 0;
+        utility::check(cphb_tsdf_extract_points(h_, nullptr, nullptr, nullptr, 0, &n, nullptr));
+        if (n) {
+            pc->points_.resize(n);
+            pc->normals_.resize(n);
+            if (color_type_ != TSDFVolumeColorType::NoColor) pc->colors_.resize(n);
+            utility::check(cphb_tsdf_extract_points(h_, (float *)pc->points_.data(), (float *)pc->normals_.data(),
+                                                    color_type_ != TSDFVolumeColorType::NoColor ? (float *)pc->colors_.data() : nullptr,
+                                                    n, &n, nullptr));
+        }
+        return pc;
+    }
+    /// ExtractVoxelPointCloud (uniform_tsdfvolume.cu:840-865): band voxel centres coloured (tsdf + 1) / 2
+    std::shared_ptr<geometry::PointCloud> ExtractVoxelPointCloud() const {
+        auto pc = std::make_shared<geometry::PointCloud>();
+        size_t n = 0;
+        utility::check(cphb_tsdf_extract_voxels(h_, nullptr, nullptr, nullptr, 0, &n, nullptr));
+        if (n) {
+            pc->points_.resize(n);
+            pc->colors_.resize(n);
+            utility::check(cphb_tsdf_extract_voxels(h_, nullptr, (float *)pc->points_.data(), (float *)pc->colors_.data(), n, &n, nullptr));
+        }
+        return pc;
+    }
+    /// ExtractVoxelGrid (uniform_tsdfvolume.cu:867-895): band voxels, origin = origin - (resolution / 2) * voxel_length
+    std::shared_ptr<geometry::VoxelGrid> ExtractVoxelGrid() const {
+        auto vg = std::make_shared<geometry::VoxelGrid>();
+        vg->voxel_size_ = voxel_length_;
+        const float half = (float)(resolution_ / 2) * voxel_length_;
+        vg->origin_ = Eigen::Vector3f(origin_[0] - half, origin_[1] - half, origin_[2] - half);
+        size_t n = 0;
+        utility::check(cphb_tsdf_extract_voxels(h_, nullptr, nullptr, nullptr, 0, &n, nullptr));
+        if (n) {
+            vg->voxels_keys_.resize(n);
+            vg->voxels_colors_.resize(n);
+            utility::check(cphb_tsdf_extract_voxels(h_, (int32_t *)vg->voxels_keys_.data(), nullptr, (float *)vg->voxels_colors_.data(), n, &n,
+                                                    nullptr));
+        }
+        return vg;
+    }
+    /// Raycast (uniform_tsdfvolume.cu:924-951): one ray per pixel from the camera at extrinsic (world-to-camera)
+    std::shared_ptr<geometry::PointCloud> Raycast(const camera::PinholeCameraIntrinsic &intrinsic, const Eigen::Matrix4f &extrinsic,
+                                                  float sdf_trunc, bool project_valid_depth_only = true) const {
+        float K[9], E[16];
+        intrinsic9(intrinsic, K);
+        utility::to_row_major(extrinsic, E);
+        const size_t npx = (size_t)std::max(intrinsic.width_, 0) * (size_t)std::max(intrinsic.height_, 0);
+        utility::device_vector<Eigen::Vector3f> p(npx), nr(npx), c(npx);
+        size_t n = 0;
+        utility::check(cphb_tsdf_raycast(h_, intrinsic.width_, intrinsic.height_, K, E, sdf_trunc, project_valid_depth_only ? 1 : 0,
+                                         (float *)p.data(), (float *)nr.data(), (float *)c.data(), npx, &n, nullptr));
+        auto pc = std::make_shared<geometry::PointCloud>();
+        pc->points_.resize(n);
+        pc->normals_.resize(n);
+        pc->colors_.resize(n);
+        if (n) {
+            utility::check(cphb_memcpy_d2d(pc->points_.data(), p.data(), 12 * n, nullptr));
+            utility::check(cphb_memcpy_d2d(pc->normals_.data(), nr.data(), 12 * n, nullptr));
+            utility::check(cphb_memcpy_d2d(pc->colors_.data(), c.data(), 12 * n, nullptr));
+            utility::check(cphb_stream_synchronize(nullptr));
+        }
+        return pc;
+    }
+
+public:
+    Eigen::Vector3f origin_;
+    float length_;
+    int resolution_;
+    size_t voxel_num_;
+
+private:
+    static void intrinsic9(const camera::PinholeCameraIntrinsic &in, float K[9]) {
+        for (int r = 0; r < 3; ++r)
+            for (int c = 0; c < 3; ++c) K[3 * r + c] = in.intrinsic_matrix_(r, c);
+    }
+    cphb_tsdf *h_ = nullptr;
+};
+}  // namespace integration
 }  // namespace cupoch

@@ -534,6 +534,58 @@ const float *cphb_dt_distance_data(const cphb_dt *dt);   /* device distance[res^
 const uint32_t *cphb_dt_nearest_data(const cphb_dt *dt); /* device nearest[res^3] (packed as above), borrowed */
 
 /* ------------------------------------------------------------------------ *
+ * integration::UniformTSDFVolume (integration/uniform_tsdfvolume.cu) and the RGB-D conversion it reads
+ * (geometry/rgbdimage_factory.cu, image.cu, image_factory.cu).  A volume owns a dense resolution^3 grid on the device:
+ * a float2 {tsdf, weight} plane and, by color_type (0 NoColor, 1 RGB8, 2 Gray32), 3, 1 or 0 float colour planes.
+ * Voxel idx = x res^2 + y res + z; its centre is origin + vl (k - res / 2) + vl / 2, vl = length / resolution.
+ * Images and outputs are device buffers, borrowed; the outputs are caller-allocated.  Matrices are row-major:
+ * the 3x3 intrinsic [[fx, 0, cx], [0, fy, cy], [0, 0, 1]] and the 4x4 world-to-camera extrinsic.
+ * ------------------------------------------------------------------------ */
+typedef struct cphb_tsdf cphb_tsdf;
+/* CreateFromColorAndDepth's image conversion, [height * width] float32 out.  to_depth: ConvertDepthToFloatImage of a
+ * 1-channel image -- raw value (x 1/255 for 8-bit) / (float)(int)depth_scale, 0 where it is >= (float)(int)depth_trunc;
+ * depth_scale < 1 (which truncates to 0) or a non-finite one is CPHB_ERR_INVALID.  Otherwise CreateFloatImage(WEIGHTED)
+ * of a 1- or 3-channel image (x 1/255 for 8-bit).  bytes_per_channel 1, 2 or 4 (uint8, uint16, float32).  Asynchronous. */
+int cphb_rgbd_convert(const void *src, int width, int height, int channels, int bytes_per_channel, int to_depth, float depth_scale,
+                      float depth_trunc, float *out, void *stream);
+/* UniformTSDFVolume(length, resolution, sdf_trunc, color_type, origin): every voxel tsdf 0, weight 0, colour (1, 1, 1).
+ * resolution outside [2, 1290] (the voxel count must fit int32), a length or sdf_trunc that is not positive and finite,
+ * or an unknown color_type: CPHB_ERR_INVALID.  origin may be NULL (zero). */
+int cphb_tsdf_create(float length, int resolution, float sdf_trunc, int color_type, const float origin[3], void *stream,
+                     cphb_tsdf **out);
+void cphb_tsdf_destroy(cphb_tsdf *volume);
+/* Reset: every voxel back to the initial state (the reference empties the grid instead).  Asynchronous. */
+int cphb_tsdf_reset(cphb_tsdf *volume, void *stream);
+/* borrowed device planes: tw [res^3][2] float32 (tsdf, weight), col [planes][res^3] float32 (NULL for NoColor) */
+int cphb_tsdf_data(const cphb_tsdf *volume, float **tw, float **col);
+/* Integrate(RGBDImage, intrinsic, extrinsic) (uniform_tsdfvolume.cu:670-701, integrate_functor.h:84-139).  depth:
+ * 1-channel float32 metres; color: uint8 RGB for RGB8, 1-channel float32 for Gray32, unread (may be NULL) for
+ * NoColor.  The reference's format checks -- and the depth and colour sizes against the intrinsic's width x height --
+ * fail with CPHB_ERR_INVALID.  Asynchronous. */
+int cphb_tsdf_integrate(cphb_tsdf *volume, const float *depth, int depth_width, int depth_height, int depth_channels,
+                        int depth_bytes_per_channel, const void *color, int color_width, int color_height, int color_channels,
+                        int color_bytes_per_channel, int width, int height, const float h_intrinsic[9], const float h_extrinsic[16],
+                        void *stream);
+/* ExtractPointCloud (uniform_tsdfvolume.cu:85-156, 703-737): one row per zero crossing between interior band voxels,
+ * in (x, y, z, axis) order; points, normals and (unless NoColor) colours [count][3].  *h_count = the number of rows;
+ * they are written only when capacity >= it (capacity 0 sizes).  Synchronises. */
+int cphb_tsdf_extract_points(const cphb_tsdf *volume, float *points, float *normals, float *colors, size_t capacity, size_t *h_count,
+                             void *stream);
+/* ExtractVoxelPointCloud / ExtractVoxelGrid (uniform_tsdfvolume.cu:352-408, 840-895): the band voxels in index order;
+ * keys [count][3] int32 grid indices and points [count][3] voxel centres (either may be NULL), colours
+ * [count][3] = (tsdf + 1) / 2.  Sizing as cphb_tsdf_extract_points.  Synchronises. */
+int cphb_tsdf_extract_voxels(const cphb_tsdf *volume, int32_t *keys, float *points, float *colors, size_t capacity, size_t *h_count,
+                             void *stream);
+/* Raycast(intrinsic, extrinsic, sdf_trunc, project_valid_depth_only) (uniform_tsdfvolume.cu:509-639, 924-951): one ray
+ * per pixel of the width x height image, entering the grid where the ray meets the box of cells [0, res - 1).  Points, normals and colours
+ * [rows][3]; capacity must be >= width * height.  project_valid_depth_only: only the hit rows, in pixel order; otherwise
+ * every pixel's row, NaN for a miss.  *h_count = rows written.  sdf_trunc not positive and finite: CPHB_ERR_INVALID.
+ * Synchronises. */
+int cphb_tsdf_raycast(const cphb_tsdf *volume, int width, int height, const float h_intrinsic[9], const float h_extrinsic[16],
+                      float sdf_trunc, int project_valid_depth_only, float *points, float *normals, float *colors, size_t capacity,
+                      size_t *h_count, void *stream);
+
+/* ------------------------------------------------------------------------ *
  * collision::ComputeIntersection (collision.h:36-160, collision.cu:1137-1231)
  * between VoxelGrids, OccupancyGrids and primitives.  Every grid element is an
  * integer key k with the box [k * vs + origin, (k + 1) * vs + origin]: a

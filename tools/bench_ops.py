@@ -44,7 +44,12 @@ def main():
     ap.add_argument("--collision", action="store_true",
                     help="instead: time collision::ComputeIntersection on the config-3 VoxelGrid, a 512^3 OccupancyGrid and "
                          "1 / 1e4 primitives")
+    ap.add_argument("--tsdf", action="store_true",
+                    help="instead: time UniformTSDFVolume Integrate of a 640x480 frame at 256^3 and 512^3 per colour type, "
+                         "both extractions and a 640x480 Raycast")
     args = ap.parse_args()
+    if args.tsdf:
+        return tsdf(args.reps, args.out)
     if args.collision:
         return collision(args.reps, args.out)
     if args.voxelgrid:
@@ -930,6 +935,105 @@ def voxelgrid(reps, out=None):
     obj = {"op": "VoxelGrid operations: dense grids, carving, CheckIfIncluded and += on the config-3 cloud voxelised at "
                  "0.02, CreateFromOccupancyGrid on a 512^3 grid after a 1 M-point scan (%d occupied cells)" % n_occ,
            "gpu": gpu, "reps": reps, "rows": rows}
+    line = json.dumps(obj)
+    print(line)
+    if out:
+        with open(out, "w") as f:
+            f.write(line + "\n")
+
+
+def tsdf_integrate_bytes(updated, planes, w, h, color_bytes):
+    """least HBM traffic of one Integrate: each updated voxel reads and writes its 8-byte {tsdf, weight} pair and 8 bytes
+    per colour plane; the depth image (4 bytes a pixel) and the colour image are read once.  A voxel that projects
+    outside the image or behind the truncation touches no voxel memory, so it is not counted."""
+    return updated * (16 + 8 * planes) + 4 * w * h + color_bytes * w * h
+
+
+def tsdf(reps, out=None):
+    """UniformTSDFVolume(2.0, res, 0.04) with res = 256 and 512 and each colour type: Integrate of one 640 x 480 frame of a
+    sphere of radius 0.6 seen from 2.5 (repeated into the same volume), then ExtractPointCloud, ExtractVoxelPointCloud and
+    a 640 x 480 Raycast after 8 views.  CUDA-event median and minimum of `reps` calls after a warm-up call (the Python
+    call, with its synchronise), the kernel times of one further call from torch.profiler, and the Integrate bytes model
+    over the kernel time against 3.35 TB/s."""
+    import subprocess
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    import cupoch_b200 as cph
+    from cupoch_b200 import _lib
+    from cupoch_b200.testing.datagen import ring_cameras, sphere_depth
+    L = _lib.lib()
+    G, I = cph.geometry, cph.integration
+    gpu = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                         capture_output=True, text=True).stdout.strip()
+    ev = [L.cphb_event_create() for _ in range(2)]
+
+    def timed(fn):
+        times = []
+        for r in range(reps + 1):
+            L.cphb_event_record(ev[0], None)
+            fn()
+            L.cphb_event_record(ev[1], None)
+            ms = C.c_float(0)
+            _lib.check(L.cphb_event_elapsed_ms(ev[0], ev[1], C.byref(ms)))
+            if r:
+                times.append(ms.value)
+        return times
+
+    def kernels(fn):
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            fn()
+            torch.cuda.synchronize()
+        k = {}
+        for e in prof.key_averages():
+            t = getattr(e, "device_time_total", getattr(e, "cuda_time_total", 0.0)) * 1e-3
+            if t > 0 and "Memset" not in e.key and "Memcpy" not in e.key:
+                k[e.key[:60]] = k.get(e.key[:60], 0.0) + t
+        return k
+
+    w, h = 640, 480
+    cams = ring_cameras(8, w, h)
+    rng = np.random.default_rng(2)
+    frames = []
+    for K, E in cams:
+        d16 = np.round(sphere_depth(K, E, w, h, 0.6) * 1000).astype(np.uint16)
+        frames.append((K, E, d16, rng.integers(0, 256, (h, w, 3), dtype=np.uint8)))
+    CT = I.TSDFVolumeColorType
+    rows = []
+    for res in (256, 512):
+        for ct in (CT.NoColor, CT.RGB8, CT.Gray32):
+            K, E, d16, col = frames[0]
+            intr = cph.camera.PinholeCameraIntrinsic(w, h, K[0, 0], K[1, 1], K[0, 2], K[1, 2])
+            im = G.RGBDImage.create_from_color_and_depth(G.Image(col), G.Image(d16), 1000.0, 100.0, ct == CT.Gray32)
+            vol = I.UniformTSDFVolume(2.0, res, 0.04, ct)
+            vol.integrate(im, intr, E)
+            updated = int(np.count_nonzero(vol.planes()[0].cpu()[:, 1]))
+            ts = timed(lambda: vol.integrate(im, intr, E))
+            k = kernels(lambda: vol.integrate(im, intr, E))
+            kern = sum(v for n, v in k.items() if "integrate" in n)
+            planes = {CT.NoColor: 0, CT.RGB8: 3, CT.Gray32: 1}[ct]
+            nbytes = tsdf_integrate_bytes(updated, planes, w, h, {CT.NoColor: 0, CT.RGB8: 3, CT.Gray32: 4}[ct])
+            rows.append({"op": "Integrate 640x480", "res": res, "color_type": ct.name, "updated_voxels": updated,
+                         "call_ms_median": float(np.median(ts)), "call_ms_min": float(np.min(ts)), "kernel_ms_profiled": k,
+                         "integrate_kernel_ms": kern, "bytes_model": nbytes,
+                         "share_of_3.35TBps_over_kernel_time": nbytes / (kern * 1e-3) / HBM_BYTES_PER_S if kern else None})
+            del vol
+        vol = I.UniformTSDFVolume(2.0, res, 0.04, CT.RGB8)
+        for K, E, d16, col in frames:
+            intr = cph.camera.PinholeCameraIntrinsic(w, h, K[0, 0], K[1, 1], K[0, 2], K[1, 2])
+            vol.integrate(G.RGBDImage.create_from_color_and_depth(G.Image(col), G.Image(d16), 1000.0, 100.0, False), intr, E)
+        K, E = frames[0][:2]
+        intr = cph.camera.PinholeCameraIntrinsic(w, h, K[0, 0], K[1, 1], K[0, 2], K[1, 2])
+        for name, fn, count in (("ExtractPointCloud", vol.extract_point_cloud, lambda r: len(r)),
+                                ("ExtractVoxelPointCloud", vol.extract_voxel_point_cloud, lambda r: len(r)),
+                                ("Raycast 640x480", lambda: vol.raycast(intr, E, 0.04), lambda r: len(r))):
+            n_out = count(fn())
+            ts = timed(fn)
+            k = kernels(fn)
+            rows.append({"op": name, "res": res, "color_type": "RGB8", "rows": n_out, "call_ms_median": float(np.median(ts)),
+                         "call_ms_min": float(np.min(ts)), "kernel_ms_profiled": k, "kernel_ms_sum": float(sum(k.values()))})
+        del vol
+    obj = {"op": "UniformTSDFVolume(2.0, res, 0.04): 640x480 sphere frames (radius 0.6, cameras at 2.5); extractions and "
+                 "Raycast after 8 views", "gpu": gpu, "reps": reps, "rows": rows}
     line = json.dumps(obj)
     print(line)
     if out:

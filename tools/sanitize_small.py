@@ -47,3 +47,12 @@ small.normals = tn[:4000]
 print("fpfh", R.compute_fpfh_feature(small, G.KDTreeSearchParamKNN(10)).cpu().shape, "dbscan clusters", int(small.cluster_dbscan(0.02, 5).cpu().max()) + 1)
 out, idx = small.remove_radius_outlier(4, 0.02)
 print("radius outlier kept", len(out), "gaussian", len(small.gaussian_filter(0.02, 1e-4, 20)))
+from cupoch_b200.testing.datagen import ring_cameras, sphere_depth
+vol = cph.integration.UniformTSDFVolume(2.0, 48, 0.08, cph.integration.TSDFVolumeColorType.RGB8)
+for K, E in ring_cameras(3, 64, 48):
+    d16 = (sphere_depth(K, E, 64, 48, 0.6) * 1000).astype(np.uint16)
+    im = G.RGBDImage.create_from_color_and_depth(G.Image(np.full((48, 64, 3), 90, np.uint8)), G.Image(d16), convert_rgb_to_intensity=False)
+    intr = cph.camera.PinholeCameraIntrinsic(64, 48, K[0, 0], K[1, 1], K[0, 2], K[1, 2])
+    vol.integrate(im, intr, E)
+print("tsdf points", len(vol.extract_point_cloud()), "voxels", len(vol.extract_voxel_grid()),
+      "raycast", len(vol.raycast(intr, E, 0.08)), len(vol.raycast(intr, E, 0.08, False)))

@@ -5,7 +5,7 @@
             cph.registration.TransformationEstimationPointToPlane())
 
 Mirrors `import cupoch as cph` for: cph.geometry.{PointCloud, KDTreeFlann, KDTreeSearchParamKNN,
-KDTreeSearchParamRadius, VoxelGrid, OccupancyGrid, OccupancyVoxel, DistanceTransform, DistanceVoxel, Image, RGBDImage,
+KDTreeSearchParamRadius, VoxelGrid, OccupancyGrid, OccupancyVoxel, DistanceTransform, DistanceVoxel, Image, RGBDImage, TriangleMesh,
 keypoint.compute_iss_keypoints},
 cph.camera.{PinholeCameraIntrinsic, PinholeCameraIntrinsicParameters, PinholeCameraParameters},
 cph.integration.{UniformTSDFVolume, TSDFVolumeColorType},

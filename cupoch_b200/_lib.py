@@ -109,6 +109,9 @@ _SIGNATURES = {
     "cphb_tsdf_extract_voxels": (C.c_int, [_P, _P, _P, _P, C.c_size_t, C.POINTER(C.c_size_t), _P]),
     "cphb_tsdf_raycast": (C.c_int, [_P, C.c_int, C.c_int, _F3, _F3, C.c_float, C.c_int, _P, _P, _P, C.c_size_t,
                                     C.POINTER(C.c_size_t), _P]),
+    "cphb_tsdf_extract_mesh": (C.c_int, [_P, _P, _P, _P, C.c_size_t, C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t), _P]),
+    "cphb_mesh_triangle_normals": (C.c_int, [_P, C.c_size_t, _P, C.c_size_t, C.c_int, _P, _P]),
+    "cphb_mesh_vertex_normals": (C.c_int, [_P, C.c_size_t, _P, C.c_size_t, C.c_int, _P, _P]),
     # name: (restype, argtypes)
     "cphb_version": (C.c_int, []),
     "cphb_last_error": (C.c_char_p, []),

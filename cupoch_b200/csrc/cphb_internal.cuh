@@ -326,6 +326,17 @@ __device__ __forceinline__ float dist2(float qx, float qy, float qz, float px, f
 __device__ __forceinline__ float dot3(float a0, float a1, float a2, float b0, float b1, float b2) {
     return __fmaf_rn(a2, b2, __fmaf_rn(a1, b1, __fmul_rn(a0, b0)));
 }
+// NormalizeNormals' rule (Eigen's normalize()): n / sqrt(dot3(n, n)) when dot3(n, n) > 0, else n unchanged; IEEE sqrt
+// and division.  -> whether n was divided.  Shared by cphb_normalize_normals (crop.cu) and the mesh normals (mesh.cu).
+__device__ __forceinline__ bool cphb_normalize3(float n[3]) {
+    const float n2 = dot3(n[0], n[1], n[2], n[0], n[1], n[2]);
+    if (!(n2 > 0.f)) return false;
+    const float l = __fsqrt_rn(n2);
+    n[0] = __fdiv_rn(n[0], l);
+    n[1] = __fdiv_rn(n[1], l);
+    n[2] = __fdiv_rn(n[2], l);
+    return true;
+}
 __device__ __forceinline__ float det2(float a, float b, float c, float d) {
     return __fmaf_rn(a, b, -__fmul_rn(c, d));
 }

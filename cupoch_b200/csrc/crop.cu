@@ -307,13 +307,11 @@ extern "C" int cphb_uniform_down_sample(const float *points, const float *normal
 __global__ void __launch_bounds__(256) normalize_normals_kernel(float *nrm, size_t n) {
     const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const float x = nrm[3 * i], y = nrm[3 * i + 1], z = nrm[3 * i + 2];
-    const float n2 = dot3(x, y, z, x, y, z);
-    if (!(n2 > 0.f)) return;
-    const float l = __fsqrt_rn(n2);
-    nrm[3 * i] = __fdiv_rn(x, l);
-    nrm[3 * i + 1] = __fdiv_rn(y, l);
-    nrm[3 * i + 2] = __fdiv_rn(z, l);
+    float v[3] = {nrm[3 * i], nrm[3 * i + 1], nrm[3 * i + 2]};
+    if (!cphb_normalize3(v)) return;
+    nrm[3 * i] = v[0];
+    nrm[3 * i + 1] = v[1];
+    nrm[3 * i + 2] = v[2];
 }
 
 // align_normals_direction_functor (estimate_normals.cu:66-78): a zero normal becomes the reference, one pointing away

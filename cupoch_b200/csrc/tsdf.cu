@@ -463,6 +463,487 @@ extern "C" int cphb_tsdf_extract_voxels(const cphb_tsdf *v, int32_t *keys, float
     return rc;
 }
 
+// ------------------------------------------------------------------------------------------------ ExtractTriangleMesh
+// Welded marching cubes (DESIGN section 4 item 19).  The tables are printed by tools/gen_mc_tables.py, whose docstring
+// states the rule; oracle/tsdf_mesh.c carries the same text.
+#define MC_TABLE static __device__ const
+/* BEGIN tables printed by tools/gen_mc_tables.py */
+#define MC_MAX_TRIS 5 /* the most triangles any configuration produces */
+/* corner i of a cube: its voxel offset */
+MC_TABLE int8_t mc_corner[8][3] = {{0, 0, 0}, {1, 0, 0}, {1, 1, 0}, {0, 1, 0}, {0, 0, 1}, {1, 0, 1}, {1, 1, 1}, {0, 1, 1}};
+/* edge e: origin corner offset and axis */
+MC_TABLE int8_t mc_edge[12][4] = {{0, 0, 0, 0}, {1, 0, 0, 1}, {0, 1, 0, 0}, {0, 0, 0, 1}, {0, 0, 1, 0}, {1, 0, 1, 1}, {0, 1, 1, 0}, {0, 0, 1, 1}, {0, 0, 0, 2}, {1, 0, 0, 2}, {1, 1, 0, 2}, {0, 1, 0, 2}};
+/* bit e: edge e is crossed */
+MC_TABLE uint16_t mc_edge_table[256] = {
+    0x000, 0x109, 0x203, 0x30a, 0x406, 0x50f, 0x605, 0x70c, 0x80c, 0x905, 0xa0f, 0xb06, 0xc0a, 0xd03, 0xe09, 0xf00,
+    0x190, 0x099, 0x393, 0x29a, 0x596, 0x49f, 0x795, 0x69c, 0x99c, 0x895, 0xb9f, 0xa96, 0xd9a, 0xc93, 0xf99, 0xe90,
+    0x230, 0x339, 0x033, 0x13a, 0x636, 0x73f, 0x435, 0x53c, 0xa3c, 0xb35, 0x83f, 0x936, 0xe3a, 0xf33, 0xc39, 0xd30,
+    0x3a0, 0x2a9, 0x1a3, 0x0aa, 0x7a6, 0x6af, 0x5a5, 0x4ac, 0xbac, 0xaa5, 0x9af, 0x8a6, 0xfaa, 0xea3, 0xda9, 0xca0,
+    0x460, 0x569, 0x663, 0x76a, 0x066, 0x16f, 0x265, 0x36c, 0xc6c, 0xd65, 0xe6f, 0xf66, 0x86a, 0x963, 0xa69, 0xb60,
+    0x5f0, 0x4f9, 0x7f3, 0x6fa, 0x1f6, 0x0ff, 0x3f5, 0x2fc, 0xdfc, 0xcf5, 0xfff, 0xef6, 0x9fa, 0x8f3, 0xbf9, 0xaf0,
+    0x650, 0x759, 0x453, 0x55a, 0x256, 0x35f, 0x055, 0x15c, 0xe5c, 0xf55, 0xc5f, 0xd56, 0xa5a, 0xb53, 0x859, 0x950,
+    0x7c0, 0x6c9, 0x5c3, 0x4ca, 0x3c6, 0x2cf, 0x1c5, 0x0cc, 0xfcc, 0xec5, 0xdcf, 0xcc6, 0xbca, 0xac3, 0x9c9, 0x8c0,
+    0x8c0, 0x9c9, 0xac3, 0xbca, 0xcc6, 0xdcf, 0xec5, 0xfcc, 0x0cc, 0x1c5, 0x2cf, 0x3c6, 0x4ca, 0x5c3, 0x6c9, 0x7c0,
+    0x950, 0x859, 0xb53, 0xa5a, 0xd56, 0xc5f, 0xf55, 0xe5c, 0x15c, 0x055, 0x35f, 0x256, 0x55a, 0x453, 0x759, 0x650,
+    0xaf0, 0xbf9, 0x8f3, 0x9fa, 0xef6, 0xfff, 0xcf5, 0xdfc, 0x2fc, 0x3f5, 0x0ff, 0x1f6, 0x6fa, 0x7f3, 0x4f9, 0x5f0,
+    0xb60, 0xa69, 0x963, 0x86a, 0xf66, 0xe6f, 0xd65, 0xc6c, 0x36c, 0x265, 0x16f, 0x066, 0x76a, 0x663, 0x569, 0x460,
+    0xca0, 0xda9, 0xea3, 0xfaa, 0x8a6, 0x9af, 0xaa5, 0xbac, 0x4ac, 0x5a5, 0x6af, 0x7a6, 0x0aa, 0x1a3, 0x2a9, 0x3a0,
+    0xd30, 0xc39, 0xf33, 0xe3a, 0x936, 0x83f, 0xb35, 0xa3c, 0x53c, 0x435, 0x73f, 0x636, 0x13a, 0x033, 0x339, 0x230,
+    0xe90, 0xf99, 0xc93, 0xd9a, 0xa96, 0xb9f, 0x895, 0x99c, 0x69c, 0x795, 0x49f, 0x596, 0x29a, 0x393, 0x099, 0x190,
+    0xf00, 0xe09, 0xd03, 0xc0a, 0xb06, 0xa0f, 0x905, 0x80c, 0x70c, 0x605, 0x50f, 0x406, 0x30a, 0x203, 0x109, 0x000,
+};
+MC_TABLE uint8_t mc_tri_count[256] = {
+    0, 1, 1, 2, 1, 2, 2, 3, 1, 2, 2, 3, 2, 3, 3, 2, 1, 2, 2, 3, 2, 3, 3, 4, 2, 3, 3, 4, 3, 4, 4, 3,
+    1, 2, 2, 3, 2, 3, 3, 4, 2, 3, 3, 4, 3, 4, 4, 3, 2, 3, 3, 2, 3, 4, 4, 3, 3, 4, 4, 3, 4, 5, 5, 2,
+    1, 2, 2, 3, 2, 3, 3, 4, 2, 3, 3, 4, 3, 4, 4, 3, 2, 3, 3, 4, 3, 4, 4, 5, 3, 4, 4, 5, 4, 5, 5, 4,
+    2, 3, 3, 4, 3, 4, 2, 3, 3, 4, 4, 5, 4, 5, 3, 2, 3, 4, 4, 3, 4, 5, 3, 2, 4, 5, 5, 4, 5, 2, 4, 1,
+    1, 2, 2, 3, 2, 3, 3, 4, 2, 3, 3, 4, 3, 4, 4, 3, 2, 3, 3, 4, 3, 4, 4, 5, 3, 2, 4, 3, 4, 3, 5, 2,
+    2, 3, 3, 4, 3, 4, 4, 5, 3, 4, 4, 5, 4, 5, 5, 4, 3, 4, 4, 3, 4, 5, 5, 4, 4, 3, 5, 2, 5, 4, 2, 1,
+    2, 3, 3, 4, 3, 4, 4, 5, 3, 4, 4, 5, 2, 3, 3, 2, 3, 4, 4, 5, 4, 5, 5, 2, 4, 3, 5, 4, 3, 2, 4, 1,
+    3, 4, 4, 5, 4, 5, 3, 4, 4, 5, 5, 2, 3, 4, 2, 1, 2, 3, 3, 2, 3, 4, 2, 1, 3, 2, 4, 1, 2, 1, 1, 0,
+};
+/* the edges of each triangle, -1 past mc_tri_count */
+MC_TABLE int8_t mc_tri_table[256][3 * MC_MAX_TRIS] = {
+    {-1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {0, 3, 8, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {0, 9, 1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {1, 3, 8, 1, 8, 9, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {1, 10, 2, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {0, 3, 8, 1, 10, 2, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {0, 9, 10, 0, 10, 2, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {2, 3, 8, 2, 8, 9, 2, 9, 10, -1, -1, -1, -1, -1, -1},
+    {2, 11, 3, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {0, 2, 11, 0, 11, 8, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {0, 9, 1, 2, 11, 3, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {1, 2, 11, 1, 11, 8, 1, 8, 9, -1, -1, -1, -1, -1, -1},
+    {1, 10, 11, 1, 11, 3, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {0, 1, 10, 0, 10, 11, 0, 11, 8, -1, -1, -1, -1, -1, -1},
+    {0, 9, 10, 0, 10, 11, 0, 11, 3, -1, -1, -1, -1, -1, -1},
+    {8, 9, 10, 8, 10, 11, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {4, 8, 7, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {0, 3, 7, 0, 7, 4, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {0, 9, 1, 4, 8, 7, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {1, 3, 7, 1, 7, 4, 1, 4, 9, -1, -1, -1, -1, -1, -1},
+    {1, 10, 2, 4, 8, 7, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {0, 3, 7, 0, 7, 4, 1, 10, 2, -1, -1, -1, -1, -1, -1},
+    {0, 9, 10, 0, 10, 2, 4, 8, 7, -1, -1, -1, -1, -1, -1},
+    {2, 3, 7, 2, 7, 4, 2, 4, 9, 2, 9, 10, -1, -1, -1},
+    {2, 11, 3, 4, 8, 7, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {0, 2, 11, 0, 11, 7, 0, 7, 4, -1, -1, -1, -1, -1, -1},
+    {0, 9, 1, 2, 11, 3, 4, 8, 7, -1, -1, -1, -1, -1, -1},
+    {1, 2, 11, 1, 11, 7, 1, 7, 4, 1, 4, 9, -1, -1, -1},
+    {1, 10, 11, 1, 11, 3, 4, 8, 7, -1, -1, -1, -1, -1, -1},
+    {0, 1, 10, 0, 10, 11, 0, 11, 7, 0, 7, 4, -1, -1, -1},
+    {0, 9, 10, 0, 10, 11, 0, 11, 3, 4, 8, 7, -1, -1, -1},
+    {4, 9, 10, 4, 10, 11, 4, 11, 7, -1, -1, -1, -1, -1, -1},
+    {4, 5, 9, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {0, 3, 8, 4, 5, 9, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {0, 4, 5, 0, 5, 1, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {1, 3, 8, 1, 8, 4, 1, 4, 5, -1, -1, -1, -1, -1, -1},
+    {1, 10, 2, 4, 5, 9, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {0, 3, 8, 1, 10, 2, 4, 5, 9, -1, -1, -1, -1, -1, -1},
+    {0, 4, 5, 0, 5, 10, 0, 10, 2, -1, -1, -1, -1, -1, -1},
+    {2, 3, 8, 2, 8, 4, 2, 4, 5, 2, 5, 10, -1, -1, -1},
+    {2, 11, 3, 4, 5, 9, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {0, 2, 11, 0, 11, 8, 4, 5, 9, -1, -1, -1, -1, -1, -1},
+    {0, 4, 5, 0, 5, 1, 2, 11, 3, -1, -1, -1, -1, -1, -1},
+    {1, 2, 11, 1, 11, 8, 1, 8, 4, 1, 4, 5, -1, -1, -1},
+    {1, 10, 11, 1, 11, 3, 4, 5, 9, -1, -1, -1, -1, -1, -1},
+    {0, 1, 10, 0, 10, 11, 0, 11, 8, 4, 5, 9, -1, -1, -1},
+    {0, 4, 5, 0, 5, 10, 0, 10, 11, 0, 11, 3, -1, -1, -1},
+    {4, 5, 10, 4, 10, 11, 4, 11, 8, -1, -1, -1, -1, -1, -1},
+    {5, 9, 8, 5, 8, 7, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {0, 3, 7, 0, 7, 5, 0, 5, 9, -1, -1, -1, -1, -1, -1},
+    {0, 8, 7, 0, 7, 5, 0, 5, 1, -1, -1, -1, -1, -1, -1},
+    {1, 3, 7, 1, 7, 5, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {1, 10, 2, 5, 9, 8, 5, 8, 7, -1, -1, -1, -1, -1, -1},
+    {0, 3, 7, 0, 7, 5, 0, 5, 9, 1, 10, 2, -1, -1, -1},
+    {0, 8, 7, 0, 7, 5, 0, 5, 10, 0, 10, 2, -1, -1, -1},
+    {2, 3, 7, 2, 7, 5, 2, 5, 10, -1, -1, -1, -1, -1, -1},
+    {2, 11, 3, 5, 9, 8, 5, 8, 7, -1, -1, -1, -1, -1, -1},
+    {0, 2, 11, 0, 11, 7, 0, 7, 5, 0, 5, 9, -1, -1, -1},
+    {0, 8, 7, 0, 7, 5, 0, 5, 1, 2, 11, 3, -1, -1, -1},
+    {1, 2, 11, 1, 11, 7, 1, 7, 5, -1, -1, -1, -1, -1, -1},
+    {1, 10, 11, 1, 11, 3, 5, 9, 8, 5, 8, 7, -1, -1, -1},
+    {0, 1, 10, 0, 10, 11, 0, 11, 7, 0, 7, 5, 0, 5, 9},
+    {0, 8, 7, 0, 7, 5, 0, 5, 10, 0, 10, 11, 0, 11, 3},
+    {5, 10, 11, 5, 11, 7, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {5, 6, 10, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {0, 3, 8, 5, 6, 10, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {0, 9, 1, 5, 6, 10, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {1, 3, 8, 1, 8, 9, 5, 6, 10, -1, -1, -1, -1, -1, -1},
+    {1, 5, 6, 1, 6, 2, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {0, 3, 8, 1, 5, 6, 1, 6, 2, -1, -1, -1, -1, -1, -1},
+    {0, 9, 5, 0, 5, 6, 0, 6, 2, -1, -1, -1, -1, -1, -1},
+    {2, 3, 8, 2, 8, 9, 2, 9, 5, 2, 5, 6, -1, -1, -1},
+    {2, 11, 3, 5, 6, 10, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {0, 2, 11, 0, 11, 8, 5, 6, 10, -1, -1, -1, -1, -1, -1},
+    {0, 9, 1, 2, 11, 3, 5, 6, 10, -1, -1, -1, -1, -1, -1},
+    {1, 2, 11, 1, 11, 8, 1, 8, 9, 5, 6, 10, -1, -1, -1},
+    {1, 5, 6, 1, 6, 11, 1, 11, 3, -1, -1, -1, -1, -1, -1},
+    {0, 1, 5, 0, 5, 6, 0, 6, 11, 0, 11, 8, -1, -1, -1},
+    {0, 9, 5, 0, 5, 6, 0, 6, 11, 0, 11, 3, -1, -1, -1},
+    {5, 6, 11, 5, 11, 8, 5, 8, 9, -1, -1, -1, -1, -1, -1},
+    {4, 8, 7, 5, 6, 10, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {0, 3, 7, 0, 7, 4, 5, 6, 10, -1, -1, -1, -1, -1, -1},
+    {0, 9, 1, 4, 8, 7, 5, 6, 10, -1, -1, -1, -1, -1, -1},
+    {1, 3, 7, 1, 7, 4, 1, 4, 9, 5, 6, 10, -1, -1, -1},
+    {1, 5, 6, 1, 6, 2, 4, 8, 7, -1, -1, -1, -1, -1, -1},
+    {0, 3, 7, 0, 7, 4, 1, 5, 6, 1, 6, 2, -1, -1, -1},
+    {0, 9, 5, 0, 5, 6, 0, 6, 2, 4, 8, 7, -1, -1, -1},
+    {2, 3, 7, 2, 7, 4, 2, 4, 9, 2, 9, 5, 2, 5, 6},
+    {2, 11, 3, 4, 8, 7, 5, 6, 10, -1, -1, -1, -1, -1, -1},
+    {0, 2, 11, 0, 11, 7, 0, 7, 4, 5, 6, 10, -1, -1, -1},
+    {0, 9, 1, 2, 11, 3, 4, 8, 7, 5, 6, 10, -1, -1, -1},
+    {1, 2, 11, 1, 11, 7, 1, 7, 4, 1, 4, 9, 5, 6, 10},
+    {1, 5, 6, 1, 6, 11, 1, 11, 3, 4, 8, 7, -1, -1, -1},
+    {0, 1, 5, 0, 5, 6, 0, 6, 11, 0, 11, 7, 0, 7, 4},
+    {0, 9, 5, 0, 5, 6, 0, 6, 11, 0, 11, 3, 4, 8, 7},
+    {9, 5, 6, 9, 6, 11, 9, 11, 7, 9, 7, 4, -1, -1, -1},
+    {4, 6, 10, 4, 10, 9, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {0, 3, 8, 4, 6, 10, 4, 10, 9, -1, -1, -1, -1, -1, -1},
+    {0, 4, 6, 0, 6, 10, 0, 10, 1, -1, -1, -1, -1, -1, -1},
+    {1, 3, 8, 1, 8, 4, 1, 4, 6, 1, 6, 10, -1, -1, -1},
+    {1, 9, 4, 1, 4, 6, 1, 6, 2, -1, -1, -1, -1, -1, -1},
+    {0, 3, 8, 1, 9, 4, 1, 4, 6, 1, 6, 2, -1, -1, -1},
+    {0, 4, 6, 0, 6, 2, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {2, 3, 8, 2, 8, 4, 2, 4, 6, -1, -1, -1, -1, -1, -1},
+    {2, 11, 3, 4, 6, 10, 4, 10, 9, -1, -1, -1, -1, -1, -1},
+    {0, 2, 11, 0, 11, 8, 4, 6, 10, 4, 10, 9, -1, -1, -1},
+    {0, 4, 6, 0, 6, 10, 0, 10, 1, 2, 11, 3, -1, -1, -1},
+    {1, 2, 11, 1, 11, 8, 1, 8, 4, 1, 4, 6, 1, 6, 10},
+    {1, 9, 4, 1, 4, 6, 1, 6, 11, 1, 11, 3, -1, -1, -1},
+    {1, 9, 4, 1, 4, 6, 1, 6, 11, 1, 11, 8, 1, 8, 0},
+    {0, 4, 6, 0, 6, 11, 0, 11, 3, -1, -1, -1, -1, -1, -1},
+    {4, 6, 11, 4, 11, 8, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {6, 10, 9, 6, 9, 8, 6, 8, 7, -1, -1, -1, -1, -1, -1},
+    {0, 3, 7, 0, 7, 6, 0, 6, 10, 0, 10, 9, -1, -1, -1},
+    {0, 8, 7, 0, 7, 6, 0, 6, 10, 0, 10, 1, -1, -1, -1},
+    {1, 3, 7, 1, 7, 6, 1, 6, 10, -1, -1, -1, -1, -1, -1},
+    {1, 9, 8, 1, 8, 7, 1, 7, 6, 1, 6, 2, -1, -1, -1},
+    {7, 6, 2, 7, 2, 1, 7, 1, 9, 7, 9, 0, 7, 0, 3},
+    {0, 8, 7, 0, 7, 6, 0, 6, 2, -1, -1, -1, -1, -1, -1},
+    {2, 3, 7, 2, 7, 6, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {2, 11, 3, 6, 10, 9, 6, 9, 8, 6, 8, 7, -1, -1, -1},
+    {0, 2, 11, 0, 11, 7, 0, 7, 6, 0, 6, 10, 0, 10, 9},
+    {0, 8, 7, 0, 7, 6, 0, 6, 10, 0, 10, 1, 2, 11, 3},
+    {1, 2, 11, 1, 11, 7, 1, 7, 6, 1, 6, 10, -1, -1, -1},
+    {1, 9, 8, 1, 8, 7, 1, 7, 6, 1, 6, 11, 1, 11, 3},
+    {0, 1, 9, 6, 11, 7, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {0, 8, 7, 0, 7, 6, 0, 6, 11, 0, 11, 3, -1, -1, -1},
+    {6, 11, 7, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {6, 7, 11, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {0, 3, 8, 6, 7, 11, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {0, 9, 1, 6, 7, 11, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {1, 3, 8, 1, 8, 9, 6, 7, 11, -1, -1, -1, -1, -1, -1},
+    {1, 10, 2, 6, 7, 11, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {0, 3, 8, 1, 10, 2, 6, 7, 11, -1, -1, -1, -1, -1, -1},
+    {0, 9, 10, 0, 10, 2, 6, 7, 11, -1, -1, -1, -1, -1, -1},
+    {2, 3, 8, 2, 8, 9, 2, 9, 10, 6, 7, 11, -1, -1, -1},
+    {2, 6, 7, 2, 7, 3, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {0, 2, 6, 0, 6, 7, 0, 7, 8, -1, -1, -1, -1, -1, -1},
+    {0, 9, 1, 2, 6, 7, 2, 7, 3, -1, -1, -1, -1, -1, -1},
+    {1, 2, 6, 1, 6, 7, 1, 7, 8, 1, 8, 9, -1, -1, -1},
+    {1, 10, 6, 1, 6, 7, 1, 7, 3, -1, -1, -1, -1, -1, -1},
+    {0, 1, 10, 0, 10, 6, 0, 6, 7, 0, 7, 8, -1, -1, -1},
+    {0, 9, 10, 0, 10, 6, 0, 6, 7, 0, 7, 3, -1, -1, -1},
+    {6, 7, 8, 6, 8, 9, 6, 9, 10, -1, -1, -1, -1, -1, -1},
+    {4, 8, 11, 4, 11, 6, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {0, 3, 11, 0, 11, 6, 0, 6, 4, -1, -1, -1, -1, -1, -1},
+    {0, 9, 1, 4, 8, 11, 4, 11, 6, -1, -1, -1, -1, -1, -1},
+    {1, 3, 11, 1, 11, 6, 1, 6, 4, 1, 4, 9, -1, -1, -1},
+    {1, 10, 2, 4, 8, 11, 4, 11, 6, -1, -1, -1, -1, -1, -1},
+    {0, 3, 11, 0, 11, 6, 0, 6, 4, 1, 10, 2, -1, -1, -1},
+    {0, 9, 10, 0, 10, 2, 4, 8, 11, 4, 11, 6, -1, -1, -1},
+    {3, 11, 6, 3, 6, 4, 3, 4, 9, 3, 9, 10, 3, 10, 2},
+    {2, 6, 4, 2, 4, 8, 2, 8, 3, -1, -1, -1, -1, -1, -1},
+    {0, 2, 6, 0, 6, 4, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {0, 9, 1, 2, 6, 4, 2, 4, 8, 2, 8, 3, -1, -1, -1},
+    {1, 2, 6, 1, 6, 4, 1, 4, 9, -1, -1, -1, -1, -1, -1},
+    {1, 10, 6, 1, 6, 4, 1, 4, 8, 1, 8, 3, -1, -1, -1},
+    {0, 1, 10, 0, 10, 6, 0, 6, 4, -1, -1, -1, -1, -1, -1},
+    {10, 6, 4, 10, 4, 8, 10, 8, 3, 10, 3, 0, 10, 0, 9},
+    {4, 9, 10, 4, 10, 6, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {4, 5, 9, 6, 7, 11, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {0, 3, 8, 4, 5, 9, 6, 7, 11, -1, -1, -1, -1, -1, -1},
+    {0, 4, 5, 0, 5, 1, 6, 7, 11, -1, -1, -1, -1, -1, -1},
+    {1, 3, 8, 1, 8, 4, 1, 4, 5, 6, 7, 11, -1, -1, -1},
+    {1, 10, 2, 4, 5, 9, 6, 7, 11, -1, -1, -1, -1, -1, -1},
+    {0, 3, 8, 1, 10, 2, 4, 5, 9, 6, 7, 11, -1, -1, -1},
+    {0, 4, 5, 0, 5, 10, 0, 10, 2, 6, 7, 11, -1, -1, -1},
+    {2, 3, 8, 2, 8, 4, 2, 4, 5, 2, 5, 10, 6, 7, 11},
+    {2, 6, 7, 2, 7, 3, 4, 5, 9, -1, -1, -1, -1, -1, -1},
+    {0, 2, 6, 0, 6, 7, 0, 7, 8, 4, 5, 9, -1, -1, -1},
+    {0, 4, 5, 0, 5, 1, 2, 6, 7, 2, 7, 3, -1, -1, -1},
+    {1, 2, 6, 1, 6, 7, 1, 7, 8, 1, 8, 4, 1, 4, 5},
+    {1, 10, 6, 1, 6, 7, 1, 7, 3, 4, 5, 9, -1, -1, -1},
+    {0, 1, 10, 0, 10, 6, 0, 6, 7, 0, 7, 8, 4, 5, 9},
+    {0, 4, 5, 0, 5, 10, 0, 10, 6, 0, 6, 7, 0, 7, 3},
+    {10, 6, 7, 10, 7, 8, 10, 8, 4, 10, 4, 5, -1, -1, -1},
+    {5, 9, 8, 5, 8, 11, 5, 11, 6, -1, -1, -1, -1, -1, -1},
+    {0, 3, 11, 0, 11, 6, 0, 6, 5, 0, 5, 9, -1, -1, -1},
+    {0, 8, 11, 0, 11, 6, 0, 6, 5, 0, 5, 1, -1, -1, -1},
+    {1, 3, 11, 1, 11, 6, 1, 6, 5, -1, -1, -1, -1, -1, -1},
+    {1, 10, 2, 5, 9, 8, 5, 8, 11, 5, 11, 6, -1, -1, -1},
+    {0, 3, 11, 0, 11, 6, 0, 6, 5, 0, 5, 9, 1, 10, 2},
+    {0, 8, 11, 0, 11, 6, 0, 6, 5, 0, 5, 10, 0, 10, 2},
+    {3, 11, 6, 3, 6, 5, 3, 5, 10, 3, 10, 2, -1, -1, -1},
+    {2, 6, 5, 2, 5, 9, 2, 9, 8, 2, 8, 3, -1, -1, -1},
+    {0, 2, 6, 0, 6, 5, 0, 5, 9, -1, -1, -1, -1, -1, -1},
+    {8, 3, 2, 8, 2, 6, 8, 6, 5, 8, 5, 1, 8, 1, 0},
+    {1, 2, 6, 1, 6, 5, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {6, 5, 9, 6, 9, 8, 6, 8, 3, 6, 3, 1, 6, 1, 10},
+    {0, 1, 10, 0, 10, 6, 0, 6, 5, 0, 5, 9, -1, -1, -1},
+    {0, 8, 3, 5, 10, 6, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {5, 10, 6, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {5, 7, 11, 5, 11, 10, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {0, 3, 8, 5, 7, 11, 5, 11, 10, -1, -1, -1, -1, -1, -1},
+    {0, 9, 1, 5, 7, 11, 5, 11, 10, -1, -1, -1, -1, -1, -1},
+    {1, 3, 8, 1, 8, 9, 5, 7, 11, 5, 11, 10, -1, -1, -1},
+    {1, 5, 7, 1, 7, 11, 1, 11, 2, -1, -1, -1, -1, -1, -1},
+    {0, 3, 8, 1, 5, 7, 1, 7, 11, 1, 11, 2, -1, -1, -1},
+    {0, 9, 5, 0, 5, 7, 0, 7, 11, 0, 11, 2, -1, -1, -1},
+    {2, 3, 8, 2, 8, 9, 2, 9, 5, 2, 5, 7, 2, 7, 11},
+    {2, 10, 5, 2, 5, 7, 2, 7, 3, -1, -1, -1, -1, -1, -1},
+    {0, 2, 10, 0, 10, 5, 0, 5, 7, 0, 7, 8, -1, -1, -1},
+    {0, 9, 1, 2, 10, 5, 2, 5, 7, 2, 7, 3, -1, -1, -1},
+    {2, 10, 5, 2, 5, 7, 2, 7, 8, 2, 8, 9, 2, 9, 1},
+    {1, 5, 7, 1, 7, 3, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {0, 1, 5, 0, 5, 7, 0, 7, 8, -1, -1, -1, -1, -1, -1},
+    {0, 9, 5, 0, 5, 7, 0, 7, 3, -1, -1, -1, -1, -1, -1},
+    {5, 7, 8, 5, 8, 9, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {4, 8, 11, 4, 11, 10, 4, 10, 5, -1, -1, -1, -1, -1, -1},
+    {0, 3, 11, 0, 11, 10, 0, 10, 5, 0, 5, 4, -1, -1, -1},
+    {0, 9, 1, 4, 8, 11, 4, 11, 10, 4, 10, 5, -1, -1, -1},
+    {3, 11, 10, 3, 10, 5, 3, 5, 4, 3, 4, 9, 3, 9, 1},
+    {1, 5, 4, 1, 4, 8, 1, 8, 11, 1, 11, 2, -1, -1, -1},
+    {11, 2, 1, 11, 1, 5, 11, 5, 4, 11, 4, 0, 11, 0, 3},
+    {5, 4, 8, 5, 8, 11, 5, 11, 2, 5, 2, 0, 5, 0, 9},
+    {2, 3, 11, 4, 9, 5, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {2, 10, 5, 2, 5, 4, 2, 4, 8, 2, 8, 3, -1, -1, -1},
+    {0, 2, 10, 0, 10, 5, 0, 5, 4, -1, -1, -1, -1, -1, -1},
+    {0, 9, 1, 2, 10, 5, 2, 5, 4, 2, 4, 8, 2, 8, 3},
+    {2, 10, 5, 2, 5, 4, 2, 4, 9, 2, 9, 1, -1, -1, -1},
+    {1, 5, 4, 1, 4, 8, 1, 8, 3, -1, -1, -1, -1, -1, -1},
+    {0, 1, 5, 0, 5, 4, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {5, 4, 8, 5, 8, 3, 5, 3, 0, 5, 0, 9, -1, -1, -1},
+    {4, 9, 5, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {4, 7, 11, 4, 11, 10, 4, 10, 9, -1, -1, -1, -1, -1, -1},
+    {0, 3, 8, 4, 7, 11, 4, 11, 10, 4, 10, 9, -1, -1, -1},
+    {0, 4, 7, 0, 7, 11, 0, 11, 10, 0, 10, 1, -1, -1, -1},
+    {1, 3, 8, 1, 8, 4, 1, 4, 7, 1, 7, 11, 1, 11, 10},
+    {1, 9, 4, 1, 4, 7, 1, 7, 11, 1, 11, 2, -1, -1, -1},
+    {0, 3, 8, 1, 9, 4, 1, 4, 7, 1, 7, 11, 1, 11, 2},
+    {0, 4, 7, 0, 7, 11, 0, 11, 2, -1, -1, -1, -1, -1, -1},
+    {2, 3, 8, 2, 8, 4, 2, 4, 7, 2, 7, 11, -1, -1, -1},
+    {2, 10, 9, 2, 9, 4, 2, 4, 7, 2, 7, 3, -1, -1, -1},
+    {2, 10, 9, 2, 9, 4, 2, 4, 7, 2, 7, 8, 2, 8, 0},
+    {4, 7, 3, 4, 3, 2, 4, 2, 10, 4, 10, 1, 4, 1, 0},
+    {1, 2, 10, 4, 7, 8, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {1, 9, 4, 1, 4, 7, 1, 7, 3, -1, -1, -1, -1, -1, -1},
+    {1, 9, 4, 1, 4, 7, 1, 7, 8, 1, 8, 0, -1, -1, -1},
+    {0, 4, 7, 0, 7, 3, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {4, 7, 8, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {8, 11, 10, 8, 10, 9, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {0, 3, 11, 0, 11, 10, 0, 10, 9, -1, -1, -1, -1, -1, -1},
+    {0, 8, 11, 0, 11, 10, 0, 10, 1, -1, -1, -1, -1, -1, -1},
+    {1, 3, 11, 1, 11, 10, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {1, 9, 8, 1, 8, 11, 1, 11, 2, -1, -1, -1, -1, -1, -1},
+    {11, 2, 1, 11, 1, 9, 11, 9, 0, 11, 0, 3, -1, -1, -1},
+    {0, 8, 11, 0, 11, 2, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {2, 3, 11, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {2, 10, 9, 2, 9, 8, 2, 8, 3, -1, -1, -1, -1, -1, -1},
+    {0, 2, 10, 0, 10, 9, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {8, 3, 2, 8, 2, 10, 8, 10, 1, 8, 1, 0, -1, -1, -1},
+    {1, 2, 10, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {1, 9, 8, 1, 8, 3, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {0, 1, 9, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {0, 8, 3, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+    {-1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1},
+};
+/* END tables printed by tools/gen_mc_tables.py */
+#undef MC_TABLE
+
+// cube byte at the cube's origin voxel (x, y, z), x, y, z <= res - 2: the cube index (bit i: corner i's tsdf < 0) when
+// all 8 corner weights are nonzero and the index is neither 0 nor 255, else 0 (UT:184-210 and its 0 / 255 filter)
+__global__ void __launch_bounds__(256) tsdf_mc_cube_kernel(const float2 *__restrict__ tw, int res, uint8_t *__restrict__ cb) {
+    const int z = blockIdx.x * 32 + threadIdx.x, y = blockIdx.y * 8 + threadIdx.y, x = blockIdx.z;
+    if (z >= res || y >= res) return;
+    int ci = 0;
+    bool ok = x < res - 1 && y < res - 1 && z < res - 1;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+        if (!ok) break;
+        const float2 c = tw[tsdf_idx(x + mc_corner[i][0], y + mc_corner[i][1], z + mc_corner[i][2], res)];
+        ok = c.y != 0.0f;
+        ci |= (c.x < 0.0f ? 1 : 0) << i;
+    }
+    cb[tsdf_idx(x, y, z, res)] = ok && ci != 255 ? (uint8_t)ci : 0;
+}
+
+// bit a of voxel v's mask: edge (v, a) is a vertex, i.e. it is crossed in a cube that emits.  The cube at v - d holds
+// the edge as its edge e with origin corner d and axis a, so the bit is the OR of mc_edge_table[cb[v - d]] >> e.
+__global__ void __launch_bounds__(256) tsdf_mc_edge_kernel(const uint8_t *__restrict__ cb, int res, uint8_t *__restrict__ em) {
+    const int z = blockIdx.x * 32 + threadIdx.x, y = blockIdx.y * 8 + threadIdx.y, x = blockIdx.z;
+    if (z >= res || y >= res) return;
+    uint8_t m = 0;
+#pragma unroll
+    for (int e = 0; e < 12; ++e) {
+        const int cx = x - mc_edge[e][0], cy = y - mc_edge[e][1], cz = z - mc_edge[e][2];
+        if (cx < 0 || cy < 0 || cz < 0) continue;
+        if (mc_edge_table[__ldg(cb + tsdf_idx(cx, cy, cz, res))] >> e & 1) m |= (uint8_t)(1 << mc_edge[e][3]);
+    }
+    em[tsdf_idx(x, y, z, res)] = m;
+}
+
+// vcnt[j] = popcount of compacted voxel j's edge mask, tcnt[j] = triangle count of compacted cube j; each array ends
+// with one 0, so the exclusive scans' last outputs are the totals
+__global__ void __launch_bounds__(256) tsdf_mc_count_kernel(const int32_t *__restrict__ vpos, size_t mv, const uint8_t *__restrict__ em,
+                                                            const int32_t *__restrict__ cpos, size_t mc, const uint8_t *__restrict__ cb,
+                                                            unsigned long long *__restrict__ vcnt, unsigned long long *__restrict__ tcnt) {
+    const size_t j = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+    if (j < mv) vcnt[j] = (unsigned long long)__popc(em[vpos[j]]);
+    if (j == mv) vcnt[j] = 0ull;
+    if (j < mc) tcnt[j] = (unsigned long long)mc_tri_count[cb[cpos[j]]];
+    if (j == mc) tcnt[j] = 0ull;
+}
+
+// the vertices of compacted voxel j, at rows voff[j] ...; vbase[v] = voff[j] for the triangle kernel.  The expression
+// order is oracle/tsdf_mesh.c's ExtractTriangleMesh.
+template <int CT>
+__global__ void __launch_bounds__(128) tsdf_mc_vertex_kernel(const float2 *__restrict__ tw, const float *__restrict__ col, size_t n, int res,
+                                                             float vl, float half, float hres, float ox, float oy, float oz,
+                                                             const int32_t *__restrict__ vpos, size_t mv, const uint8_t *__restrict__ em,
+                                                             const unsigned long long *__restrict__ voff, int32_t *__restrict__ vbase,
+                                                             float *__restrict__ verts, float *__restrict__ vcols) {
+    const size_t j = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+    if (j >= mv) return;
+    const size_t i0 = (size_t)vpos[j];
+    const int mask = em[i0];
+    const size_t rr = (size_t)res * res;
+    const int k[3] = {(int)(i0 / rr), (int)((i0 / res) % res), (int)(i0 % res)};
+    const size_t stride[3] = {rr, (size_t)res, 1};
+    const float o[3] = {ox, oy, oz};
+    size_t row = voff[j];
+    vbase[i0] = (int32_t)row;
+    const float f0 = fabsf(tw[i0].x);
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+        if (!(mask >> a & 1)) continue;
+        const size_t i1 = i0 + stride[a];
+        const float f1 = fabsf(tw[i1].x), fs = f0 + f1;
+        float p[3];
+#pragma unroll
+        for (int b = 0; b < 3; ++b) p[b] = __fmaf_rn(vl, (float)k[b], half);
+        p[a] = p[a] + (f0 * vl) / fs;
+#pragma unroll
+        for (int b = 0; b < 3; ++b) verts[3 * row + b] = (p[b] + o[b]) - hres;
+        if (CT == TSDF_RGB8) {
+#pragma unroll
+            for (int b = 0; b < 3; ++b) vcols[3 * row + b] = __fmaf_rn(f0, col[b * n + i1] / 255.0f, f1 * (col[b * n + i0] / 255.0f)) / fs;
+        } else if (CT == TSDF_GRAY32) {
+            const float g = __fmaf_rn(f0, col[i1], f1 * col[i0]) / fs;
+            vcols[3 * row] = vcols[3 * row + 1] = vcols[3 * row + 2] = g;
+        }
+        ++row;
+    }
+}
+
+// the triangles of compacted cube j, at rows toff[j] ...: edge e of the cube at c is vertex vbase[v] + popc(em[v] &
+// ((1 << a) - 1)), v = c + its origin corner, a = its axis
+__global__ void __launch_bounds__(128) tsdf_mc_triangle_kernel(const int32_t *__restrict__ cpos, size_t mc, const uint8_t *__restrict__ cb,
+                                                               const uint8_t *__restrict__ em, const int32_t *__restrict__ vbase, int res,
+                                                               const unsigned long long *__restrict__ toff, int32_t *__restrict__ tris) {
+    const size_t j = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+    if (j >= mc) return;
+    const size_t c = (size_t)cpos[j];
+    const int ci = cb[c];
+    const int nt = mc_tri_count[ci];
+    int32_t *out = tris + 3 * toff[j];
+    for (int t = 0; t < 3 * nt; ++t) {
+        const int e = mc_tri_table[ci][t];
+        const size_t v = c + ((size_t)mc_edge[e][0] * res + mc_edge[e][1]) * res + mc_edge[e][2];
+        out[t] = __ldg(vbase + v) + __popc(__ldg(em + v) & ((1 << mc_edge[e][3]) - 1));
+    }
+}
+
+static int tsdf_scan(const unsigned long long *cnt, unsigned long long *off, size_t n, cphb_scratch &sc, cudaStream_t s) {
+    size_t tmp_bytes = 0;
+    CPHB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, cnt, off, (int64_t)n, s));
+    char *tmp = nullptr;
+    const int rc = sc.alloc(&tmp, tmp_bytes ? tmp_bytes : 16);
+    if (rc) return rc;
+    CPHB_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, cnt, off, (int64_t)n, s));
+    g_cphb_launches += 2;  // CUB's init and scan kernels
+    return CPHB_OK;
+}
+
+extern "C" int cphb_tsdf_extract_mesh(const cphb_tsdf *v, float *vertices, float *colors, int32_t *triangles, size_t vertex_capacity,
+                                      size_t triangle_capacity, size_t *h_n_vertices, size_t *h_n_triangles, void *stream) {
+    cudaStream_t s = (cudaStream_t)stream;
+    const char *who = "cphb_tsdf_extract_mesh";
+    if (!v || !h_n_vertices || !h_n_triangles) return tsdf_invalid(who, "null argument");
+    *h_n_vertices = *h_n_triangles = 0;
+    if ((vertex_capacity || triangle_capacity) && (!vertices || !triangles || (v->ct != TSDF_NO_COLOR && !colors)))
+        return tsdf_invalid(who, "null output");
+    cphb_scratch sc(s);
+    uint8_t *cb = nullptr, *em = nullptr;
+    int32_t *vpos = nullptr, *cpos = nullptr, *vbase = nullptr;
+    int rc = sc.alloc(&cb, v->n);
+    if (!rc) rc = sc.alloc(&em, v->n);
+    if (!rc) rc = sc.alloc(&vpos, v->n);
+    if (!rc) rc = sc.alloc(&cpos, v->n);
+    if (!rc) rc = sc.alloc(&vbase, v->n);
+    if (rc) return rc;
+    const dim3 g = tsdf_vox_grid(v->res);
+    CPHB_LAUNCH(tsdf_mc_cube_kernel, g, TSDF_VOX_BLOCK, 0, s, v->tw, v->res, cb);
+    CPHB_LAUNCH(tsdf_mc_edge_kernel, g, TSDF_VOX_BLOCK, 0, s, cb, v->res, em);
+    size_t mv = 0, mc = 0;
+    rc = cphb_compact_flags(em, v->n, vpos, &mv, s);
+    if (!rc) rc = cphb_compact_flags(cb, v->n, cpos, &mc, s);
+    if (rc) return rc;
+    // output offsets: exclusive scans of the vertex counts of the mv edge voxels and of the triangle counts of the mc
+    // emitting cubes, each with one trailing 0.  They run also when a count is 0, so the launches do not depend on
+    // the data.
+    unsigned long long *vcnt = nullptr, *voff = nullptr, *tcnt = nullptr, *toff = nullptr;
+    rc = sc.alloc(&vcnt, mv + 1);
+    if (!rc) rc = sc.alloc(&voff, mv + 1);
+    if (!rc) rc = sc.alloc(&tcnt, mc + 1);
+    if (!rc) rc = sc.alloc(&toff, mc + 1);
+    if (rc) return rc;
+    CPHB_LAUNCH(tsdf_mc_count_kernel, tsdf_blocks(max(mv, mc) + 1, 256), 256, 0, s, vpos, mv, em, cpos, mc, cb, vcnt, tcnt);
+    rc = tsdf_scan(vcnt, voff, mv + 1, sc, s);
+    if (!rc) rc = tsdf_scan(tcnt, toff, mc + 1, sc, s);
+    unsigned long long nv = 0, nt = 0;
+    if (!rc) rc = cphb_read_back(&nv, voff + mv, sizeof(nv), s, who);
+    if (!rc) rc = cphb_read_back(&nt, toff + mc, sizeof(nt), s, who);
+    if (rc) return rc;
+    if (nv > (unsigned long long)INT32_MAX) {  // vertex indices are int32: refuse rather than truncate
+        cphb_set_error("%s: the mesh has %llu vertices, more than int32 vertex indices can name", who, nv);
+        return CPHB_ERR_INVALID;
+    }
+    // the writing launches always happen: a fixed launch count
+    const bool write = nv && vertex_capacity >= nv && triangle_capacity >= nt;
+    const size_t mvw = write ? mv : 0, mcw = write ? mc : 0;
+#define TSDF_MC_VERTS(CT)                                                                                                    \
+    CPHB_LAUNCH(tsdf_mc_vertex_kernel<CT>, tsdf_blocks(mvw, 128), 128, 0, s, v->tw, v->col, v->n, v->res, v->vl, v->half,  \
+                (float)v->h * v->vl, v->o[0], v->o[1], v->o[2], vpos, mvw, em, voff, vbase, vertices, colors)
+    if (v->ct == TSDF_RGB8)
+        TSDF_MC_VERTS(TSDF_RGB8);
+    else if (v->ct == TSDF_GRAY32)
+        TSDF_MC_VERTS(TSDF_GRAY32);
+    else
+        TSDF_MC_VERTS(TSDF_NO_COLOR);
+#undef TSDF_MC_VERTS
+    CPHB_LAUNCH(tsdf_mc_triangle_kernel, tsdf_blocks(mcw, 128), 128, 0, s, cpos, mcw, cb, em, vbase, v->res, toff, triangles);
+    rc = cphb_read_back(nullptr, nullptr, 0, s, who);
+    if (!rc) {
+        *h_n_vertices = (size_t)nv;
+        *h_n_triangles = (size_t)nt;
+    }
+    return rc;
+}
+
 // ------------------------------------------------------------------------------------------------ Raycast
 struct TsdfRay {
     float P[12];  // camera pose (InverseTransform of the extrinsic), rows 0..2

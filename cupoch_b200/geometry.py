@@ -451,6 +451,87 @@ class PointCloud:
         return True
 
 
+class TriangleMesh:
+    """geometry::TriangleMesh (trianglemesh.h): vertices_, triangles_ (int32 vertex indices), vertex_colors_,
+    vertex_normals_ and triangle_normals_ on the device.  Only the normal computations run here; the rest of the
+    reference's TriangleMesh is not provided."""
+
+    def __init__(self, vertices=None, triangles=None):
+        self._vertices = self._triangles = self._vertex_colors = self._vertex_normals = self._triangle_normals = None
+        if vertices is not None:
+            self.vertices = vertices
+        if triangles is not None:
+            self.triangles = triangles
+
+    vertices = property(lambda s: s._vertices, lambda s, v: setattr(s, "_vertices", Vector3fVector(v)))
+    triangles = property(lambda s: s._triangles, lambda s, v: setattr(s, "_triangles", _vector3i(v)))
+    vertex_colors = property(lambda s: s._vertex_colors, lambda s, v: setattr(s, "_vertex_colors", Vector3fVector(v)))
+    vertex_normals = property(lambda s: s._vertex_normals, lambda s, v: setattr(s, "_vertex_normals", Vector3fVector(v)))
+    triangle_normals = property(lambda s: s._triangle_normals, lambda s, v: setattr(s, "_triangle_normals", Vector3fVector(v)))
+
+    def __repr__(self):
+        return "geometry::TriangleMesh with %d points and %d triangles." % (self._n(self._vertices), self._n(self._triangles))
+
+    @staticmethod
+    def _n(a):
+        return 0 if a is None else len(a)
+
+    def is_empty(self):
+        return not self.has_vertices()
+
+    # trianglemesh.h / meshbase.h: "non-empty and, for a per-vertex or per-triangle attribute, of matching length"
+    def has_vertices(self):
+        return self._n(self._vertices) > 0
+
+    def has_triangles(self):
+        return self.has_vertices() and self._n(self._triangles) > 0
+
+    def has_vertex_colors(self):
+        return self.has_vertices() and self._n(self._vertex_colors) == len(self._vertices)
+
+    def has_vertex_normals(self):
+        return self.has_vertices() and self._n(self._vertex_normals) == len(self._vertices)
+
+    def has_triangle_normals(self):
+        return self.has_triangles() and self._n(self._triangle_normals) == len(self._triangles)
+
+    def compute_triangle_normals(self, normalized=True):
+        """ComputeTriangleNormals (trianglemesh.cu:466-477): (v1 - v0) x (v2 - v0) per triangle, then normalised when
+        asked.  A vertex index outside [0, len(vertices)) raises."""
+        m = self._n(self._triangles)
+        out = DeviceArray((m, 3), np.float32)
+        if m:
+            _lib.check(_lib.lib().cphb_mesh_triangle_normals(self._vertices.ptr if self._vertices is not None else None,
+                                                             self._n(self._vertices), self._triangles.ptr, m, int(bool(normalized)),
+                                                             out.ptr, None))
+        self._triangle_normals = out
+        return self
+
+    def compute_vertex_normals(self, normalized=True):
+        """ComputeVertexNormals (trianglemesh.cu:479-503): the unnormalised triangle normals first when the mesh has
+        none; each vertex's normal is the sum of its triangles' normals in ascending triangle order, then normalised
+        when asked.  A vertex in no triangle gets a zero normal (the reference drops it and misaligns the rest)."""
+        if not self.has_triangle_normals():
+            self.compute_triangle_normals(False)
+        n, m = self._n(self._vertices), self._n(self._triangles)
+        out = DeviceArray((n, 3), np.float32)
+        if n or m:
+            _lib.check(_lib.lib().cphb_mesh_vertex_normals(self._triangles.ptr if m else None, m,
+                                                           self._triangle_normals.ptr if m else None, n, int(bool(normalized)),
+                                                           out.ptr, None))
+        self._vertex_normals = out
+        return self
+
+
+def _vector3i(a):
+    if a is None:
+        return None
+    d = DeviceArray.wrap(a, np.int32)
+    if len(d.shape) != 2 or d.shape[1] != 3:
+        raise ValueError("expected (n,3) int32")
+    return d
+
+
 def _v3(v):
     return np.asarray(v, np.float32).reshape(3).copy()
 

@@ -9,7 +9,7 @@ import enum
 import numpy as np
 
 from . import _lib
-from .geometry import PointCloud, VoxelGrid
+from .geometry import PointCloud, TriangleMesh, VoxelGrid
 from .utility import DeviceArray
 
 
@@ -101,6 +101,24 @@ class UniformTSDFVolume:
         if m:
             pc._points, pc._normals, pc._colors = outs
         return pc
+
+    def extract_triangle_mesh(self):
+        """ExtractTriangleMesh (uniform_tsdfvolume.cu:184-350, 739-838), welded: one vertex per crossed grid edge of
+        a valid cube (all 8 corner weights nonzero), in (x, y, z, axis) order of the edge's origin voxel, coloured
+        unless NoColor; the triangles of each cube in cube index order, oriented so that their right-hand normals
+        point from negative to positive tsdf (outwards)."""
+        L = _lib.lib()
+        has_c = self._color_type != TSDFVolumeColorType.NoColor
+        nv, nt = C.c_size_t(0), C.c_size_t(0)
+        _lib.check(L.cphb_tsdf_extract_mesh(self._h, None, None, None, 0, 0, C.byref(nv), C.byref(nt), None))
+        mesh = TriangleMesh()
+        if nv.value:
+            v, t = DeviceArray((nv.value, 3), np.float32), DeviceArray((nt.value, 3), np.int32)
+            c = DeviceArray((nv.value, 3), np.float32) if has_c else None
+            _lib.check(L.cphb_tsdf_extract_mesh(self._h, v.ptr, c.ptr if c is not None else None, t.ptr, nv.value, nt.value,
+                                                C.byref(nv), C.byref(nt), None))
+            mesh._vertices, mesh._triangles, mesh._vertex_colors = v, t, c
+        return mesh
 
     def extract_voxel_point_cloud(self):
         """ExtractVoxelPointCloud (uniform_tsdfvolume.cu:840-865): the centre of every band voxel, coloured (tsdf + 1) / 2"""

@@ -37,6 +37,10 @@ def main():
     print("extract_point_cloud:", len(volume.extract_point_cloud()), "points with normals")
     print("extract_voxel_point_cloud:", len(volume.extract_voxel_point_cloud()), "voxels in the band")
     print("extract_voxel_grid:", len(volume.extract_voxel_grid()), "voxels")
+    mesh = volume.extract_triangle_mesh()
+    mesh.compute_vertex_normals()
+    print("extract_triangle_mesh:", len(mesh.vertices) if mesh.has_vertices() else 0, "vertices,",
+          len(mesh.triangles) if mesh.has_triangles() else 0, "triangles, with vertex normals")
 
     E = cams[0][1]
     target = volume.raycast(intrinsic, E, 0.04)

@@ -1910,6 +1910,54 @@ private:
 };
 }  // namespace geometry
 
+namespace geometry {
+/// geometry::TriangleMesh (trianglemesh.h, meshbase.h): vertices_, vertex_normals_, vertex_colors_, triangles_ (int32
+/// vertex indices) and triangle_normals_ on the device.  Only the two normal computations are provided.
+class TriangleMesh {
+public:
+    TriangleMesh() {}
+    TriangleMesh(const utility::device_vector<Eigen::Vector3f> &vertices, const utility::device_vector<Eigen::Vector3i> &triangles)
+        : vertices_(vertices), triangles_(triangles) {}
+    TriangleMesh(const std::vector<Eigen::Vector3f> &vertices, const std::vector<Eigen::Vector3i> &triangles)
+        : vertices_(vertices), triangles_(triangles) {}
+
+    bool IsEmpty() const { return !HasVertices(); }
+    bool HasVertices() const { return vertices_.size() > 0; }
+    bool HasVertexNormals() const { return HasVertices() && vertex_normals_.size() == vertices_.size(); }
+    bool HasVertexColors() const { return HasVertices() && vertex_colors_.size() == vertices_.size(); }
+    bool HasTriangles() const { return HasVertices() && triangles_.size() > 0; }
+    bool HasTriangleNormals() const { return HasTriangles() && triangle_normals_.size() == triangles_.size(); }
+
+    /// ComputeTriangleNormals (trianglemesh.cu:466-477): (v1 - v0) x (v2 - v0), normalised when asked.  A vertex index
+    /// outside [0, vertices_.size()) throws.
+    TriangleMesh &ComputeTriangleNormals(bool normalized = true) {
+        triangle_normals_.resize(triangles_.size());
+        if (triangles_.size())
+            utility::check(cphb_mesh_triangle_normals((const float *)vertices_.data(), vertices_.size(), (const int32_t *)triangles_.data(),
+                                                      triangles_.size(), normalized ? 1 : 0, (float *)triangle_normals_.data(), nullptr));
+        return *this;
+    }
+    /// ComputeVertexNormals (trianglemesh.cu:479-503): the unnormalised triangle normals first when there are none; each
+    /// vertex's normal is the sum of its triangles' normals in ascending triangle order, normalised when asked.  A vertex
+    /// in no triangle gets a zero normal, so vertex_normals_ stays aligned with vertices_.
+    TriangleMesh &ComputeVertexNormals(bool normalized = true) {
+        if (!HasTriangleNormals()) ComputeTriangleNormals(false);
+        vertex_normals_.resize(vertices_.size());
+        if (vertices_.size() || triangles_.size())
+            utility::check(cphb_mesh_vertex_normals((const int32_t *)triangles_.data(), triangles_.size(), (const float *)triangle_normals_.data(),
+                                                    vertices_.size(), normalized ? 1 : 0, (float *)vertex_normals_.data(), nullptr));
+        return *this;
+    }
+
+public:
+    utility::device_vector<Eigen::Vector3f> vertices_;
+    utility::device_vector<Eigen::Vector3f> vertex_normals_;
+    utility::device_vector<Eigen::Vector3f> vertex_colors_;
+    utility::device_vector<Eigen::Vector3i> triangles_;
+    utility::device_vector<Eigen::Vector3f> triangle_normals_;
+};
+}  // namespace geometry
+
 namespace integration {
 /// integration::TSDFVolumeColorType (tsdfvolume.h)
 enum class TSDFVolumeColorType { NoColor = 0, RGB8 = 1, Gray32 = 2 };
@@ -1920,6 +1968,8 @@ public:
     TSDFVolume(float voxel_length, float sdf_trunc, TSDFVolumeColorType color_type)
         : voxel_length_(voxel_length), sdf_trunc_(sdf_trunc), color_type_(color_type) {}
     virtual ~TSDFVolume() {}
+    /// the surface as a welded triangle mesh (tsdfvolume.h:68)
+    virtual std::shared_ptr<geometry::TriangleMesh> ExtractTriangleMesh() = 0;
 
 public:
     float voxel_length_;
@@ -1976,6 +2026,22 @@ public:
                                                     n, &n, nullptr));
         }
         return pc;
+    }
+    /// ExtractTriangleMesh (uniform_tsdfvolume.cu:739-838), welded: one vertex per crossed grid edge of a valid cube,
+    /// coloured unless NoColor; triangles cube by cube, their right-hand normals pointing from negative to positive tsdf
+    std::shared_ptr<geometry::TriangleMesh> ExtractTriangleMesh() override {
+        auto mesh = std::make_shared<geometry::TriangleMesh>();
+        const bool has_c = color_type_ != TSDFVolumeColorType::NoColor;
+        size_t nv = 0, nt = 0;
+        utility::check(cphb_tsdf_extract_mesh(h_, nullptr, nullptr, nullptr, 0, 0, &nv, &nt, nullptr));
+        if (nv) {
+            mesh->vertices_.resize(nv);
+            if (has_c) mesh->vertex_colors_.resize(nv);
+            mesh->triangles_.resize(nt);
+            utility::check(cphb_tsdf_extract_mesh(h_, (float *)mesh->vertices_.data(), has_c ? (float *)mesh->vertex_colors_.data() : nullptr,
+                                                  (int32_t *)mesh->triangles_.data(), nv, nt, &nv, &nt, nullptr));
+        }
+        return mesh;
     }
     /// ExtractVoxelPointCloud (uniform_tsdfvolume.cu:840-865): band voxel centres coloured (tsdf + 1) / 2
     std::shared_ptr<geometry::PointCloud> ExtractVoxelPointCloud() const {

@@ -584,6 +584,26 @@ int cphb_tsdf_extract_voxels(const cphb_tsdf *volume, int32_t *keys, float *poin
 int cphb_tsdf_raycast(const cphb_tsdf *volume, int width, int height, const float h_intrinsic[9], const float h_extrinsic[16],
                       float sdf_trunc, int project_valid_depth_only, float *points, float *normals, float *colors, size_t capacity,
                       size_t *h_count, void *stream);
+/* ExtractTriangleMesh: welded marching cubes (DESIGN section 4 item 19).  One vertex per crossed grid edge of a valid
+ * cube (all 8 corner weights nonzero), in (x, y, z, axis) order of the edge's origin voxel: vertices [n_vertices][3]
+ * and, unless NoColor, colours [n_vertices][3]; triangles [n_triangles][3] int32 vertex indices, cube by cube in cube
+ * index order, then table order, oriented so that (v1 - v0) x (v2 - v0) points from negative to positive tsdf.
+ * *h_n_vertices / *h_n_triangles are the counts; the rows are written only when both capacities hold them (0 sizes).
+ * A vertex count past INT32_MAX is CPHB_ERR_INVALID.  Synchronises. */
+int cphb_tsdf_extract_mesh(const cphb_tsdf *volume, float *vertices, float *colors, int32_t *triangles, size_t vertex_capacity,
+                           size_t triangle_capacity, size_t *h_n_vertices, size_t *h_n_triangles, void *stream);
+
+/* ------------------------------------------------------------------------ *
+ * TriangleMesh normals (geometry/trianglemesh.cu), on device arrays: vertices [n_vertices][3] float32, triangles
+ * [n_triangles][3] int32.  A vertex index outside [0, n_vertices) is CPHB_ERR_INVALID.  Synchronise.
+ * ------------------------------------------------------------------------ */
+/* ComputeTriangleNormals: (v1 - v0) x (v2 - v0) per triangle, normalised (NormalizeNormals' rule) when asked */
+int cphb_mesh_triangle_normals(const float *vertices, size_t n_vertices, const int32_t *triangles, size_t n_triangles, int normalized,
+                               float *triangle_normals, void *stream);
+/* ComputeVertexNormals' sum: vertex v's normal is the sum of its triangles' normals in ascending (triangle, corner)
+ * order, normalised when asked; a vertex in no triangle gets 0, so the rows stay aligned with the vertices */
+int cphb_mesh_vertex_normals(const int32_t *triangles, size_t n_triangles, const float *triangle_normals, size_t n_vertices,
+                             int normalized, float *vertex_normals, void *stream);
 
 /* ------------------------------------------------------------------------ *
  * collision::ComputeIntersection (collision.h:36-160, collision.cu:1137-1231)

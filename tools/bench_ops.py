@@ -47,7 +47,12 @@ def main():
     ap.add_argument("--tsdf", action="store_true",
                     help="instead: time UniformTSDFVolume Integrate of a 640x480 frame at 256^3 and 512^3 per colour type, "
                          "both extractions and a 640x480 Raycast")
+    ap.add_argument("--tsdf-mesh", action="store_true",
+                    help="instead: time UniformTSDFVolume.extract_triangle_mesh and compute_vertex_normals at 256^3 and 512^3 "
+                         "after 8 ring-camera sphere views")
     args = ap.parse_args()
+    if args.tsdf_mesh:
+        return tsdf_mesh(args.reps, args.out)
     if args.tsdf:
         return tsdf(args.reps, args.out)
     if args.collision:
@@ -1034,6 +1039,94 @@ def tsdf(reps, out=None):
         del vol
     obj = {"op": "UniformTSDFVolume(2.0, res, 0.04): 640x480 sphere frames (radius 0.6, cameras at 2.5); extractions and "
                  "Raycast after 8 views", "gpu": gpu, "reps": reps, "rows": rows}
+    line = json.dumps(obj)
+    print(line)
+    if out:
+        with open(out, "w") as f:
+            f.write(line + "\n")
+
+
+def tsdf_mesh_bytes(n_voxels, nv, nt, colour_planes):
+    """least HBM traffic of one ExtractTriangleMesh: the {tsdf, weight} plane read once (8 bytes a voxel), plus the
+    outputs written once: 12 bytes a vertex, 12 a vertex colour when the volume has colour, 12 a triangle.  The colour
+    planes are read only at the vertices' voxels, which is not counted; nor is the scratch (cube bytes, edge masks,
+    positions)."""
+    return 8 * n_voxels + 12 * nv * (2 if colour_planes else 1) + 12 * nt
+
+
+def tsdf_mesh(reps, out=None):
+    """UniformTSDFVolume(2.0, res, 0.04, RGB8) with res = 256 and 512 after the 8 ring-camera 640 x 480 views of a sphere
+    of radius 0.6 (tests/test_gpu_tsdf.py's scene): extract_triangle_mesh (the sizing call and the writing call, as the
+    Python front end makes them) and compute_vertex_normals of its mesh.  CUDA-event median and minimum of `reps` calls
+    after a warm-up call, the kernel times of one further call from torch.profiler, and the bytes model of
+    tsdf_mesh_bytes over the extraction's kernel time against 3.35 TB/s."""
+    import subprocess
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    import cupoch_b200 as cph
+    from cupoch_b200 import _lib
+    from cupoch_b200.testing.datagen import ring_cameras, sphere_depth
+    L = _lib.lib()
+    G, I = cph.geometry, cph.integration
+    gpu = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                         capture_output=True, text=True).stdout.strip()
+    ev = [L.cphb_event_create() for _ in range(2)]
+
+    def timed(fn):
+        times = []
+        for r in range(reps + 1):
+            L.cphb_event_record(ev[0], None)
+            fn()
+            L.cphb_event_record(ev[1], None)
+            ms = C.c_float(0)
+            _lib.check(L.cphb_event_elapsed_ms(ev[0], ev[1], C.byref(ms)))
+            if r:
+                times.append(ms.value)
+        return times
+
+    def kernels(fn):
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            fn()
+            torch.cuda.synchronize()
+        k = {}
+        for e in prof.key_averages():
+            t = getattr(e, "device_time_total", getattr(e, "cuda_time_total", 0.0)) * 1e-3
+            if t > 0 and "Memset" not in e.key and "Memcpy" not in e.key:
+                k[e.key[:60]] = k.get(e.key[:60], 0.0) + t
+        return k
+
+    w, h = 640, 480
+    rng = np.random.default_rng(2)
+    rows = []
+    for res in (256, 512):
+        vol = I.UniformTSDFVolume(2.0, res, 0.04, I.TSDFVolumeColorType.RGB8)
+        for K, E in ring_cameras(8, w, h):
+            d16 = np.round(sphere_depth(K, E, w, h, 0.6) * 1000).astype(np.uint16)
+            intr = cph.camera.PinholeCameraIntrinsic(w, h, K[0, 0], K[1, 1], K[0, 2], K[1, 2])
+            col = rng.integers(0, 256, (h, w, 3), dtype=np.uint8)
+            vol.integrate(G.RGBDImage.create_from_color_and_depth(G.Image(col), G.Image(d16), 1000.0, 100.0, False), intr, E)
+        mesh = vol.extract_triangle_mesh()
+        nv, nt = len(mesh.vertices), len(mesh.triangles)
+        ts = timed(vol.extract_triangle_mesh)
+        k = kernels(vol.extract_triangle_mesh)
+        kern = float(sum(k.values()))
+        nbytes = tsdf_mesh_bytes(res ** 3, nv, nt, 3)
+        rows.append({"op": "ExtractTriangleMesh (sizing + writing call)", "res": res, "color_type": "RGB8", "vertices": nv,
+                     "triangles": nt, "call_ms_median": float(np.median(ts)), "call_ms_min": float(np.min(ts)),
+                     "kernel_ms_profiled": k, "kernel_ms_sum": kern, "bytes_model": nbytes,
+                     "share_of_3.35TBps_over_kernel_time": nbytes / (kern * 1e-3) / HBM_BYTES_PER_S if kern else None})
+
+        def normals():
+            mesh.triangle_normals = None
+            mesh.compute_vertex_normals()
+        ts = timed(normals)
+        k = kernels(normals)
+        rows.append({"op": "ComputeVertexNormals (triangle normals first)", "res": res, "vertices": nv, "triangles": nt,
+                     "call_ms_median": float(np.median(ts)), "call_ms_min": float(np.min(ts)), "kernel_ms_profiled": k,
+                     "kernel_ms_sum": float(sum(k.values()))})
+        del mesh, vol
+    obj = {"op": "UniformTSDFVolume(2.0, res, 0.04, RGB8) after 8 640x480 ring-camera views of a sphere (radius 0.6, cameras "
+                 "at 2.5): ExtractTriangleMesh and ComputeVertexNormals", "gpu": gpu, "reps": reps, "rows": rows}
     line = json.dumps(obj)
     print(line)
     if out:

@@ -56,3 +56,6 @@ for K, E in ring_cameras(3, 64, 48):
     vol.integrate(im, intr, E)
 print("tsdf points", len(vol.extract_point_cloud()), "voxels", len(vol.extract_voxel_grid()),
       "raycast", len(vol.raycast(intr, E, 0.08)), len(vol.raycast(intr, E, 0.08, False)))
+mesh = vol.extract_triangle_mesh()
+mesh.compute_vertex_normals()
+print("tsdf mesh vertices", len(mesh.vertices), "triangles", len(mesh.triangles), "vertex normals", len(mesh.vertex_normals))

@@ -7,9 +7,11 @@
   +-0.98, the crossing interpolation and its (x, y, z, axis) order, the zero-gradient normal.
 - The deviations: Reset restores the initial voxels, ExtractPointCloud is sized by its crossings, Raycast enters the grid
   on the box of the cells it samples (also along axis-aligned rays and from a camera on the grid's high side).
-- A float64 restatement of Integrate: the voxels whose update decision differs are listed with their margins, which
-  must stay within a stated bound.  Raycast has no float64 restatement; its hits are checked against the analytic
-  sphere (within one voxel) and, on the GPU, against this oracle bit for bit."""
+- A float64 restatement of Integrate, at an even resolution and at an odd one with an origin off the voxel lattice: the
+  voxels whose update decision differs are listed with their margins, which must stay within a stated bound.
+  ExtractPointCloud and Raycast are checked against their float64 restatements (cupoch_b200/testing/tsdf64.py) and
+  against analytic planar and spherical fields in test_oracle_tsdf64.py; on the GPU all of them are checked against
+  this oracle bit for bit."""
 import os
 
 import numpy as np
@@ -211,16 +213,17 @@ def test_raycast_enters_on_the_grids_real_box():
     assert np.all(np.abs(np.linalg.norm(hp, axis=1) - 0.6) < 2.0 / 64)
 
 
-def test_integrate_against_a_float64_restatement():
-    """Integrate restated in float64 on a 48^3 volume and 4 sphere views: the update decisions that differ from the
-    float32 restatement are listed with their margins -- how far the float64 quantity was from the rule's threshold
-    (z <= 0, the image bounds, sdf > -trunc) -- which stay below 1e-5; the tsdf of the voxels both update agrees to 1e-4."""
-    res, length, trunc, w, h = 48, 2.0, 0.1, 80, 60
-    vol = T.Volume(length, res, trunc)
+def integrate_vs_float64(res, origin=(0.0, 0.0, 0.0)):
+    """Integrate restated in float64 on 4 sphere views: the update decisions that differ from the float32 restatement
+    are listed with their margins -- how far the float64 quantity was from the rule's threshold (z <= 0, the image
+    bounds, sdf > -trunc) -- which stay below 1e-5; the tsdf of the voxels both update agrees to 1e-4."""
+    length, trunc, w, h = 2.0, 0.1, 80, 60
+    vol = T.Volume(length, res, trunc, origin=origin)
     vl = length / res
     hres = res // 2
+    o = np.asarray(origin, np.float32).astype(np.float64)
     k = (np.arange(res) - hres) * vl + vl / 2
-    X, Y, Z = np.meshgrid(k, k, k, indexing="ij")
+    X, Y, Z = np.meshgrid(k + o[0], k + o[1], k + o[2], indexing="ij")
     P = np.stack([X, Y, Z], -1).reshape(-1, 3)
     tsdf64, w64 = np.zeros(len(P)), np.zeros(len(P))
     differing = []
@@ -251,6 +254,16 @@ def test_integrate_against_a_float64_restatement():
     both = (vol.tw[:, 1] == w64) & (w64 > 0)
     assert both.sum() > 1000 and len(differing) < 0.001 * both.sum()
     assert np.max(np.abs(vol.tw[both, 0] - tsdf64[both])) < 1e-4
+
+
+def test_integrate_against_a_float64_restatement():
+    """a 48^3 volume at the origin"""
+    integrate_vs_float64(48)
+
+
+def test_integrate_against_a_float64_restatement_at_odd_res_and_an_offset_origin():
+    """47^3 (res / 2 rounds down) with an origin off the voxel lattice"""
+    integrate_vs_float64(47, (0.0123, -0.0311, 0.0057))
 
 
 def test_raycast_from_a_camera_on_the_high_side_hits():

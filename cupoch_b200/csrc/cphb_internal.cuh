@@ -175,6 +175,9 @@ int cphb_sort_pairs_u64(const uint64_t *keys_in, uint64_t *keys_out, const uint3
 // stable compaction (filters.cu): ascending positions i < n with keep[i] != 0 -> indices_out, their number to
 // *h_n_out (synchronises the stream)
 int cphb_compact_flags(const uint8_t *keep, size_t n, int32_t *indices_out, size_t *h_n_out, cudaStream_t s);
+// the middle step of every block compaction (filters.cu's keep_scan_kernel, one launch on s): exclusive scan of the nb
+// per-block counts in place, their sum to *total.  Allocates nothing and does not synchronise.
+void cphb_scan_block_counts(unsigned *counts, unsigned nb, unsigned *total, cudaStream_t s);
 
 // neighbour table of an index client (search.cu): create builds an index of points[n] and searches the rows
 // [first, first + count) against it into idx / d2 [count][k] -- KNN(knn) when knn > 0, else Radius(radius, max_nn),
@@ -295,6 +298,42 @@ __device__ __forceinline__ double p2p_exchange_sum(const P2pView &v, double mine
 // device helpers
 // ---------------------------------------------------------------------------
 __device__ __forceinline__ int lane_id() { return threadIdx.x & 31; }
+
+// The two per-block steps of a stable compaction, around cphb_scan_block_counts: a count kernel stores
+// block_flag_count(flag) of each block, a write kernel puts a flagged thread's payload at
+// block_offsets[blockIdx.x] + block_flag_rank(flag).  Every thread of the block calls them; blockDim.x is a multiple
+// of 32, at most 1024.
+// -> the number of set flags in the block, valid in thread 0
+__device__ __forceinline__ unsigned block_flag_count(bool v) {
+    __shared__ unsigned s_w[32];
+    const unsigned m = __ballot_sync(CPHB_FULL, v);
+    if (lane_id() == 0) s_w[threadIdx.x >> 5] = __popc(m);
+    __syncthreads();
+    // the first warp adds the warp counts.  REDUX, not a shuffle tree: the block's slot is held until this tail ends,
+    // and a shuffle tree under this branch also gets a divergent-warp fallback from nvcc (3-4 % slower count kernels)
+    unsigned c = 0;
+    if (threadIdx.x < 32) c = __reduce_add_sync(CPHB_FULL, threadIdx.x < (blockDim.x >> 5) ? s_w[threadIdx.x] : 0u);
+    return c;
+}
+// -> the number of set flags of the block's lower threads (this thread's position among the block's flagged threads)
+__device__ __forceinline__ unsigned block_flag_rank(bool v) {
+    __shared__ unsigned s_w[32];
+    const unsigned m = __ballot_sync(CPHB_FULL, v);
+    if (lane_id() == 0) s_w[threadIdx.x >> 5] = __popc(m);
+    __syncthreads();
+    if (threadIdx.x < 32) {  // exclusive scan of the warp counts (entries past the block's warps are never read)
+        const unsigned ws = s_w[threadIdx.x];
+        unsigned z = ws;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const unsigned y = __shfl_up_sync(CPHB_FULL, z, o);
+            if (lane_id() >= o) z += y;
+        }
+        s_w[threadIdx.x] = z - ws;
+    }
+    __syncthreads();
+    return s_w[threadIdx.x >> 5] + __popc(m & ((1u << lane_id()) - 1u));
+}
 
 // order-preserving float <-> uint (for atomicMin/Max and REDUX on signed floats)
 __host__ __device__ __forceinline__ unsigned f2ord(float f) {

@@ -125,21 +125,14 @@ __global__ void __launch_bounds__(256) stat_keep_kernel(const float *__restrict_
 
 // ---- stable compaction of the indices whose flag is set ---------------------
 __global__ void __launch_bounds__(FLT_BLOCK) keep_count_kernel(const uint8_t *__restrict__ keep, size_t n, unsigned *block_counts) {
-    __shared__ unsigned s_w[32];
     const size_t i = blockIdx.x * (size_t)FLT_BLOCK + threadIdx.x;
-    const bool v = i < n && keep[i];
-    const unsigned m = __ballot_sync(CPHB_FULL, v);
-    if (lane_id() == 0) s_w[threadIdx.x >> 5] = __popc(m);
-    __syncthreads();
-    if (threadIdx.x < 32) {
-        unsigned c = s_w[threadIdx.x];
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(CPHB_FULL, c, o);
-        if (threadIdx.x == 0) block_counts[blockIdx.x] = c;
-    }
+    const unsigned c = block_flag_count(i < n && keep[i]);
+    if (threadIdx.x == 0) block_counts[blockIdx.x] = c;
 }
-// exclusive scan of the block counts in place (one block), total to *total
-__global__ void __launch_bounds__(FLT_BLOCK) keep_scan_kernel(unsigned *block_counts, unsigned nb, unsigned long long *total) {
+// exclusive scan of the block counts in place (one block), total to *total.  The one copy of this step: every block
+// compaction of the engine (this file's, VoxelDownSample's dense path, ICP's correspondence list) launches it through
+// cphb_scan_block_counts.
+__global__ void __launch_bounds__(FLT_BLOCK) keep_scan_kernel(unsigned *block_counts, unsigned nb, unsigned *total) {
     __shared__ unsigned s_w[32];
     __shared__ unsigned s_carry;
     if (threadIdx.x == 0) s_carry = 0;
@@ -176,44 +169,30 @@ __global__ void __launch_bounds__(FLT_BLOCK) keep_scan_kernel(unsigned *block_co
 }
 __global__ void __launch_bounds__(FLT_BLOCK) keep_write_kernel(const uint8_t *__restrict__ keep, size_t n,
                                                                const unsigned *__restrict__ block_offsets, int32_t *out) {
-    __shared__ unsigned s_w[32];
     const size_t i = blockIdx.x * (size_t)FLT_BLOCK + threadIdx.x;
     const bool v = i < n && keep[i];
-    const unsigned m = __ballot_sync(CPHB_FULL, v);
-    if (lane_id() == 0) s_w[threadIdx.x >> 5] = __popc(m);
-    __syncthreads();
-    if (threadIdx.x < 32) {
-        const unsigned ws = s_w[threadIdx.x];
-        unsigned z = ws;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const unsigned y = __shfl_up_sync(CPHB_FULL, z, o);
-            if (lane_id() >= o) z += y;
-        }
-        s_w[threadIdx.x] = z - ws;  // exclusive offset of each warp inside the block
-    }
-    __syncthreads();
-    if (v) {
-        const unsigned pos = block_offsets[blockIdx.x] + s_w[threadIdx.x >> 5] + __popc(m & ((1u << lane_id()) - 1u));
-        out[pos] = (int32_t)i;
-    }
+    const unsigned r = block_flag_rank(v);
+    if (v) out[block_offsets[blockIdx.x] + r] = (int32_t)i;
+}
+
+void cphb_scan_block_counts(unsigned *counts, unsigned nb, unsigned *total, cudaStream_t s) {
+    CPHB_LAUNCH(keep_scan_kernel, 1, FLT_BLOCK, 0, s, counts, nb, total);
 }
 
 // keep flags -> ascending indices in indices_out, count to *h_n_out (synchronises)
 int cphb_compact_flags(const uint8_t *keep, size_t n, int32_t *indices_out, size_t *h_n_out, cudaStream_t s) {
     const unsigned nb = (unsigned)((n + FLT_BLOCK - 1) / FLT_BLOCK);
     cphb_scratch sc(s);
-    unsigned *counts = nullptr;
-    unsigned long long *total = nullptr;
+    unsigned *counts = nullptr, *total = nullptr;
     int rc = sc.alloc(&counts, (size_t)nb + 4);
     if (!rc) rc = sc.alloc(&total, 1);
     if (rc) return rc;
     CPHB_LAUNCH(keep_count_kernel, nb, FLT_BLOCK, 0, s, keep, n, counts);
-    CPHB_LAUNCH(keep_scan_kernel, 1, FLT_BLOCK, 0, s, counts, nb, total);
+    cphb_scan_block_counts(counts, nb, total, s);
     CPHB_LAUNCH(keep_write_kernel, nb, FLT_BLOCK, 0, s, keep, n, counts, indices_out);
-    unsigned long long h = 0;
+    unsigned h = 0;
     rc = cphb_read_back(&h, total, sizeof(h), s, "cphb_compact_flags");
-    if (!rc) *h_n_out = (size_t)h;
+    if (!rc) *h_n_out = h;
     return rc;
 }
 

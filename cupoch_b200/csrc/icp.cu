@@ -435,7 +435,7 @@ static int compact_correspondences(cphb_icp *icp, int32_t *corr_out, cudaStream_
     unsigned nb = (n + CMP_BLOCK - 1) / CMP_BLOCK;
     if (nb == 0) nb = 1;
     CPHB_LAUNCH(compact_count_kernel, nb, CMP_BLOCK, 0, s, icp->corr_index, n, icp->cmp_counts);
-    CPHB_LAUNCH(compact_scan_kernel, 1, 1024, 0, s, icp->cmp_counts, nb, icp->cmp_total);
+    cphb_scan_block_counts(icp->cmp_counts, nb, icp->cmp_total, s);
     CPHB_LAUNCH(compact_write_kernel, nb, CMP_BLOCK, 0, s, icp->corr_index, n, icp->cmp_counts, corr_out);
     CPHB_CHECK_LAUNCH();
     return CPHB_OK;

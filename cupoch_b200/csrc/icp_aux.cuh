@@ -71,75 +71,19 @@ __global__ void __launch_bounds__(256) gather_target_kernel(const float4 *__rest
 #define CMP_BLOCK 1024
 __global__ void __launch_bounds__(CMP_BLOCK) compact_count_kernel(const int32_t *__restrict__ ci, unsigned n,
                                                                   unsigned *block_counts) {
-    __shared__ unsigned s_w[32];
     unsigned i = blockIdx.x * CMP_BLOCK + threadIdx.x;
-    bool v = i < n && ci[i] >= 0;
-    unsigned m = __ballot_sync(CPHB_FULL, v);
-    if (lane_id() == 0) s_w[threadIdx.x >> 5] = __popc(m);
-    __syncthreads();
-    if (threadIdx.x < 32) {
-        unsigned c = s_w[threadIdx.x];
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(CPHB_FULL, c, o);
-        if (threadIdx.x == 0) block_counts[blockIdx.x] = c;
-    }
-}
-__global__ void __launch_bounds__(1024) compact_scan_kernel(unsigned *block_counts, unsigned nb, unsigned *total) {
-    __shared__ unsigned s_w[32];
-    __shared__ unsigned s_carry;
-    if (threadIdx.x == 0) s_carry = 0;
-    __syncthreads();
-    for (unsigned base = 0; base < nb; base += 1024) {
-        unsigned i = base + threadIdx.x;
-        unsigned v = i < nb ? block_counts[i] : 0u;
-        unsigned x = v;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            unsigned y = __shfl_up_sync(CPHB_FULL, x, o);
-            if (lane_id() >= o) x += y;
-        }
-        if (lane_id() == 31) s_w[threadIdx.x >> 5] = x;
-        __syncthreads();
-        if (threadIdx.x < 32) {
-            unsigned ws = s_w[threadIdx.x], z = ws;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                unsigned y = __shfl_up_sync(CPHB_FULL, z, o);
-                if (lane_id() >= o) z += y;
-            }
-            s_w[threadIdx.x] = z - ws;
-        }
-        __syncthreads();
-        unsigned excl = x - v + s_w[threadIdx.x >> 5] + s_carry;
-        if (i < nb) block_counts[i] = excl;
-        __syncthreads();
-        if (threadIdx.x == 1023) s_carry = excl + v;
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) *total = s_carry;
+    unsigned c = block_flag_count(i < n && ci[i] >= 0);
+    if (threadIdx.x == 0) block_counts[blockIdx.x] = c;
 }
 __global__ void __launch_bounds__(CMP_BLOCK) compact_write_kernel(const int32_t *__restrict__ ci, unsigned n,
                                                                   const unsigned *__restrict__ block_offsets,
                                                                   int32_t *out_pairs) {
-    __shared__ unsigned s_w[32];
     unsigned i = blockIdx.x * CMP_BLOCK + threadIdx.x;
     int32_t j = i < n ? ci[i] : -1;
     bool v = j >= 0;
-    unsigned m = __ballot_sync(CPHB_FULL, v);
-    if (lane_id() == 0) s_w[threadIdx.x >> 5] = __popc(m);
-    __syncthreads();
-    if (threadIdx.x < 32) {
-        unsigned ws = s_w[threadIdx.x], z = ws;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            unsigned y = __shfl_up_sync(CPHB_FULL, z, o);
-            if (lane_id() >= o) z += y;
-        }
-        s_w[threadIdx.x] = z - ws;
-    }
-    __syncthreads();
+    unsigned r = block_flag_rank(v);
     if (v) {
-        unsigned pos = block_offsets[blockIdx.x] + s_w[threadIdx.x >> 5] + __popc(m & ((1u << lane_id()) - 1u));
+        unsigned pos = block_offsets[blockIdx.x] + r;
         out_pairs[2 * (size_t)pos] = (int32_t)i;
         out_pairs[2 * (size_t)pos + 1] = j;
     }

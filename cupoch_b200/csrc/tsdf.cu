@@ -396,6 +396,17 @@ static int tsdf_flag_compact(const cphb_tsdf *v, int mode, cphb_scratch &sc, uin
     return cphb_compact_flags(*flags, v->n, *pos, m, s);
 }
 
+static int tsdf_scan(const unsigned long long *cnt, unsigned long long *off, size_t n, cphb_scratch &sc, cudaStream_t s) {
+    size_t tmp_bytes = 0;
+    CPHB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, cnt, off, (int64_t)n, s));
+    char *tmp = nullptr;
+    const int rc = sc.alloc(&tmp, tmp_bytes ? tmp_bytes : 16);
+    if (rc) return rc;
+    CPHB_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, cnt, off, (int64_t)n, s));
+    g_cphb_launches += 2;  // CUB's init and scan kernels
+    return CPHB_OK;
+}
+
 extern "C" int cphb_tsdf_extract_points(const cphb_tsdf *v, float *points, float *normals, float *colors, size_t capacity, size_t *h_count,
                                         void *stream) {
     cudaStream_t s = (cudaStream_t)stream;
@@ -416,13 +427,8 @@ extern "C" int cphb_tsdf_extract_points(const cphb_tsdf *v, float *points, float
     if (!rc) rc = sc.alloc(&off, m + 1);
     if (rc) return rc;
     CPHB_LAUNCH(tsdf_popc_kernel, tsdf_blocks(m + 1, 256), 256, 0, s, pos, m, flags, cnt);
-    size_t tmp_bytes = 0;
-    CPHB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, cnt, off, (int64_t)(m + 1), s));
-    char *tmp = nullptr;
-    rc = sc.alloc(&tmp, tmp_bytes ? tmp_bytes : 16);
+    rc = tsdf_scan(cnt, off, m + 1, sc, s);
     if (rc) return rc;
-    CPHB_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, cnt, off, (int64_t)(m + 1), s));
-    g_cphb_launches += 2;  // CUB's init and scan kernels
     unsigned long long total = 0;
     rc = cphb_read_back(&total, off + m, sizeof(unsigned long long), s, who);
     if (rc) return rc;
@@ -867,17 +873,6 @@ __global__ void __launch_bounds__(128) tsdf_mc_triangle_kernel(const int32_t *__
     }
 }
 
-static int tsdf_scan(const unsigned long long *cnt, unsigned long long *off, size_t n, cphb_scratch &sc, cudaStream_t s) {
-    size_t tmp_bytes = 0;
-    CPHB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, cnt, off, (int64_t)n, s));
-    char *tmp = nullptr;
-    const int rc = sc.alloc(&tmp, tmp_bytes ? tmp_bytes : 16);
-    if (rc) return rc;
-    CPHB_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, cnt, off, (int64_t)n, s));
-    g_cphb_launches += 2;  // CUB's init and scan kernels
-    return CPHB_OK;
-}
-
 extern "C" int cphb_tsdf_extract_mesh(const cphb_tsdf *v, float *vertices, float *colors, int32_t *triangles, size_t vertex_capacity,
                                       size_t triangle_capacity, size_t *h_n_vertices, size_t *h_n_triangles, void *stream) {
     cudaStream_t s = (cudaStream_t)stream;
@@ -1082,20 +1077,6 @@ __global__ void __launch_bounds__(128) tsdf_raycast_kernel(const float2 *__restr
     if (hit) hit[i] = ok ? 1 : 0;
 }
 
-__global__ void __launch_bounds__(256) tsdf_gather_rows_kernel(const int32_t *__restrict__ sel, size_t m, const float *__restrict__ a,
-                                                               const float *__restrict__ b, const float *__restrict__ c,
-                                                               float *__restrict__ oa, float *__restrict__ ob, float *__restrict__ oc) {
-    const size_t t = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
-    if (t >= m) return;
-    const size_t i = (size_t)sel[t];
-#pragma unroll
-    for (int k = 0; k < 3; ++k) {
-        oa[3 * t + k] = a[3 * i + k];
-        ob[3 * t + k] = b[3 * i + k];
-        oc[3 * t + k] = c[3 * i + k];
-    }
-}
-
 extern "C" int cphb_tsdf_raycast(const cphb_tsdf *v, int width, int height, const float h_intrinsic[9], const float h_extrinsic[16],
                                  float sdf_trunc, int project_valid_depth_only, float *points, float *normals, float *colors,
                                  size_t capacity, size_t *h_count, void *stream) {
@@ -1152,8 +1133,8 @@ extern "C" int cphb_tsdf_raycast(const cphb_tsdf *v, int width, int height, cons
     size_t m = npx;
     if (project_valid_depth_only) {  // RemoveNoneFinitePoints(true, true) (UT:948-949): the hit rows, in pixel order
         int rc = cphb_compact_flags(hit, npx, sel, &m, s);
+        if (!rc) rc = cphb_select_by_index(rp, rn, rc_, npx, sel, m, points, normals, colors, s);
         if (rc) return rc;
-        CPHB_LAUNCH(tsdf_gather_rows_kernel, tsdf_blocks(m, 256), 256, 0, s, sel, m, rp, rn, rc_, points, normals, colors);
     }
     const int rc = cphb_read_back(nullptr, nullptr, 0, s, who);
     if (!rc) *h_count = m;

@@ -243,81 +243,22 @@ __global__ void __launch_bounds__(256) voxel_dense_accum_kernel(const float *__r
 template <int A>
 __global__ void __launch_bounds__(VD_BLOCK) voxel_dense_count_kernel(const double *__restrict__ acc, size_t cells, unsigned *block_counts) {
     constexpr int S = dense_stride<A>();
-    __shared__ unsigned s_w[32];
     const size_t c = blockIdx.x * (size_t)VD_BLOCK + threadIdx.x;
-    const bool occ = c < cells && acc[c * S + (A == 1 ? 3 : A == 2 ? 6 : 9)] > 0.0;
-    const unsigned m = __ballot_sync(CPHB_FULL, occ);
-    if (lane_id() == 0) s_w[threadIdx.x >> 5] = __popc(m);
-    __syncthreads();
-    if (threadIdx.x < 32) {
-        unsigned v = s_w[threadIdx.x];
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(CPHB_FULL, v, o);
-        if (threadIdx.x == 0) block_counts[blockIdx.x] = v;
-    }
-}
-// exclusive scan of the block counts (one block; the grid has cells / 1024 entries), total to *total
-__global__ void __launch_bounds__(1024) voxel_dense_scan_kernel(unsigned *block_counts, unsigned nb, unsigned *total) {
-    __shared__ unsigned s_w[32];
-    __shared__ unsigned s_carry;
-    if (threadIdx.x == 0) s_carry = 0;
-    __syncthreads();
-    for (unsigned base = 0; base < nb; base += 1024) {
-        const unsigned i = base + threadIdx.x;
-        const unsigned v = i < nb ? block_counts[i] : 0u;
-        unsigned x = v;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const unsigned y = __shfl_up_sync(CPHB_FULL, x, o);
-            if (lane_id() >= o) x += y;
-        }
-        if (lane_id() == 31) s_w[threadIdx.x >> 5] = x;
-        __syncthreads();
-        if (threadIdx.x < 32) {
-            const unsigned ws = s_w[threadIdx.x];
-            unsigned z = ws;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const unsigned y = __shfl_up_sync(CPHB_FULL, z, o);
-                if (lane_id() >= o) z += y;
-            }
-            s_w[threadIdx.x] = z - ws;
-        }
-        __syncthreads();
-        const unsigned excl = x - v + s_w[threadIdx.x >> 5] + s_carry;
-        if (i < nb) block_counts[i] = excl;
-        __syncthreads();
-        if (threadIdx.x == 1023) s_carry = excl + v;
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) *total = s_carry;
+    const unsigned v = block_flag_count(c < cells && acc[c * S + (A == 1 ? 3 : A == 2 ? 6 : 9)] > 0.0);
+    if (threadIdx.x == 0) block_counts[blockIdx.x] = v;
 }
 template <int A>
 __global__ void __launch_bounds__(VD_BLOCK) voxel_dense_write_kernel(const double *__restrict__ acc, size_t cells,
                                                                      const unsigned *__restrict__ block_offsets, int a1_is_normal,
                                                                      float *out_p, float *out_a1, float *out_a2) {
     constexpr int S = dense_stride<A>();
-    __shared__ unsigned s_w[32];
     const size_t c = blockIdx.x * (size_t)VD_BLOCK + threadIdx.x;
     double cntd = 0.0;
     if (c < cells) cntd = acc[c * S + (A == 1 ? 3 : A == 2 ? 6 : 9)];
     const bool occ = cntd > 0.0;
-    const unsigned m = __ballot_sync(CPHB_FULL, occ);
-    if (lane_id() == 0) s_w[threadIdx.x >> 5] = __popc(m);
-    __syncthreads();
-    if (threadIdx.x < 32) {
-        const unsigned ws = s_w[threadIdx.x];
-        unsigned z = ws;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const unsigned y = __shfl_up_sync(CPHB_FULL, z, o);
-            if (lane_id() >= o) z += y;
-        }
-        s_w[threadIdx.x] = z - ws;
-    }
-    __syncthreads();
+    const unsigned r = block_flag_rank(occ);
     if (!occ) return;
-    const size_t pos = (size_t)block_offsets[blockIdx.x] + s_w[threadIdx.x >> 5] + __popc(m & ((1u << lane_id()) - 1u));
+    const size_t pos = (size_t)block_offsets[blockIdx.x] + r;
     const double *s = acc + c * S;
     const float cnt = (float)cntd;
     // divide_tuple_functor: x / (float)count
@@ -354,7 +295,7 @@ static int voxel_dense(const float *points, const float *a1, const float *a2, si
     CPHB_CUDA(cudaMemsetAsync(acc, 0, sizeof(double) * S * cells, s));
     CPHB_LAUNCH(voxel_dense_accum_kernel<A>, (unsigned)((n + 1023) / 1024), 256, 0, s, points, a1, a2, n, g, acc);
     CPHB_LAUNCH(voxel_dense_count_kernel<A>, nb, VD_BLOCK, 0, s, acc, cells, bc);
-    CPHB_LAUNCH(voxel_dense_scan_kernel, 1, 1024, 0, s, bc, nb, total);
+    cphb_scan_block_counts(bc, nb, total, s);
     CPHB_LAUNCH(voxel_dense_write_kernel<A>, nb, VD_BLOCK, 0, s, acc, cells, bc, a1_is_normal, out_p, out_a1, out_a2);
     CPHB_CHECK_LAUNCH();
     unsigned h = 0;

@@ -112,6 +112,18 @@ _SIGNATURES = {
     "cphb_tsdf_extract_mesh": (C.c_int, [_P, _P, _P, _P, C.c_size_t, C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t), _P]),
     "cphb_mesh_triangle_normals": (C.c_int, [_P, C.c_size_t, _P, C.c_size_t, C.c_int, _P, _P]),
     "cphb_mesh_vertex_normals": (C.c_int, [_P, C.c_size_t, _P, C.c_size_t, C.c_int, _P, _P]),
+    "cphb_stsdf_create": (C.c_int, [C.c_float, C.c_float, C.c_int, C.c_int, C.c_int, _P, C.POINTER(_P)]),
+    "cphb_stsdf_destroy": (None, [_P]),
+    "cphb_stsdf_reset": (C.c_int, [_P, _P]),
+    "cphb_stsdf_integrate": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                       C.c_int, _F3, _F3, _P]),
+    "cphb_stsdf_extract_points": (C.c_int, [_P, _P, _P, _P, C.c_size_t, C.POINTER(C.c_size_t), _P]),
+    "cphb_stsdf_extract_voxels": (C.c_int, [_P, _P, _P, C.c_size_t, C.POINTER(C.c_size_t), _P]),
+    "cphb_stsdf_data": (C.c_int, [_P, C.POINTER(C.c_size_t), C.POINTER(_P), C.POINTER(_P), C.POINTER(_P)]),
+    "cphb_stsdf_info": (C.c_int, [_P, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]),
+    "cphb_depth_to_points": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_int, _P, C.c_int, C.c_int,
+                                       C.c_int, C.c_int, _F3, _F3, C.c_float, C.c_int, C.c_int, _P, _P, _P, C.c_size_t,
+                                       C.POINTER(C.c_size_t), _P]),
     # name: (restype, argtypes)
     "cphb_version": (C.c_int, []),
     "cphb_last_error": (C.c_char_p, []),

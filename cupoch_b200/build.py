@@ -21,14 +21,14 @@ OBJ = os.path.join(SRC, "_build")
 LIB = os.path.join(HERE, "lib", "libcupoch_b200.so")
 SOURCES = ["index.cu", "sort.cu", "search.cu", "icp.cu", "voxel.cu", "features.cu", "filters.cu", "voxelgrid.cu", "comm.cu",
            "reduce.cu", "fpfh.cu", "cluster.cu", "occgrid.cu", "segment.cu", "fps.cu", "iss.cu", "edt.cu", "shot.cu",
-           "crop.cu", "collision.cu", "tsdf.cu", "mesh.cu"]
+           "crop.cu", "collision.cu", "tsdf.cu", "mesh.cu", "depth_cloud.cu", "stsdf.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-fmad=false",
          "-Xcompiler", "-fPIC", "-I" + os.path.join(ROOT, "include"), "-I" + SRC]
 
 
 HEADERS = ["cphb_internal.cuh", "cphb_searchk.cuh", "fused_neighbourhood.cuh", "cphb_eigen3.cuh", "icp_types.cuh", "icp_solve.cuh", "icp_rows.cuh", "icp_kernels.cuh",
-           "icp_estimate.cuh", "icp_aux.cuh", "voxelkey.cuh"]
+           "icp_estimate.cuh", "icp_aux.cuh", "voxelkey.cuh", "depth_project.cuh", "tsdf_update.cuh"]
 MANIFEST = os.path.join(OBJ, "manifest.json")
 
 

@@ -16,11 +16,8 @@
 #include <cub/device/device_scan.cuh>
 #include <memory>
 
-#include "cphb_internal.cuh"
+#include "tsdf_update.cuh"
 
-#define TSDF_NO_COLOR 0
-#define TSDF_RGB8 1
-#define TSDF_GRAY32 2
 #define TSDF_MAX_RES 1290  // res^3 <= 2^31 - 1: cphb_compact_flags writes int32 positions
 
 struct cphb_tsdf {
@@ -163,13 +160,6 @@ extern "C" int cphb_tsdf_data(const cphb_tsdf *v, float **tw, float **col) {
 }
 
 // ------------------------------------------------------------------------------------------------ Integrate
-struct TsdfCam {
-    float E[12];  // world-to-camera rows 0..2
-    float S[3];   // vl * E[r][2]
-    float fx, fy, cx, cy, fxi, fyi, safe_w, safe_h;
-    int w;
-};
-
 // uniform_integrate_functor (IF:84-139, 182-190); the expression order is oracle/tsdf.c's Integrate
 template <int CT>
 __global__ void __launch_bounds__(256) tsdf_integrate_kernel(float2 *__restrict__ tw, float *__restrict__ col, size_t n, int res, int h,
@@ -183,35 +173,9 @@ __global__ void __launch_bounds__(256) tsdf_integrate_kernel(float2 *__restrict_
     const float p2 = half + oz;
     const float kz = (float)(z - h);
     float cam[3];
-#pragma unroll
-    for (int r = 0; r < 3; ++r) {
-        const float b = __fmaf_rn(c.E[4 * r + 2], p2, __fmaf_rn(c.E[4 * r + 1], p1, c.E[4 * r] * p0)) + c.E[4 * r + 3];
-        cam[r] = __fmaf_rn(kz, c.S[r], b);
-    }
-    if (cam[2] <= 0.f) return;
-    const float uf = (cam[0] * c.fx) / cam[2] + c.cx + 0.5f;
-    const float vf = (cam[1] * c.fy) / cam[2] + c.cy + 0.5f;
-    if (!(uf >= 0.0001f && uf < c.safe_w && vf >= 0.0001f && vf < c.safe_h)) return;
-    const int u = __float2int_rd(uf), v = __float2int_rd(vf);
-    const size_t px = (size_t)v * c.w + u;
-    const float d = __ldg(depth + px);
-    if (d <= 0.f) return;
-    // the depth-to-camera-distance multiplier of pixel (u, v) (IFC:136-164), computed here instead of read from an image
-    const float xx = ((float)u - c.cx) * c.fxi, yy = ((float)v - c.cy) * c.fyi;
-    const float sdf = (d - cam[2]) * sqrtf(__fmaf_rn(yy, yy, xx * xx) + 1.0f);
-    if (!(sdf > -trunc)) return;
-    const float t = fminf(1.0f, sdf * trunc_inv);
+    tsdf_camera_point(c, p0, p1, p2, kz, cam);
     const size_t i = tsdf_idx(x, y, z, res);
-    const float2 cur = tw[i];
-    const float w1 = cur.y + 1.0f;
-    tw[i] = make_float2(__fmaf_rn(cur.x, cur.y, t) / w1, w1);
-    if (CT == TSDF_RGB8) {
-        const uint8_t *rgb = (const uint8_t *)color + 3 * px;
-#pragma unroll
-        for (int k = 0; k < 3; ++k) col[k * n + i] = __fmaf_rn(col[k * n + i], cur.y, (float)__ldg(rgb + k)) / w1;
-    } else if (CT == TSDF_GRAY32) {
-        col[i] = __fmaf_rn(col[i], cur.y, __ldg((const float *)color + px)) / w1;
-    }
+    tsdf_update_voxel<CT>(c, cam, depth, color, trunc, trunc_inv, tw + i, col + i, n);
 }
 
 // the reference's format checks (UT:677-695) and this project's: the depth image must match the intrinsic too
@@ -222,27 +186,12 @@ extern "C" int cphb_tsdf_integrate(cphb_tsdf *v, const float *depth, int depth_w
     cudaStream_t s = (cudaStream_t)stream;
     const char *who = "cphb_tsdf_integrate";
     if (!v || !h_intrinsic || !h_extrinsic) return tsdf_invalid(who, "null argument");
-    const bool bad = depth_channels != 1 || depth_bytes_per_channel != 4 || depth_width != width || depth_height != height ||
-                     (v->ct == TSDF_RGB8 && (color_channels != 3 || color_bytes_per_channel != 1)) ||
-                     (v->ct == TSDF_GRAY32 && (color_channels != 1 || color_bytes_per_channel != 4)) ||
-                     (v->ct != TSDF_NO_COLOR && (color_width != width || color_height != height));
+    const bool bad = tsdf_bad_format(v->ct, depth_width, depth_height, depth_channels, depth_bytes_per_channel, color_width, color_height,
+                                     color_channels, color_bytes_per_channel, width, height);
     if (bad) return tsdf_invalid(who, "[UniformTSDFVolume::Integrate] Unsupported image format.");
     if (width <= 0 || height <= 0) return tsdf_invalid(who, "the intrinsic's image size is not positive");
     if (!depth || (v->ct != TSDF_NO_COLOR && !color)) return tsdf_invalid(who, "null image");
-    TsdfCam c;
-    for (int r = 0; r < 3; ++r) {
-        for (int q = 0; q < 4; ++q) c.E[4 * r + q] = h_extrinsic[4 * r + q];
-        c.S[r] = v->vl * h_extrinsic[4 * r + 2];  // extrinsic_scaled_ = voxel_length * extrinsic (IF:53)
-    }
-    c.fx = h_intrinsic[0];
-    c.fy = h_intrinsic[4];
-    c.cx = h_intrinsic[2];
-    c.cy = h_intrinsic[5];
-    c.fxi = 1.0f / c.fx;
-    c.fyi = 1.0f / c.fy;
-    c.safe_w = (float)width - 0.0001f;  // UT:906-907
-    c.safe_h = (float)height - 0.0001f;
-    c.w = width;
+    const TsdfCam c = tsdf_cam(v->vl, h_intrinsic, h_extrinsic, width, height);
     const dim3 g = tsdf_vox_grid(v->res);
 #define TSDF_INTEGRATE(CT)                                                                                                        \
     CPHB_LAUNCH(tsdf_integrate_kernel<CT>, g, TSDF_VOX_BLOCK, 0, s, v->tw, v->col, v->n, v->res, v->h, v->vl, v->half, v->o[0], v->o[1], \

@@ -431,6 +431,54 @@ class PointCloud:
             out._points, out._colors = pts, cols
         return out
 
+    @staticmethod
+    def _from_depth(d_depth, d_color, intrinsic, extrinsic, depth_scale, depth_trunc, stride, depth_cutoff, compute_normals,
+                    valid_only):
+        """cphb_depth_to_points into width / stride x height / stride rows; the rows kept are views of the first m"""
+        w, h, dch, dbytes = RGBDImage._info(d_depth)
+        cw, chh, cch, cbytes = RGBDImage._info(d_color) if d_color is not None else (0, 0, 0, 0)
+        stride = int(stride)
+        n = (w // stride) * (h // stride) if stride >= 1 else 0
+        outs = [DeviceArray((n, 3), np.float32) if n and want else None
+                for want in (True, compute_normals, d_color is not None)]
+        m = C.c_size_t(0)
+        _lib.check(_lib.lib().cphb_depth_to_points(
+            d_depth.ptr, w, h, dch, dbytes, float(depth_scale), float(depth_trunc), stride,
+            d_color.ptr if d_color is not None else None, cw, chh, cch, cbytes, _floats(intrinsic.intrinsic_matrix, 9),
+            _floats(extrinsic, 16), float(depth_cutoff), int(bool(compute_normals)), int(bool(valid_only)),
+            *[o.ptr if o is not None else None for o in outs], n, C.byref(m), None))
+        out = PointCloud()
+        if m.value:
+            out._points, out._normals, out._colors = [None if o is None else o if m.value == n else
+                                                      DeviceArray((m.value, 3), np.float32, ptr=o.ptr, base=o) for o in outs]
+        return out
+
+    @staticmethod
+    def create_from_depth_image(depth, intrinsic, extrinsic=np.eye(4), depth_scale=1000.0, depth_trunc=1000.0, stride=1):
+        """PointCloud::CreateFromDepthImage (pointcloud_factory.cu:43-105, 329-350): the point of every stride-th pixel
+        of every stride-th row whose depth is > 0, in pixel order, in the world frame of the world-to-camera extrinsic.
+        depth: a 1-channel uint16 geometry.Image (raw / int(depth_scale), 0 where that is >= int(depth_trunc)) or
+        float32 one (metres, as it is).  Another format, stride < 1 or a singular extrinsic raises."""
+        if depth.num_of_channels != 1 or depth.bytes_per_channel not in (2, 4):
+            raise ValueError("[PointCloud::CreateFromDepthImage] Unsupported image format.")
+        d = DeviceArray.from_numpy(depth._data.reshape(depth.height, depth.width), depth._data.dtype)
+        return PointCloud._from_depth(d, None, intrinsic, extrinsic, depth_scale, depth_trunc, stride, -1.0, False, True)
+
+    @staticmethod
+    def create_from_rgbd_image(image, intrinsic, extrinsic=np.eye(4), project_valid_depth_only=True, depth_cutoff=-1.0,
+                               compute_normals=False):
+        """PointCloud::CreateFromRGBDImage (pointcloud_factory.cu:107-200, 288-327, 352-373), from the device images the
+        RGBDImage holds: a point and colour per pixel whose depth is > 0 (and < depth_cutoff when that is > 0).  The
+        colour image is uint8 RGB (c / 255) or 1-channel float32 intensity (g -> (g, g, g)); another format raises.
+        compute_normals: structured normals from the four neighbouring pixels (0 on the border rows and columns),
+        turned towards the camera (z <= 0).  project_valid_depth_only=False: one row per pixel, NaN where there is no
+        point."""
+        d_color, d_depth = image._device()
+        if RGBDImage._info(d_depth)[2:] != (1, 4):
+            raise ValueError("[PointCloud::CreateFromRGBDImage] the depth image must be 1-channel float32")
+        return PointCloud._from_depth(d_depth, d_color, intrinsic, extrinsic, 1000.0, 1000.0, 1, depth_cutoff, compute_normals,
+                                      project_valid_depth_only)
+
     def normalize_normals(self):
         """NormalizeNormals (pointcloud.cu:282-285), in place: every non-zero normal divided by its length"""
         if self._normals is not None and len(self._normals):
@@ -521,6 +569,10 @@ class TriangleMesh:
                                                            out.ptr, None))
         self._vertex_normals = out
         return self
+
+
+def _floats(a, n):
+    return (C.c_float * n)(*np.asarray(a, np.float32).reshape(n).tolist())
 
 
 def _vector3i(a):

@@ -1,4 +1,5 @@
-"""cupoch.integration mirror: UniformTSDFVolume (integration/uniform_tsdfvolume.h; pybind integration/integration.cpp).
+"""cupoch.integration mirror: UniformTSDFVolume and ScalableTSDFVolume (integration/{uniform,scalable}_tsdfvolume.h;
+pybind integration/integration.cpp).
 
 The volume is a dense resolution^3 grid on the device, owned by a csrc/tsdf.cu handle: a {tsdf, weight} float pair per
 voxel and colour planes only when the volume has colour.  Every operation runs there; nothing falls back to the CPU.
@@ -159,6 +160,105 @@ class UniformTSDFVolume:
                 outs = [_copy_rows(o, m) for o in outs]
             pc._points, pc._normals, pc._colors = outs
         return pc
+
+
+class ScalableTSDFVolume:
+    """integration::ScalableTSDFVolume(voxel_length, sdf_trunc, color_type, depth_sampling_stride = 4, map_size = 1000):
+    16^3-voxel units, unit length voxel_length * 16, allocated on the device near the surfaces each frame observes.
+    map_size is the first capacity of the unit pool, which doubles as needed; it changes no result."""
+
+    def __init__(self, voxel_length, sdf_trunc, color_type, depth_sampling_stride=4, map_size=1000):
+        _lib.require_gpu()
+        self._h = C.c_void_p()
+        self._voxel_length, self._sdf_trunc = float(np.float32(voxel_length)), float(np.float32(sdf_trunc))
+        self._color_type, self._stride = TSDFVolumeColorType(color_type), int(depth_sampling_stride)
+        _lib.check(_lib.lib().cphb_stsdf_create(self._voxel_length, self._sdf_trunc, int(self._color_type), self._stride,
+                                                int(map_size), None, C.byref(self._h)))
+
+    voxel_length = property(lambda s: s._voxel_length)
+    sdf_trunc = property(lambda s: s._sdf_trunc)
+    color_type = property(lambda s: s._color_type)
+    depth_sampling_stride = property(lambda s: s._stride)
+    volume_unit_length = property(lambda s: float(np.float32(s._voxel_length) * np.float32(16)))
+
+    def __repr__(self):
+        return "integration::ScalableTSDFVolume " + ("without color." if self._color_type == TSDFVolumeColorType.NoColor
+                                                    else "with color.")
+
+    def __del__(self):
+        try:
+            if self._h:
+                _lib.lib().cphb_stream_synchronize(None)
+                _lib.lib().cphb_stsdf_destroy(self._h)
+                self._h = None
+        except Exception:
+            pass
+
+    def reset(self):
+        """Reset: no unit is allocated"""
+        _lib.check(_lib.lib().cphb_stsdf_reset(self._h, None))
+        _lib.check(_lib.lib().cphb_stream_synchronize(None))
+
+    def integrate(self, image, intrinsic, extrinsic):
+        """Integrate(RGBDImage, intrinsic, extrinsic) (scalable_tsdfvolume.cu:311-343): allocates the units within
+        sdf_trunc of the frame's strided depth points, then updates every allocated voxel.  The image rules of
+        UniformTSDFVolume.integrate; a unit key outside [-2^20, 2^20) or a singular extrinsic raises, and a frame that
+        raises leaves the volume unchanged."""
+        d_color, d_depth = image._device()
+        dep, col = image._depth_info(), image._color_info()
+        _lib.check(_lib.lib().cphb_stsdf_integrate(self._h, d_depth.ptr, *dep, d_color.ptr, *col, int(intrinsic.width),
+                                                   int(intrinsic.height), _m(intrinsic.intrinsic_matrix, 9), _m(extrinsic, 16), None))
+
+    def info(self):
+        """(allocated units, pool capacity in units, device bytes of the pool and its table)"""
+        u, c, b = C.c_size_t(0), C.c_size_t(0), C.c_size_t(0)
+        _lib.check(_lib.lib().cphb_stsdf_info(self._h, C.byref(u), C.byref(c), C.byref(b)))
+        return u.value, c.value, b.value
+
+    def units(self):
+        """the device state as borrowed views: (keys [units] uint64 packed, tw [units, 4096, 2] float32, col [units,
+        planes, 4096] float32 or None); key axis a = ((key >> (42 - 21 a)) & (2^21 - 1)) - 2^20"""
+        n, keys, tw, col = C.c_size_t(0), C.c_void_p(), C.c_void_p(), C.c_void_p()
+        _lib.check(_lib.lib().cphb_stsdf_data(self._h, C.byref(n), C.byref(keys), C.byref(tw), C.byref(col)))
+        u = n.value
+        if not u:
+            return np.zeros(0, np.uint64), np.zeros((0, 4096, 2), np.float32), None
+        planes = {TSDFVolumeColorType.NoColor: 0, TSDFVolumeColorType.RGB8: 3, TSDFVolumeColorType.Gray32: 1}[self._color_type]
+        return (DeviceArray((u,), np.uint64, ptr=keys.value, base=self), DeviceArray((u, 4096, 2), np.float32, ptr=tw.value, base=self),
+                DeviceArray((u, planes, 4096), np.float32, ptr=col.value, base=self) if planes else None)
+
+    def extract_point_cloud(self):
+        """ExtractPointCloud (scalable_tsdfvolume.cu:125-290, 345-366): a point, normal and (with colour) colour per zero
+        crossing between a band voxel and its +1 neighbour, across unit faces, in (unit, voxel, axis) order"""
+        L = _lib.lib()
+        has_c = self._color_type != TSDFVolumeColorType.NoColor
+        n = C.c_size_t(0)
+        _lib.check(L.cphb_stsdf_extract_points(self._h, None, None, None, 0, C.byref(n), None))
+        pc = PointCloud()
+        m = n.value
+        if m:
+            p, nr = DeviceArray((m, 3), np.float32), DeviceArray((m, 3), np.float32)
+            c = DeviceArray((m, 3), np.float32) if has_c else None
+            _lib.check(L.cphb_stsdf_extract_points(self._h, p.ptr, nr.ptr, c.ptr if c is not None else None, m, C.byref(n), None))
+            pc._points, pc._normals, pc._colors = p, nr, c
+        return pc
+
+    def extract_voxel_point_cloud(self):
+        """ExtractVoxelPointCloud: the centre of every band voxel, coloured (tsdf + 1) / 2, in (unit, voxel) order"""
+        L = _lib.lib()
+        n = C.c_size_t(0)
+        _lib.check(L.cphb_stsdf_extract_voxels(self._h, None, None, 0, C.byref(n), None))
+        pc = PointCloud()
+        m = n.value
+        if m:
+            p, c = DeviceArray((m, 3), np.float32), DeviceArray((m, 3), np.float32)
+            _lib.check(L.cphb_stsdf_extract_voxels(self._h, p.ptr, c.ptr, m, C.byref(n), None))
+            pc._points, pc._colors = p, c
+        return pc
+
+    def extract_triangle_mesh(self):
+        """not implemented, as in the reference (scalable_tsdfvolume.cu:375-381)"""
+        raise NotImplementedError("ScalableTSDFVolume::ExtractTriangleMesh is not implemented")
 
 
 def _copy_rows(a, m):

@@ -484,11 +484,28 @@ inline OrientedBoundingBox OrientedBoundingBox::CreateFromAxisAlignedBoundingBox
 
 /// geometry::PointCloud (pointcloud.h:43-263), hot-path subset.
 class OccupancyGrid;
+class Image;
+class RGBDImage;
 class PointCloud {
 public:
     PointCloud() {}
     /// PointCloud::CreateFromOccupancyGrid (pointcloud_factory.cu:418-430), defined after OccupancyGrid
     static std::shared_ptr<PointCloud> CreateFromOccupancyGrid(const OccupancyGrid &occgrid);
+    /// PointCloud::CreateFromDepthImage (pointcloud_factory.cu:43-105, 329-350), defined after RGBDImage: the point of
+    /// every stride-th pixel of every stride-th row with depth > 0, in pixel order.  depth: 1-channel uint16 (raw /
+    /// int(depth_scale), 0 where that is >= int(depth_trunc)) or float32 metres; another format, stride < 1 or a
+    /// singular extrinsic throws.
+    static std::shared_ptr<PointCloud> CreateFromDepthImage(const Image &depth, const camera::PinholeCameraIntrinsic &intrinsic,
+                                                            const Eigen::Matrix4f &extrinsic = Eigen::Matrix4f::Identity(),
+                                                            float depth_scale = 1000.0f, float depth_trunc = 1000.0f, int stride = 1);
+    /// PointCloud::CreateFromRGBDImage (pointcloud_factory.cu:107-200, 352-373), defined after RGBDImage: a point and
+    /// colour (RGB8 c / 255, Gray32 (g, g, g)) per pixel with depth > 0 (and < depth_cutoff when that is > 0);
+    /// compute_normals gives structured normals (0 on the border rows and columns); project_valid_depth_only = false
+    /// keeps one row per pixel, NaN where there is no point.
+    static std::shared_ptr<PointCloud> CreateFromRGBDImage(const RGBDImage &image, const camera::PinholeCameraIntrinsic &intrinsic,
+                                                           const Eigen::Matrix4f &extrinsic = Eigen::Matrix4f::Identity(),
+                                                           bool project_valid_depth_only = true, float depth_cutoff = -1.0f,
+                                                           bool compute_normals = false);
     PointCloud(const std::vector<Eigen::Vector3f> &points) : points_(points) {}
     virtual ~PointCloud() {}
     bool IsEmpty() const { return points_.empty(); }
@@ -1908,6 +1925,47 @@ private:
         utility::check(cphb_stream_synchronize(nullptr));
     }
 };
+
+namespace detail {
+/// cphb_depth_to_points into width / stride x height / stride rows, shrunk to the rows kept
+inline std::shared_ptr<PointCloud> depth_to_points(const Image &d, const Image *c, const camera::PinholeCameraIntrinsic &intrinsic,
+                                                   const Eigen::Matrix4f &extrinsic, float depth_scale, float depth_trunc, int stride,
+                                                   float depth_cutoff, bool normals, bool valid_only) {
+    float K[9], E[16];
+    for (int r = 0; r < 3; ++r)
+        for (int q = 0; q < 3; ++q) K[3 * r + q] = intrinsic.intrinsic_matrix_(r, q);
+    utility::to_row_major(extrinsic, E);
+    const size_t n = stride >= 1 ? (size_t)std::max(d.width_ / stride, 0) * (size_t)std::max(d.height_ / stride, 0) : 0;
+    auto pc = std::make_shared<PointCloud>();
+    pc->points_.resize(n);
+    if (normals) pc->normals_.resize(n);
+    if (c) pc->colors_.resize(n);
+    size_t m = 0;
+    utility::check(cphb_depth_to_points(d.data_.data(), d.width_, d.height_, d.num_of_channels_, d.bytes_per_channel_, depth_scale, depth_trunc,
+                                        stride, c ? c->data_.data() : nullptr, c ? c->width_ : 0, c ? c->height_ : 0,
+                                        c ? c->num_of_channels_ : 0, c ? c->bytes_per_channel_ : 0, K, E, depth_cutoff, normals ? 1 : 0,
+                                        valid_only ? 1 : 0, (float *)pc->points_.data(), normals ? (float *)pc->normals_.data() : nullptr,
+                                        c ? (float *)pc->colors_.data() : nullptr, n, &m, nullptr));
+    pc->points_.resize(m);
+    if (normals) pc->normals_.resize(m);
+    if (c) pc->colors_.resize(m);
+    return pc;
+}
+}  // namespace detail
+
+inline std::shared_ptr<PointCloud> PointCloud::CreateFromDepthImage(const Image &depth, const camera::PinholeCameraIntrinsic &intrinsic,
+                                                                    const Eigen::Matrix4f &extrinsic, float depth_scale, float depth_trunc,
+                                                                    int stride) {
+    return detail::depth_to_points(depth, nullptr, intrinsic, extrinsic, depth_scale, depth_trunc, stride, -1.0f, false, true);
+}
+inline std::shared_ptr<PointCloud> PointCloud::CreateFromRGBDImage(const RGBDImage &image, const camera::PinholeCameraIntrinsic &intrinsic,
+                                                                   const Eigen::Matrix4f &extrinsic, bool project_valid_depth_only,
+                                                                   float depth_cutoff, bool compute_normals) {
+    if (image.depth_.num_of_channels_ != 1 || image.depth_.bytes_per_channel_ != 4)
+        throw std::runtime_error("[PointCloud::CreateFromRGBDImage] the depth image must be 1-channel float32");
+    return detail::depth_to_points(image.depth_, &image.color_, intrinsic, extrinsic, 1000.0f, 1000.0f, 1, depth_cutoff, compute_normals,
+                                   project_valid_depth_only);
+}
 }  // namespace geometry
 
 namespace geometry {
@@ -2107,6 +2165,87 @@ private:
             for (int c = 0; c < 3; ++c) K[3 * r + c] = in.intrinsic_matrix_(r, c);
     }
     cphb_tsdf *h_ = nullptr;
+};
+
+/// integration::ScalableTSDFVolume (scalable_tsdfvolume.h): 16^3-voxel units allocated on the device near observed
+/// surfaces, owned by a cphb_stsdf handle.  map_size is the first capacity of the unit pool, which doubles as needed.
+/// Argument errors, a rejected frame (which leaves the volume unchanged) and ExtractTriangleMesh (not implemented, as
+/// in the reference) throw.  Not copyable.
+class ScalableTSDFVolume : public TSDFVolume {
+public:
+    ScalableTSDFVolume(float voxel_length, float sdf_trunc, TSDFVolumeColorType color_type, int depth_sampling_stride = 4,
+                       int map_size = 1000)
+        : TSDFVolume(voxel_length, sdf_trunc, color_type), volume_unit_length_(voxel_length * 16.0f),
+          depth_sampling_stride_(depth_sampling_stride) {
+        utility::check(cphb_stsdf_create(voxel_length, sdf_trunc, (int)color_type, depth_sampling_stride, map_size, nullptr, &h_));
+    }
+    ScalableTSDFVolume(const ScalableTSDFVolume &) = delete;
+    ScalableTSDFVolume &operator=(const ScalableTSDFVolume &) = delete;
+    ~ScalableTSDFVolume() override {
+        if (h_) {
+            cphb_stream_synchronize(nullptr);
+            cphb_stsdf_destroy(h_);
+        }
+    }
+    void Reset() {
+        utility::check(cphb_stsdf_reset(h_, nullptr));
+        utility::check(cphb_stream_synchronize(nullptr));
+    }
+    /// Integrate (scalable_tsdfvolume.cu:311-343); extrinsic is world-to-camera
+    void Integrate(const geometry::RGBDImage &image, const camera::PinholeCameraIntrinsic &intrinsic, const Eigen::Matrix4f &extrinsic) {
+        float K[9], E[16];
+        for (int r = 0; r < 3; ++r)
+            for (int c = 0; c < 3; ++c) K[3 * r + c] = intrinsic.intrinsic_matrix_(r, c);
+        utility::to_row_major(extrinsic, E);
+        const geometry::Image &d = image.depth_, &c = image.color_;
+        utility::check(cphb_stsdf_integrate(h_, reinterpret_cast<const float *>(d.data_.data()), d.width_, d.height_, d.num_of_channels_,
+                                            d.bytes_per_channel_, c.data_.data(), c.width_, c.height_, c.num_of_channels_,
+                                            c.bytes_per_channel_, intrinsic.width_, intrinsic.height_, K, E, nullptr));
+    }
+    /// ExtractPointCloud (scalable_tsdfvolume.cu:345-366): points, normals and (with colour) colours of the crossings
+    std::shared_ptr<geometry::PointCloud> ExtractPointCloud() {
+        auto pc = std::make_shared<geometry::PointCloud>();
+        const bool has_c = color_type_ != TSDFVolumeColorType::NoColor;
+        size_t n = 0;
+        utility::check(cphb_stsdf_extract_points(h_, nullptr, nullptr, nullptr, 0, &n, nullptr));
+        if (n) {
+            pc->points_.resize(n);
+            pc->normals_.resize(n);
+            if (has_c) pc->colors_.resize(n);
+            utility::check(cphb_stsdf_extract_points(h_, (float *)pc->points_.data(), (float *)pc->normals_.data(),
+                                                     has_c ? (float *)pc->colors_.data() : nullptr, n, &n, nullptr));
+        }
+        return pc;
+    }
+    /// ExtractVoxelPointCloud: band voxel centres coloured (tsdf + 1) / 2
+    std::shared_ptr<geometry::PointCloud> ExtractVoxelPointCloud() const {
+        auto pc = std::make_shared<geometry::PointCloud>();
+        size_t n = 0;
+        utility::check(cphb_stsdf_extract_voxels(h_, nullptr, nullptr, 0, &n, nullptr));
+        if (n) {
+            pc->points_.resize(n);
+            pc->colors_.resize(n);
+            utility::check(cphb_stsdf_extract_voxels(h_, (float *)pc->points_.data(), (float *)pc->colors_.data(), n, &n, nullptr));
+        }
+        return pc;
+    }
+    /// not implemented, as in the reference (scalable_tsdfvolume.cu:375-381)
+    std::shared_ptr<geometry::TriangleMesh> ExtractTriangleMesh() override {
+        throw std::runtime_error("ScalableTSDFVolume::ExtractTriangleMesh is not implemented");
+    }
+    /// the number of allocated units
+    size_t UnitCount() const {
+        size_t u = 0, cap = 0, bytes = 0;
+        utility::check(cphb_stsdf_info(h_, &u, &cap, &bytes));
+        return u;
+    }
+
+public:
+    float volume_unit_length_;
+    int depth_sampling_stride_;
+
+private:
+    cphb_stsdf *h_ = nullptr;
 };
 }  // namespace integration
 }  // namespace cupoch

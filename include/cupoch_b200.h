@@ -594,6 +594,45 @@ int cphb_tsdf_extract_mesh(const cphb_tsdf *volume, float *vertices, float *colo
                            size_t triangle_capacity, size_t *h_n_vertices, size_t *h_n_triangles, void *stream);
 
 /* ------------------------------------------------------------------------ *
+ * integration::ScalableTSDFVolume (integration/scalable_tsdfvolume.cu): 16^3-voxel units allocated on demand near
+ * observed surfaces.  Unit key floor(p / U), U = voxel_length * 16, each axis in [-2^20, 2^20).  Voxel (x, y, z) of the
+ * unit with key k has the centre fma(vl, (x, y, z), vl / 2) + k * U and index x * 256 + y * 16 + z in its slot.  Units
+ * are kept in slots in the order the frames first touched them, ascending key within a frame (the packed key: each
+ * axis + 2^20 in 21 bits, x highest); the extractions go in slot order, voxel index, axis.  map_size is the pool's
+ * first capacity, which doubles as needed.  Conventions as cphb_tsdf_*.
+ * ------------------------------------------------------------------------ */
+typedef struct cphb_stsdf cphb_stsdf;
+/* ScalableTSDFVolume(voxel_length, sdf_trunc, color_type, depth_sampling_stride, map_size).  A voxel_length or
+ * sdf_trunc that is not positive and finite, sdf_trunc over 64 units, an unknown color_type, a stride or map_size
+ * below 1: CPHB_ERR_INVALID. */
+int cphb_stsdf_create(float voxel_length, float sdf_trunc, int color_type, int depth_sampling_stride, int map_size, void *stream,
+                      cphb_stsdf **out);
+void cphb_stsdf_destroy(cphb_stsdf *volume);
+/* Reset: no unit allocated.  Asynchronous. */
+int cphb_stsdf_reset(cphb_stsdf *volume, void *stream);
+/* Integrate(RGBDImage, intrinsic, extrinsic): the units within sdf_trunc of the frame's strided depth points
+ * (cphb_depth_to_points' projection, every depth_sampling_stride-th pixel) are allocated, then every allocated voxel
+ * is updated as cphb_tsdf_integrate updates a voxel.  The image rules of cphb_tsdf_integrate; a singular extrinsic, a
+ * unit key out of range or more than 524287 units (the voxel count must fit int32) is CPHB_ERR_INVALID, and a failed
+ * allocation CPHB_ERR_CUDA; a call that fails leaves the volume as it was.  Synchronises. */
+int cphb_stsdf_integrate(cphb_stsdf *volume, const float *depth, int depth_width, int depth_height, int depth_channels,
+                         int depth_bytes_per_channel, const void *color, int color_width, int color_height, int color_channels,
+                         int color_bytes_per_channel, int width, int height, const float h_intrinsic[9], const float h_extrinsic[16],
+                         void *stream);
+/* ExtractPointCloud: one row per zero crossing between a band voxel and its +1 neighbour on an axis (across unit
+ * faces; a missing unit counts as weight 0); points, normals (GetNormalAt) and, unless NoColor, colours.  Sizing as
+ * cphb_tsdf_extract_points.  Synchronises. */
+int cphb_stsdf_extract_points(const cphb_stsdf *volume, float *points, float *normals, float *colors, size_t capacity, size_t *h_count,
+                              void *stream);
+/* ExtractVoxelPointCloud: every band voxel's centre, colour (tsdf + 1) / 2.  Sizing as above.  Synchronises. */
+int cphb_stsdf_extract_voxels(const cphb_stsdf *volume, float *points, float *colors, size_t capacity, size_t *h_count, void *stream);
+/* borrowed device state: the unit count, keys [units] packed, tw [units][4096][2] float32 and col
+ * [units][planes][4096] float32 (NULL for NoColor) */
+int cphb_stsdf_data(const cphb_stsdf *volume, size_t *h_units, uint64_t **keys, float **tw, float **col);
+/* the unit count, the pool's capacity in units and the device bytes of the pool and its table */
+int cphb_stsdf_info(const cphb_stsdf *volume, size_t *h_units, size_t *h_capacity, size_t *h_device_bytes);
+
+/* ------------------------------------------------------------------------ *
  * TriangleMesh normals (geometry/trianglemesh.cu), on device arrays: vertices [n_vertices][3] float32, triangles
  * [n_triangles][3] int32.  A vertex index outside [0, n_vertices) is CPHB_ERR_INVALID.  Synchronise.
  * ------------------------------------------------------------------------ */
@@ -604,6 +643,30 @@ int cphb_mesh_triangle_normals(const float *vertices, size_t n_vertices, const i
  * order, normalised when asked; a vertex in no triangle gets 0, so the rows stay aligned with the vertices */
 int cphb_mesh_vertex_normals(const int32_t *triangles, size_t n_triangles, const float *triangle_normals, size_t n_vertices,
                              int normalized, float *vertex_normals, void *stream);
+
+/* ------------------------------------------------------------------------ *
+ * PointCloud::CreateFromDepthImage / CreateFromRGBDImage (geometry/pointcloud_factory.cu:43-200, 329-373).  Images are
+ * device buffers, row-major; outputs are caller-allocated device [rows][3] float32.
+ * ------------------------------------------------------------------------ */
+/* The point of every stride-th pixel of every stride-th row, (width / stride) x (height / stride) samples in pixel
+ * order.  depth: 1 channel, uint16 (bytes 2: raw / (float)(int)depth_scale, 0 where that is >= (float)(int)depth_trunc,
+ * as cphb_rgbd_convert's to_depth) or float32 metres (bytes 4, taken as it is; depth_scale and depth_trunc unread).
+ * A sample has a point when d > 0, d < depth_cutoff if depth_cutoff > 0, and the point is finite:
+ * x = ((col - cx) d) / fx, y = ((row - cy) d) / fy, z = d, moved by the camera pose extrinsic^-1 (inverted in float64,
+ * rounded to float32; extrinsic row-major world-to-camera).  color (may be NULL): uint8 RGB (colour c / 255) or 1-channel
+ * float32 (grey g as (g, g, g)), the depth's size.  compute_normals: the structured normal of a sample from its
+ * left / right / up / down neighbouring samples ((left - right) x (up - down), a neighbour without a point counting as
+ * zero, normalised and turned to z <= 0); a sample on a border row or column, or with a zero cross product, gets 0.
+ * project_valid_depth_only: only the samples with a point, in pixel order; otherwise one row per sample, NaN in
+ * every attribute where there is no point.  *h_count = the number of rows; they are written only when capacity >= it
+ * (capacity 0 sizes).  CPHB_ERR_INVALID: an unsupported image format, images of different sizes, stride < 1, a NaN
+ * depth_cutoff, a depth_scale / depth_trunc outside cphb_rgbd_convert's range for uint16 depth, a singular extrinsic.
+ * Synchronises. */
+int cphb_depth_to_points(const void *depth, int width, int height, int depth_channels, int depth_bytes_per_channel, float depth_scale,
+                         float depth_trunc, int stride, const void *color, int color_width, int color_height, int color_channels,
+                         int color_bytes_per_channel, const float h_intrinsic[9], const float h_extrinsic[16], float depth_cutoff,
+                         int compute_normals, int project_valid_depth_only, float *points, float *normals, float *colors,
+                         size_t capacity, size_t *h_count, void *stream);
 
 /* ------------------------------------------------------------------------ *
  * collision::ComputeIntersection (collision.h:36-160, collision.cu:1137-1231)

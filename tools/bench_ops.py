@@ -50,7 +50,11 @@ def main():
     ap.add_argument("--tsdf-mesh", action="store_true",
                     help="instead: time UniformTSDFVolume.extract_triangle_mesh and compute_vertex_normals at 256^3 and 512^3 "
                          "after 8 ring-camera sphere views")
+    ap.add_argument("--depth-cloud", action="store_true",
+                    help="instead: time PointCloud.create_from_rgbd_image and create_from_depth_image at 640x480 and 1280x720")
     args = ap.parse_args()
+    if args.depth_cloud:
+        return depth_cloud(args.reps, args.out)
     if args.tsdf_mesh:
         return tsdf_mesh(args.reps, args.out)
     if args.tsdf:
@@ -1039,6 +1043,92 @@ def tsdf(reps, out=None):
         del vol
     obj = {"op": "UniformTSDFVolume(2.0, res, 0.04): 640x480 sphere frames (radius 0.6, cameras at 2.5); extractions and "
                  "Raycast after 8 views", "gpu": gpu, "reps": reps, "rows": rows}
+    line = json.dumps(obj)
+    print(line)
+    if out:
+        with open(out, "w") as f:
+            f.write(line + "\n")
+
+
+def depth_cloud_bytes(w, h, stride, depth_bytes, color_bytes, rows, attrs):
+    """least HBM traffic of one CreateFrom*Image call: each sampled pixel's depth (and colour) read once, `attrs` float3
+    attributes written per output row.  The structured normal's neighbour reads are not counted (they hit cache
+    lines the row above and below already bring in)."""
+    samples = (w // stride) * (h // stride)
+    return samples * (depth_bytes + color_bytes) + 12 * attrs * rows
+
+
+def depth_cloud(reps, out=None):
+    """PointCloud.create_from_rgbd_image (RGB8 colour, without and with structured normals, valid rows only and every row)
+    and create_from_depth_image (uint16, strides 1 and 4) at 640 x 480 and 1280 x 720: a sphere of radius 0.6 seen from
+    2.5 over a wall, 10 % of the pixels holes.  CUDA-event median and minimum of `reps` Python calls after a warm-up
+    call, the kernel times of one further call from torch.profiler, and the bytes model over the kernel time against
+    3.35 TB/s."""
+    import subprocess
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    import cupoch_b200 as cph
+    from cupoch_b200 import _lib
+    from cupoch_b200.testing.datagen import ring_cameras, sphere_depth
+    L = _lib.lib()
+    G = cph.geometry
+    gpu = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                         capture_output=True, text=True).stdout.strip()
+    ev = [L.cphb_event_create() for _ in range(2)]
+
+    def timed(fn):
+        times = []
+        for r in range(reps + 1):
+            L.cphb_event_record(ev[0], None)
+            fn()
+            L.cphb_event_record(ev[1], None)
+            ms = C.c_float(0)
+            _lib.check(L.cphb_event_elapsed_ms(ev[0], ev[1], C.byref(ms)))
+            if r:
+                times.append(ms.value)
+        return times
+
+    def kernels(fn):
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            fn()
+            torch.cuda.synchronize()
+        k = {}
+        for e in prof.key_averages():
+            t = getattr(e, "device_time_total", getattr(e, "cuda_time_total", 0.0)) * 1e-3
+            if t > 0 and "Memset" not in e.key and "Memcpy" not in e.key:
+                k[e.key[:60]] = k.get(e.key[:60], 0.0) + t
+        return k
+
+    rows = []
+    rng = np.random.default_rng(4)
+    for w, h in ((640, 480), (1280, 720)):
+        K, E = ring_cameras(8, w, h)[0]
+        d = sphere_depth(K, E, w, h, 0.6)
+        d = np.where(d > 0, d, 3.5).astype(np.float32)  # the wall behind the sphere
+        d[rng.random(d.shape) < 0.1] = 0
+        d16 = np.round(d * 1000).astype(np.uint16)
+        col = rng.integers(0, 256, (h, w, 3), dtype=np.uint8)
+        intr = cph.camera.PinholeCameraIntrinsic(w, h, K[0, 0], K[1, 1], K[0, 2], K[1, 2])
+        im = G.RGBDImage.create_from_color_and_depth(G.Image(col), G.Image(d16), 1000.0, 4.0, False)
+        cases = [("CreateFromRGBDImage", 1, valid, normals, lambda v=valid, n=normals: G.PointCloud.create_from_rgbd_image(im, intr, E, v, -1.0, n))
+                 for valid, normals in ((True, False), (True, True), (False, False))]
+        depth_img = G.Image(d16)
+        cases += [("CreateFromDepthImage uint16", s, True, False,
+                   lambda s=s: G.PointCloud.create_from_depth_image(depth_img, intr, E, 1000.0, 4.0, s)) for s in (1, 4)]
+        for name, stride, valid, normals, fn in cases:
+            n_out = len(fn())
+            ts = timed(fn)
+            k = kernels(fn)
+            kern = sum(v for kn, v in k.items() if "dc_" in kn)
+            rgbd = name == "CreateFromRGBDImage"
+            nbytes = depth_cloud_bytes(w, h, stride, 4 if rgbd else 2, 3 if rgbd else 0, n_out, 1 + rgbd + normals)
+            rows.append({"op": name, "width": w, "height": h, "stride": stride, "project_valid_depth_only": valid,
+                         "compute_normals": normals, "rows": n_out, "call_ms_median": float(np.median(ts)),
+                         "call_ms_min": float(np.min(ts)), "kernel_ms_profiled": k, "depth_cloud_kernel_ms": kern,
+                         "bytes_model": nbytes,
+                         "share_of_3.35TBps_over_kernel_time": nbytes / (kern * 1e-3) / HBM_BYTES_PER_S if kern else None})
+    obj = {"op": "PointCloud from depth / RGB-D frames: a sphere (radius 0.6, camera at 2.5) over a wall at 3.5 m, 10 % holes",
+           "gpu": gpu, "reps": reps, "rows": rows}
     line = json.dumps(obj)
     print(line)
     if out:

@@ -59,3 +59,6 @@ print("tsdf points", len(vol.extract_point_cloud()), "voxels", len(vol.extract_v
 mesh = vol.extract_triangle_mesh()
 mesh.compute_vertex_normals()
 print("tsdf mesh vertices", len(mesh.vertices), "triangles", len(mesh.triangles), "vertex normals", len(mesh.vertex_normals))
+print("rgbd points", len(G.PointCloud.create_from_rgbd_image(im, intr, E, True, -1.0, True)),
+      len(G.PointCloud.create_from_rgbd_image(im, intr, E, False, 2.4, True)),
+      "depth points", len(G.PointCloud.create_from_depth_image(G.Image(d16), intr, E, 1000.0, 4.0, 3)))

@@ -14,8 +14,46 @@
 #include "fused_neighbourhood.cuh"
 #include "cphb_searchk.cuh"
 
-// ComputeNormal (estimate_normals.cu:38-54): covariance E[xx^T] - E[x]E[x]^T in float32, eigenvector of the smallest
-// eigenvalue, (0,0,1) with fewer than 3 neighbours or a zero / NaN vector
+__device__ __forceinline__ bool usable_vector(const float *v) {
+    const float nn = sqrtf(dot3(v[0], v[1], v[2], v[0], v[1], v[2]));
+    return nn > 0.f && nn <= FLT_MAX;  // false for 0, NaN and inf
+}
+
+// The smallest eigenvalue's eigenvector when FastEigen3x3's is NaN or zero: its eigvec1 evaluates signf(0) = 0/0 when a
+// projection vanishes exactly, as on axis-aligned lattice planes (DESIGN.md section 4, item 22).  e are the
+// eigenvalues FastEigen3x3 returned, those of A = cov / max coefficient.  eigvec0's rule gives v0 directly: the largest
+// cross product of two rows of A - e[mi] I.  That rule needs e[mi] to be a simple eigenvalue: near a double root (a
+// line) the rows are nearly parallel and their cross products are rounding noise.  There, with the middle eigenvalue
+// within 2^-10 of the spread above e[mi] (FastEigen3x3's eigenvalues are only good to about the square root of float32
+// precision as two of them meet), any unit vector perpendicular to the largest eigenvalue's eigenvector is a normal;
+// eigvec1's U is one.
+__device__ void normal_direct(const float *cov, const float *e, int mi, float *n) {
+    float A[9];
+    float mc = cov[0];
+#pragma unroll
+    for (int i = 1; i < 9; ++i) if (cov[i] > mc) mc = cov[i];
+#pragma unroll
+    for (int i = 0; i < 9; ++i) A[i] = cov[i] / mc;
+    int ma = 0;
+    if (e[1] > e[ma]) ma = 1;
+    if (e[2] > e[ma]) ma = 2;
+    const float mid = __fsub_rn(__fsub_rn(__fadd_rn(__fadd_rn(e[0], e[1]), e[2]), e[mi]), e[ma]);
+    if (mid - e[mi] > 0x1p-10f * (e[ma] - e[mi])) {
+        eigvec0(A, e[mi], n);
+        return;
+    }
+    float v2[3];
+    eigvec0(A, e[ma], v2);
+    const float mx = fmaxf(fabsf(v2[0]), fabsf(v2[1]));
+    const float inv_len = 1 / sqrtf(__fmaf_rn(v2[2], v2[2], mx * mx));
+    if (fabsf(v2[0]) > fabsf(v2[1])) { n[0] = -v2[2]; n[1] = 0; n[2] = v2[0]; }
+    else { n[0] = 0; n[1] = v2[2]; n[2] = -v2[1]; }
+    n[0] *= inv_len; n[1] *= inv_len; n[2] *= inv_len;
+}
+
+// ComputeNormal (estimate_normals.cu:38-54): the eigenvector of the covariance's smallest eigenvalue; (0,0,1) with
+// fewer than 3 neighbours.  Where FastEigen3x3's vector is NaN or zero the reference's normal is NaN; here
+// normal_direct computes it (DESIGN.md section 4, item 22), and only a covariance that is not finite still gives (0,0,1).
 __device__ __forceinline__ void normal_from_cumulants(const double (&cum)[9], int cnt, float &nx, float &ny, float &nz) {
     nx = 0.f; ny = 0.f; nz = 1.f;
     if (cnt < 3) return;
@@ -26,9 +64,9 @@ __device__ __forceinline__ void normal_from_cumulants(const double (&cum)[9], in
     int mi = 0;
     if (e[1] < e[mi]) mi = 1;
     if (e[2] < e[mi]) mi = 2;
-    nx = V[mi]; ny = V[3 + mi]; nz = V[6 + mi];
-    const float nn = sqrtf(dot3(nx, ny, nz, nx, ny, nz));
-    if (nn == 0.0f || nn != nn) { nx = 0.f; ny = 0.f; nz = 1.f; }
+    float n[3] = {V[mi], V[3 + mi], V[6 + mi]};
+    if (!usable_vector(n)) normal_direct(cov, e, mi, n);
+    if (usable_vector(n)) { nx = n[0]; ny = n[1]; nz = n[2]; }
 }
 
 __global__ void __launch_bounds__(256) fill_normals_kernel(float *out, size_t n) {

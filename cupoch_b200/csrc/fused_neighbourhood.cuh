@@ -16,18 +16,20 @@ __device__ __forceinline__ void cumulant_add(double (&cum)[9], float x, float y,
     cum[7] = fma((double)y, (double)z, cum[7]); cum[8] = fma((double)z, (double)z, cum[8]);
 }
 
-// covariance E[xx^T] - E[x]E[x]^T in float32 from the cumulants divided by (float)cnt, row-major (estimate_normals.cu:38-54,
-// iss_keypoints.cu:51-63).  cnt == 0 gives NaN coefficients.
+// covariance E[xx^T] - E[x]E[x]^T from the cumulants, row-major (estimate_normals.cu:38-54, iss_keypoints.cu:51-63).
+// Deviation (DESIGN.md section 4, item 22): the mean and the subtraction are float64, E[x_a x_b] - m_a m_b as
+// fma(-m_a, m_b, cum / cnt), and each coefficient is rounded to float32 once.  The reference subtracts in float32,
+// which cancels |m|^2 against a variance of the neighbourhood's size squared: normals 20 degrees off 10 m from the
+// origin.  Here the cancellation costs about cnt 2^-53 |m|^2.  cnt == 0 gives NaN coefficients.
 __device__ __forceinline__ void covariance_from_cumulants(const double (&cum)[9], int cnt, float (&cov)[9]) {
-    float c[9];
-#pragma unroll
-    for (int a = 0; a < 9; ++a) c[a] = (float)cum[a] / (float)cnt;
-    cov[0] = __fmaf_rn(-c[0], c[0], c[3]);
-    cov[4] = __fmaf_rn(-c[1], c[1], c[6]);
-    cov[8] = __fmaf_rn(-c[2], c[2], c[8]);
-    cov[1] = cov[3] = __fmaf_rn(-c[0], c[1], c[4]);
-    cov[2] = cov[6] = __fmaf_rn(-c[0], c[2], c[5]);
-    cov[5] = cov[7] = __fmaf_rn(-c[1], c[2], c[7]);
+    const double c = (double)cnt;
+    const double m0 = __ddiv_rn(cum[0], c), m1 = __ddiv_rn(cum[1], c), m2 = __ddiv_rn(cum[2], c);
+    cov[0] = (float)fma(-m0, m0, __ddiv_rn(cum[3], c));
+    cov[4] = (float)fma(-m1, m1, __ddiv_rn(cum[6], c));
+    cov[8] = (float)fma(-m2, m2, __ddiv_rn(cum[8], c));
+    cov[1] = cov[3] = (float)fma(-m0, m1, __ddiv_rn(cum[4], c));
+    cov[2] = cov[6] = (float)fma(-m0, m2, __ddiv_rn(cum[5], c));
+    cov[5] = cov[7] = (float)fma(-m1, m2, __ddiv_rn(cum[7], c));
 }
 
 // Per-lane query and empty k-best list of a fused kernel.  Dynamic shared memory per warp: 2 leaf tiles, 2 mbarriers,

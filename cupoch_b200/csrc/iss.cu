@@ -17,7 +17,7 @@
 // Arithmetic (DESIGN.md arithmetic contract; oracle/iss.c restates it):
 //   - resolution sum: tiles of ISS_TILE consecutive slot-1 d2 (original order) summed sequentially in double from 0,
 //     then the tile sums in tile order, rounded to float once; resolution = sqrtf(sum / (float)n), IEEE;
-//   - covariance: EstimateNormals' (float64 cumulants, cum / (float)count, explicit FMAs);
+//   - covariance: EstimateNormals' (covariance_from_cumulants: float64 cumulants, mean and subtraction, rounded once);
 //   - isZero: Eigen's DenseBase::isZero() with dummy_precision<float>() = 1e-5, i.e. isMuchSmallerThan(c, 1, 1e-5) =
 //     |c| <= 1 * 1e-5 for every coefficient -- an ABSOLUTE threshold (Eigen/src/Core/Fuzzy.h, MathFunctions.h);
 //   - FastEigen3x3Val (eigenvalue.inl:164-170): (min, ((e0 + e1) + e2) - min - max, max) of FastEigen3x3's eigenvalues,

@@ -67,14 +67,8 @@ static float iss_saliency(const float *pts, const int32_t *idx, int k, int min_n
         ++cnt;
     }
     if (cnt < min_neighbors) return -1.0f;
-    float c[9], cov[9];
-    for (int a = 0; a < 9; ++a) c[a] = (float)cum[a] / (float)cnt; /* cnt == 0: NaN, which fails every test below */
-    cov[0] = fmaf(-c[0], c[0], c[3]);
-    cov[4] = fmaf(-c[1], c[1], c[6]);
-    cov[8] = fmaf(-c[2], c[2], c[8]);
-    cov[1] = cov[3] = fmaf(-c[0], c[1], c[4]);
-    cov[2] = cov[6] = fmaf(-c[0], c[2], c[5]);
-    cov[5] = cov[7] = fmaf(-c[1], c[2], c[7]);
+    float cov[9];
+    covariance_from_cumulants(cum, cnt, cov); /* cnt == 0: NaN, which fails every test below */
     int zero = 1;
     for (int a = 0; a < 9; ++a) zero = zero && fabsf(cov[a]) <= ISS_ZERO_PREC;
     if (zero) return -1.0f;

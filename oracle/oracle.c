@@ -684,6 +684,52 @@ static void inverse3x3(const float *m, float *inv) {
 /* ======================================================================== */
 /* EstimateNormals  estimate_normals.cu:38-127, geometry_functor.h:35-55      */
 /* ======================================================================== */
+/* covariance E[xx^T] - E[x]E[x]^T from the float64 cumulants (also ISS's).  Deviation (DESIGN.md section 4, item 22):
+ * the mean and the subtraction are float64, fma(-m_a, m_b, cum / cnt), each coefficient rounded to float once; the
+ * reference subtracts in float32.  cnt == 0 gives NaN coefficients. */
+static void covariance_from_cumulants(const double cum[9], int cnt, float cov[9]) {
+    const double c = (double)cnt;
+    const double m0 = cum[0] / c, m1 = cum[1] / c, m2 = cum[2] / c;
+    cov[0] = (float)fma(-m0, m0, cum[3] / c);
+    cov[4] = (float)fma(-m1, m1, cum[6] / c);
+    cov[8] = (float)fma(-m2, m2, cum[8] / c);
+    cov[1] = cov[3] = (float)fma(-m0, m1, cum[4] / c);
+    cov[2] = cov[6] = (float)fma(-m0, m2, cum[5] / c);
+    cov[5] = cov[7] = (float)fma(-m1, m2, cum[7] / c);
+}
+static int usable_vector(const float *v) {
+    const float nn = sqrtf(dot3f(v[0], v[1], v[2], v[0], v[1], v[2]));
+    return nn > 0.f && nn <= FLT_MAX; /* false for 0, NaN and inf */
+}
+/* Deviation (item 22): the smallest eigenvalue's eigenvector where FastEigen3x3's is NaN or zero (eigvec1's signf(0) =
+ * 0/0).  e: FastEigen3x3's eigenvalues, those of A = cov / max coefficient.  eigvec0 of A with e[mi] when e[mi] is
+ * simple: the middle eigenvalue more than 2^-10 of the spread above it; else (a line) eigvec1's U for the largest
+ * eigenvalue's eigenvector, a unit vector perpendicular to it. */
+static void normal_direct(const float *cov, const float *e, int mi, float *n) {
+    float A[9];
+    float mc = cov[0];
+    for (int i = 1; i < 9; ++i)
+        if (cov[i] > mc) mc = cov[i];
+    for (int i = 0; i < 9; ++i) A[i] = cov[i] / mc;
+    int ma = 0;
+    if (e[1] > e[ma]) ma = 1;
+    if (e[2] > e[ma]) ma = 2;
+    const float mid = ((e[0] + e[1]) + e[2] - e[mi]) - e[ma];
+    if (mid - e[mi] > 0x1p-10f * (e[ma] - e[mi])) {
+        eigvec0(A, e[mi], n);
+        return;
+    }
+    float v2[3];
+    eigvec0(A, e[ma], v2);
+    const float mx = fmaxf(fabsf(v2[0]), fabsf(v2[1]));
+    const float inv_len = 1 / sqrtf(fmaf(v2[2], v2[2], mx * mx));
+    if (fabsf(v2[0]) > fabsf(v2[1])) {
+        n[0] = -v2[2]; n[1] = 0; n[2] = v2[0];
+    } else {
+        n[0] = 0; n[1] = v2[2]; n[2] = -v2[1];
+    }
+    for (int i = 0; i < 3; ++i) n[i] *= inv_len;
+}
 void orc_normals_from_neighbors(const float *pts, int n, const int32_t *nbr,
                                 int k, float *out) {
 #pragma omp parallel for schedule(static)
@@ -702,24 +748,17 @@ void orc_normals_from_neighbors(const float *pts, int n, const int32_t *nbr,
         }
         float *o = out + 3 * (size_t)i;
         if (cnt < 3) { o[0] = 0; o[1] = 0; o[2] = 1; continue; }
-        float c[9];
-        for (int a = 0; a < 9; ++a) c[a] = (float)cum[a] / (float)cnt;
         float cov[9];
-        cov[0] = fmaf(-c[0], c[0], c[3]);
-        cov[4] = fmaf(-c[1], c[1], c[6]);
-        cov[8] = fmaf(-c[2], c[2], c[8]);
-        cov[1] = cov[3] = fmaf(-c[0], c[1], c[4]);
-        cov[2] = cov[6] = fmaf(-c[0], c[2], c[5]);
-        cov[5] = cov[7] = fmaf(-c[1], c[2], c[7]);
+        covariance_from_cumulants(cum, cnt, cov);
         float e[3], V[9];
         fast_eigen3x3(cov, e, V);
         int mi = 0; /* Eigen minCoeff: first minimum */
         if (e[1] < e[mi]) mi = 1;
         if (e[2] < e[mi]) mi = 2;
-        float nx = V[mi], ny = V[3 + mi], nz = V[6 + mi];
-        float nn = sqrtf(dot3f(nx, ny, nz, nx, ny, nz));
-        if (nn == 0.0f || nn != nn) { nx = 0; ny = 0; nz = 1; }
-        o[0] = nx; o[1] = ny; o[2] = nz;
+        float v[3] = {V[mi], V[3 + mi], V[6 + mi]};
+        if (!usable_vector(v)) normal_direct(cov, e, mi, v);
+        if (!usable_vector(v)) { v[0] = 0; v[1] = 0; v[2] = 1; } /* a covariance that is not finite */
+        o[0] = v[0]; o[1] = v[1]; o[2] = v[2];
     }
 }
 void orc_estimate_normals(const float *pts, int n, int knn, float radius,

@@ -6,7 +6,7 @@
 
 Mirrors `import cupoch as cph` for: cph.geometry.{PointCloud, KDTreeFlann, KDTreeSearchParamKNN,
 KDTreeSearchParamRadius, VoxelGrid, OccupancyGrid, OccupancyVoxel, DistanceTransform, DistanceVoxel, Image, RGBDImage, TriangleMesh,
-keypoint.compute_iss_keypoints},
+FilterScope, keypoint.compute_iss_keypoints},
 cph.camera.{PinholeCameraIntrinsic, PinholeCameraIntrinsicParameters, PinholeCameraParameters},
 cph.integration.{UniformTSDFVolume, TSDFVolumeColorType},
 cph.registration.{registration_icp,

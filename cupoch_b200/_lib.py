@@ -112,6 +112,11 @@ _SIGNATURES = {
     "cphb_tsdf_extract_mesh": (C.c_int, [_P, _P, _P, _P, C.c_size_t, C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t), _P]),
     "cphb_mesh_triangle_normals": (C.c_int, [_P, C.c_size_t, _P, C.c_size_t, C.c_int, _P, _P]),
     "cphb_mesh_vertex_normals": (C.c_int, [_P, C.c_size_t, _P, C.c_size_t, C.c_int, _P, _P]),
+    "cphb_mesh_edge_list": (C.c_int, [_P, C.c_size_t, C.c_size_t, _P, C.c_size_t, C.POINTER(C.c_size_t), _P]),
+    "cphb_mesh_filter": (C.c_int, [C.c_int, C.c_int, C.c_float, C.c_float, _P, C.c_size_t, C.c_size_t, _P, _P, _P, C.c_int, _P, _P, _P,
+                                   _P]),
+    "cphb_mesh_surface_area": (C.c_int, [_P, C.c_size_t, _P, C.c_size_t, _P, C.POINTER(C.c_float), _P]),
+    "cphb_mesh_sample_points_uniformly": (C.c_int, [_P, C.c_size_t, _P, C.c_size_t, _P, _P, _P, C.c_size_t, _P, _P, _P, _P]),
     "cphb_stsdf_create": (C.c_int, [C.c_float, C.c_float, C.c_int, C.c_int, C.c_int, _P, C.POINTER(_P)]),
     "cphb_stsdf_destroy": (None, [_P]),
     "cphb_stsdf_reset": (C.c_int, [_P, _P]),

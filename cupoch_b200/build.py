@@ -28,7 +28,8 @@ FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c
 
 
 HEADERS = ["cphb_internal.cuh", "cphb_searchk.cuh", "fused_neighbourhood.cuh", "cphb_eigen3.cuh", "icp_types.cuh", "icp_solve.cuh", "icp_rows.cuh", "icp_kernels.cuh",
-           "icp_estimate.cuh", "icp_aux.cuh", "voxelkey.cuh", "depth_project.cuh", "tsdf_update.cuh"]
+           "icp_estimate.cuh", "icp_aux.cuh", "voxelkey.cuh", "depth_project.cuh", "tsdf_update.cuh",
+           "minstd.cuh", "sum_values.cuh"]
 MANIFEST = os.path.join(OBJ, "manifest.json")
 
 

@@ -21,15 +21,10 @@
 #include <math.h>
 
 #include "cphb_internal.cuh"
+#include "minstd.cuh"
 
 #define SEG_TILE 1024      // summation tile, also the scoring kernel's shared-memory tile (12 KB of points)
 #define SEG_KEY_STEPS 16   // key-kernel positions per thread
-#define SEG_LCG_A 48271u   // thrust::default_random_engine = minstd_rand
-#define SEG_LCG_M 2147483647u
-
-struct SegLcgPow {
-    uint32_t p[32];  // a^(2^j) mod m
-};
 
 struct SegState {
     float4 plane;  // best hypothesis, then the refit
@@ -38,13 +33,6 @@ struct SegState {
     float fitness, rmse;
 };
 
-__host__ __device__ __forceinline__ uint32_t seg_mulmod(uint32_t x, uint32_t y) {  // x * y mod 2^31 - 1
-    const uint64_t p = (uint64_t)x * y;
-    uint64_t r = (p & SEG_LCG_M) + (p >> 31);
-    r = (r & SEG_LCG_M) + (r >> 31);
-    return (uint32_t)(r >= SEG_LCG_M ? r - SEG_LCG_M : r);
-}
-
 __device__ __forceinline__ float seg_dist(float4 pl, float x, float y, float z) {
     return fabsf(__fadd_rn(dot3(pl.x, pl.y, pl.z, x, y, z), pl.w));
 }
@@ -52,15 +40,12 @@ __device__ __forceinline__ float seg_dist(float4 pl, float x, float y, float z) 
 // ---- sampling ---------------------------------------------------------------
 // keys[p] = random_functor(seed, n)(p): the draw after discard(p) is x_{p+1} = a^(p+1) x0 mod m.  Lane l of a warp owns
 // positions first + 32 i (coalesced stores): one jump-ahead by a^(first+1) from the table, then steps of a^32.
-__global__ void __launch_bounds__(256) seg_keys_kernel(uint32_t x0, uint32_t n, SegLcgPow pw, uint32_t *__restrict__ keys) {
+__global__ void __launch_bounds__(256) seg_keys_kernel(uint32_t x0, uint32_t n, cphb_minstd_pow pw, uint32_t *__restrict__ keys) {
     const size_t warp = (blockIdx.x * (size_t)blockDim.x + threadIdx.x) >> 5;
     const size_t first = warp * (32 * SEG_KEY_STEPS) + lane_id();
     if (first >= n) return;
     const uint64_t e = first + 1;
-    uint32_t x = x0;
-#pragma unroll
-    for (int j = 0; j < 32; ++j)
-        if ((e >> j) & 1u) x = seg_mulmod(x, pw.p[j]);
+    uint32_t x = cphb_minstd_jump(x0, e, pw);
     const uint32_t a32 = pw.p[5];
     const double span = (double)(n - 1u) + 1.0;  // uniform_real_distribution(0, (n-1) + 1)
 #pragma unroll 4
@@ -68,7 +53,7 @@ __global__ void __launch_bounds__(256) seg_keys_kernel(uint32_t x0, uint32_t n, 
         const size_t p = first + 32 * (size_t)i;
         if (p >= n) break;
         keys[p] = (uint32_t)(int)__dmul_rn(__ddiv_rn((double)(x - 1u), 2147483646.0), span);
-        x = seg_mulmod(x, a32);
+        x = cphb_minstd_mulmod(x, a32);
     }
 }
 
@@ -282,9 +267,8 @@ extern "C" int cphb_segment_plane(const float *points, size_t n, float distance_
     const size_t n_tiles = (n + SEG_TILE - 1) / SEG_TILE;
     int bits = 1;
     while (((size_t)1 << bits) < n) ++bits;  // keys lie in [0, n)
-    SegLcgPow pw;
-    pw.p[0] = SEG_LCG_A;
-    for (int j = 1; j < 32; ++j) pw.p[j] = seg_mulmod(pw.p[j - 1], pw.p[j - 1]);
+    cphb_minstd_pow pw;
+    cphb_minstd_table(&pw);
 
     uint32_t *keys = nullptr, *keys_out = nullptr, *cards = nullptr, *cards_alt = nullptr;
     int32_t *samples = nullptr;
@@ -326,7 +310,7 @@ extern "C" int cphb_segment_plane(const float *points, size_t n, float distance_
         const size_t key_threads = (n + SEG_KEY_STEPS * 32 - 1) / (SEG_KEY_STEPS * 32) * 32;
         const unsigned key_blocks = (unsigned)((key_threads + 255) / 256);
         for (int t = 0; t < T && !rc; ++t) {
-            uint32_t x0 = (uint32_t)h_seeds[t] % SEG_LCG_M;  // the int seed as the engine's uint32_t, mod m, 0 -> 1
+            uint32_t x0 = (uint32_t)h_seeds[t] % CPHB_MINSTD_M;  // the int seed as the engine's uint32_t, mod m, 0 -> 1
             if (x0 == 0) x0 = 1;
             CPHB_LAUNCH(seg_keys_kernel, key_blocks, 256, 0, s, x0, (uint32_t)n, pw, keys);
             rc = cphb_sort_pairs_u32(keys, keys_out, cards, cards_alt, n, bits, s);

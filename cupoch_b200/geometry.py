@@ -4,6 +4,7 @@ Names, argument meaning and error behaviour follow src/python/cupoch_pybind/geom
 pointcloud.cpp and kdtree_flann.cpp; computation goes through the C ABI only.
 """
 import ctypes as C
+import enum
 import sys
 
 import numpy as np
@@ -499,13 +500,28 @@ class PointCloud:
         return True
 
 
+class FilterScope(enum.IntEnum):
+    """MeshBase::FilterScope (meshbase.h:55): which vertex attributes a mesh filter changes"""
+    All = 0
+    Color = 1
+    Normal = 2
+    Vertex = 3
+
+
+# cphb_mesh_filter's kinds and attribute mask bits (include/cupoch_b200.h)
+_SHARPEN, _SIMPLE, _LAPLACIAN, _TAUBIN = 0, 1, 2, 3
+_SCOPE_MASK = {FilterScope.All: 7, FilterScope.Vertex: 1, FilterScope.Normal: 2, FilterScope.Color: 4}
+
+
 class TriangleMesh:
     """geometry::TriangleMesh (trianglemesh.h): vertices_, triangles_ (int32 vertex indices), vertex_colors_,
-    vertex_normals_ and triangle_normals_ on the device.  Only the normal computations run here; the rest of the
-    reference's TriangleMesh is not provided."""
+    vertex_normals_, triangle_normals_ and edge_list_ (int32 pairs) on the device.  The normal computations,
+    ComputeEdgeList, the four vertex filters, GetSurfaceArea and SamplePointsUniformly run here; mesh IO, cleanup,
+    primitives and textures are not provided."""
 
     def __init__(self, vertices=None, triangles=None):
         self._vertices = self._triangles = self._vertex_colors = self._vertex_normals = self._triangle_normals = None
+        self._edge_list = None
         if vertices is not None:
             self.vertices = vertices
         if triangles is not None:
@@ -516,6 +532,7 @@ class TriangleMesh:
     vertex_colors = property(lambda s: s._vertex_colors, lambda s, v: setattr(s, "_vertex_colors", Vector3fVector(v)))
     vertex_normals = property(lambda s: s._vertex_normals, lambda s, v: setattr(s, "_vertex_normals", Vector3fVector(v)))
     triangle_normals = property(lambda s: s._triangle_normals, lambda s, v: setattr(s, "_triangle_normals", Vector3fVector(v)))
+    edge_list = property(lambda s: s._edge_list, lambda s, v: setattr(s, "_edge_list", _vector2i(v)))
 
     def __repr__(self):
         return "geometry::TriangleMesh with %d points and %d triangles." % (self._n(self._vertices), self._n(self._triangles))
@@ -543,6 +560,9 @@ class TriangleMesh:
     def has_triangle_normals(self):
         return self.has_triangles() and self._n(self._triangle_normals) == len(self._triangles)
 
+    def has_edge_list(self):
+        return self._n(self._edge_list) > 0
+
     def compute_triangle_normals(self, normalized=True):
         """ComputeTriangleNormals (trianglemesh.cu:466-477): (v1 - v0) x (v2 - v0) per triangle, then normalised when
         asked.  A vertex index outside [0, len(vertices)) raises."""
@@ -569,6 +589,127 @@ class TriangleMesh:
                                                            out.ptr, None))
         self._vertex_normals = out
         return self
+
+    def compute_edge_list(self):
+        """ComputeEdgeList (trianglemesh.cu:505-519): the directed edges (a, b) and (b, a) of every triangle edge, sorted
+        and unique, as an (n, 2) int32 device array.  A vertex index outside [0, len(vertices)) raises."""
+        m = self._n(self._triangles)
+        buf = DeviceArray((max(6 * m, 1), 2), np.int32)
+        n = C.c_size_t(0)
+        _lib.check(_lib.lib().cphb_mesh_edge_list(self._triangles.ptr if m else None, m, self._n(self._vertices), buf.ptr, 6 * m,
+                                                  C.byref(n), None))
+        self._edge_list = _rows(buf, n.value)
+        return self
+
+    def _filter(self, kind, number_of_iterations, c0, c1, filter_scope):
+        """the four filters' common path: a new mesh with the triangles, the edge list (this mesh's own when it has one,
+        checked for range and order) and every vertex attribute, filtered or copied"""
+        mask = _SCOPE_MASK[FilterScope(filter_scope)]
+        if not self.has_edge_list():
+            self.compute_edge_list()
+        n = self._n(self._vertices)
+        out = TriangleMesh()
+        out._triangles, out._edge_list = self._triangles, self._edge_list
+        ins = [self._vertices if n else None, self._vertex_normals if self.has_vertex_normals() else None,
+               self._vertex_colors if self.has_vertex_colors() else None]
+        outs = [None if a is None else DeviceArray((n, 3), np.float32) for a in ins]
+        _lib.check(_lib.lib().cphb_mesh_filter(kind, int(number_of_iterations), float(c0), float(c1), self._edge_list.ptr,
+                                               self._n(self._edge_list), n, *[None if a is None else a.ptr for a in ins], mask,
+                                               *[None if a is None else a.ptr for a in outs], None))
+        out._vertices, out._vertex_normals, out._vertex_colors = outs
+        if out._vertices is None:
+            out._vertices = DeviceArray((0, 3), np.float32)
+        return out
+
+    def filter_sharpen(self, number_of_iterations=1, strength=1.0, filter_scope=FilterScope.All):
+        """FilterSharpen (trianglemesh.cu:521-599) -> a new mesh: per iteration v + strength * (v * N - sum of the N
+        neighbours).  A vertex without neighbours keeps its value; number_of_iterations <= 0 copies."""
+        return self._filter(_SHARPEN, number_of_iterations, strength, 0.0, filter_scope)
+
+    def filter_smooth_simple(self, number_of_iterations=1, filter_scope=FilterScope.All):
+        """FilterSmoothSimple (trianglemesh.cu:601-679) -> a new mesh: per iteration (v + sum of the N neighbours) /
+        (1 + N)."""
+        return self._filter(_SIMPLE, number_of_iterations, 0.0, 0.0, filter_scope)
+
+    def filter_smooth_laplacian(self, number_of_iterations=1, lambda_=0.5, filter_scope=FilterScope.All, **kw):
+        """FilterSmoothLaplacian (trianglemesh.cu:681-735) -> a new mesh: per iteration v + lambda (sum w_nb v_nb /
+        sum w_nb - v), w = 1 / (|v - v_nb| + 1e-12) from the input vertices.  The reference's keyword `lambda` is
+        accepted as lambda_."""
+        return self._filter(_LAPLACIAN, number_of_iterations, kw.pop("lambda", lambda_), 0.0, _no_more(filter_scope, kw))
+
+    def filter_smooth_taubin(self, number_of_iterations=1, lambda_=0.5, mu=-0.53, filter_scope=FilterScope.All, **kw):
+        """FilterSmoothTaubin (trianglemesh.cu:737-800) -> a new mesh: per iteration a Laplacian step with lambda, then
+        one with mu, with the weights of the input vertices.  `lambda` is accepted as lambda_."""
+        return self._filter(_TAUBIN, number_of_iterations, kw.pop("lambda", lambda_), mu, _no_more(filter_scope, kw))
+
+    def get_surface_area(self):
+        """GetSurfaceArea (trianglemesh.cu:802-813): the sum of 0.5 |(p0 - p1) x (p0 - p2)| over the triangles, in
+        float64 in a fixed order, as float32"""
+        return self._surface_area(None)
+
+    def _surface_area(self, areas):
+        m = self._n(self._triangles)
+        a = C.c_float(0)
+        if m:
+            _lib.check(_lib.lib().cphb_mesh_surface_area(self._vertices.ptr if self.has_vertices() else None, self._n(self._vertices),
+                                                         self._triangles.ptr, m, None if areas is None else areas.ptr, C.byref(a), None))
+        return float(a.value)
+
+    def sample_points_uniformly(self, number_of_points=100, use_triangle_normal=False):
+        """SamplePointsUniformly (trianglemesh.cu:830-901) -> a device PointCloud of exactly number_of_points points,
+        triangle i taking llrint(cdf_i n) - llrint(cdf_{i-1} n) of them.  Normals: the triangle's when
+        use_triangle_normal (computed, normalised, and kept on this mesh when it has none), else the interpolated vertex
+        normals when there are any; colours are interpolated.  number_of_points 0 or above 2^30 - 1, no triangles or a
+        surface area that is not positive and finite raises."""
+        n = int(number_of_points)
+        if n <= 0:
+            raise ValueError("[SamplePointsUniformly] number_of_points <= 0")
+        if not self.has_triangles():
+            raise ValueError("[SamplePointsUniformly] input mesh has no triangles")
+        if use_triangle_normal and not self.has_triangle_normals():
+            self.compute_triangle_normals(True)
+        vn = self._vertex_normals if self.has_vertex_normals() else None
+        tn = self._triangle_normals if use_triangle_normal else None
+        vc = self._vertex_colors if self.has_vertex_colors() else None
+        if n > _MAX_SAMPLES:
+            raise ValueError("[SamplePointsUniformly] number_of_points exceeds 2^30 - 1")
+        pts = DeviceArray((n, 3), np.float32)
+        nrm = DeviceArray((n, 3), np.float32) if (vn is not None or tn is not None) else None
+        col = DeviceArray((n, 3), np.float32) if vc is not None else None
+        _lib.check(_lib.lib().cphb_mesh_sample_points_uniformly(
+            self._vertices.ptr, len(self._vertices), self._triangles.ptr, len(self._triangles), None if vn is None else vn.ptr,
+            None if tn is None else tn.ptr, None if vc is None else vc.ptr, n, pts.ptr, None if nrm is None else nrm.ptr,
+            None if col is None else col.ptr, None))
+        pc = PointCloud()
+        pc._points, pc._normals, pc._colors = pts, nrm, col
+        return pc
+
+
+_MAX_SAMPLES = 2 ** 30 - 1  # CPHB_MESH_MAX_SAMPLES: draw 2 n must stay inside minstd_rand's period 2^31 - 2
+
+
+def _no_more(filter_scope, kw):
+    if kw:
+        raise TypeError("unexpected keyword argument(s): %s" % ", ".join(sorted(kw)))
+    return filter_scope
+
+
+def _rows(buf, n):
+    """the first n rows of a device array, as an array of their own"""
+    out = DeviceArray((n,) + buf.shape[1:], buf.dtype)
+    if out.nbytes:
+        _lib.check(_lib.lib().cphb_memcpy_d2d(out.ptr, buf.ptr, out.nbytes, None))
+        _lib.check(_lib.lib().cphb_stream_synchronize(None))
+    return out
+
+
+def _vector2i(a):
+    if a is None:
+        return None
+    d = DeviceArray.wrap(a, np.int32)
+    if len(d.shape) != 2 or d.shape[1] != 2:
+        raise ValueError("expected (n,2) int32")
+    return d
 
 
 def _floats(a, n):

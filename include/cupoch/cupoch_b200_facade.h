@@ -1969,9 +1969,18 @@ inline std::shared_ptr<PointCloud> PointCloud::CreateFromRGBDImage(const RGBDIma
 }  // namespace geometry
 
 namespace geometry {
+/// geometry::MeshBase (meshbase.h): only what TriangleMesh's filters need, FilterScope, so that both
+/// MeshBase::FilterScope and TriangleMesh::FilterScope name it.
+class MeshBase {
+public:
+    enum class FilterScope { All, Color, Normal, Vertex };
+    virtual ~MeshBase() {}
+};
+
 /// geometry::TriangleMesh (trianglemesh.h, meshbase.h): vertices_, vertex_normals_, vertex_colors_, triangles_ (int32
-/// vertex indices) and triangle_normals_ on the device.  Only the two normal computations are provided.
-class TriangleMesh {
+/// vertex indices), triangle_normals_ and edge_list_ on the device.  The two normal computations, ComputeEdgeList,
+/// the four vertex filters, GetSurfaceArea and SamplePointsUniformly are provided (no IO, cleanup or primitives).
+class TriangleMesh : public MeshBase {
 public:
     TriangleMesh() {}
     TriangleMesh(const utility::device_vector<Eigen::Vector3f> &vertices, const utility::device_vector<Eigen::Vector3i> &triangles)
@@ -2007,12 +2016,100 @@ public:
         return *this;
     }
 
+    bool HasEdgeList() const { return edge_list_.size() > 0; }
+    /// ComputeEdgeList (trianglemesh.cu:505-519): the directed edges (a, b) and (b, a) of every triangle edge, sorted and
+    /// unique.  A vertex index outside [0, vertices_.size()) throws.
+    TriangleMesh &ComputeEdgeList() {
+        utility::device_vector<Eigen::Vector2i> buf(6 * triangles_.size());
+        size_t n = 0;
+        utility::check(cphb_mesh_edge_list((const int32_t *)triangles_.data(), triangles_.size(), vertices_.size(), (int32_t *)buf.data(),
+                                           buf.size(), &n, nullptr));
+        edge_list_.resize(n);
+        if (n) {
+            utility::check(cphb_memcpy_d2d(edge_list_.data(), buf.data(), n * sizeof(Eigen::Vector2i), nullptr));
+            utility::check(cphb_stream_synchronize(nullptr));
+        }
+        return *this;
+    }
+    /// FilterSharpen (trianglemesh.cu:521-599): per iteration v + strength (v N - sum of the N neighbours)
+    std::shared_ptr<TriangleMesh> FilterSharpen(int number_of_iterations, float strength, FilterScope scope = FilterScope::All) const {
+        return Filter(CPHB_MESH_SHARPEN, number_of_iterations, strength, 0.f, scope);
+    }
+    /// FilterSmoothSimple (trianglemesh.cu:601-679): per iteration (v + sum of the N neighbours) / (1 + N)
+    std::shared_ptr<TriangleMesh> FilterSmoothSimple(int number_of_iterations, FilterScope scope = FilterScope::All) const {
+        return Filter(CPHB_MESH_SIMPLE, number_of_iterations, 0.f, 0.f, scope);
+    }
+    /// FilterSmoothLaplacian (trianglemesh.cu:681-735): per iteration v + lambda (sum w v_nb / sum w - v), w = 1 / (|v -
+    /// v_nb| + 1e-12) from the input vertices
+    std::shared_ptr<TriangleMesh> FilterSmoothLaplacian(int number_of_iterations, float lambda, FilterScope scope = FilterScope::All) const {
+        return Filter(CPHB_MESH_LAPLACIAN, number_of_iterations, lambda, 0.f, scope);
+    }
+    /// FilterSmoothTaubin (trianglemesh.cu:737-800): per iteration a Laplacian step with lambda, then one with mu
+    std::shared_ptr<TriangleMesh> FilterSmoothTaubin(int number_of_iterations, float lambda = 0.5f, float mu = -0.53f,
+                                                     FilterScope scope = FilterScope::All) const {
+        return Filter(CPHB_MESH_TAUBIN, number_of_iterations, lambda, mu, scope);
+    }
+    /// GetSurfaceArea (trianglemesh.cu:802-828): the float64 fixed-order sum of 0.5 |(p0 - p1) x (p0 - p2)|, as float
+    float GetSurfaceArea() const { return SurfaceArea(nullptr); }
+    float GetSurfaceArea(utility::device_vector<float> &triangle_areas) const {
+        triangle_areas.resize(triangles_.size());
+        return SurfaceArea(triangle_areas.data());
+    }
+    /// SamplePointsUniformly (trianglemesh.cu:830-901): exactly number_of_points points; with use_triangle_normal the
+    /// normalised triangle normals are computed and kept when the mesh has none.  number_of_points 0 or above 2^30 - 1,
+    /// no triangles, or a surface area that is not positive and finite throws.
+    std::shared_ptr<PointCloud> SamplePointsUniformly(size_t number_of_points, bool use_triangle_normal = false) {
+        if (number_of_points == 0) throw std::runtime_error("[SamplePointsUniformly] number_of_points <= 0");
+        if (triangles_.size() == 0) throw std::runtime_error("input mesh has no triangles");
+        if (use_triangle_normal && !HasTriangleNormals()) ComputeTriangleNormals(true);
+        const bool vn = HasVertexNormals(), vc = HasVertexColors();
+        auto pc = std::make_shared<PointCloud>();
+        pc->points_.resize(number_of_points);
+        if (vn || use_triangle_normal) pc->normals_.resize(number_of_points);
+        if (vc) pc->colors_.resize(number_of_points);
+        utility::check(cphb_mesh_sample_points_uniformly(
+            (const float *)vertices_.data(), vertices_.size(), (const int32_t *)triangles_.data(), triangles_.size(),
+            vn ? (const float *)vertex_normals_.data() : nullptr, use_triangle_normal ? (const float *)triangle_normals_.data() : nullptr,
+            vc ? (const float *)vertex_colors_.data() : nullptr, number_of_points, (float *)pc->points_.data(),
+            (vn || use_triangle_normal) ? (float *)pc->normals_.data() : nullptr, vc ? (float *)pc->colors_.data() : nullptr, nullptr));
+        return pc;
+    }
+
 public:
     utility::device_vector<Eigen::Vector3f> vertices_;
     utility::device_vector<Eigen::Vector3f> vertex_normals_;
     utility::device_vector<Eigen::Vector3f> vertex_colors_;
     utility::device_vector<Eigen::Vector3i> triangles_;
     utility::device_vector<Eigen::Vector3f> triangle_normals_;
+    utility::device_vector<Eigen::Vector2i> edge_list_;
+
+private:
+    // the filters' common path: a new mesh with the triangles, the edge list (this mesh's own when it has one, checked
+    // for range and order) and every vertex attribute, filtered or copied; triangle normals are not carried
+    std::shared_ptr<TriangleMesh> Filter(int kind, int iterations, float c0, float c1, FilterScope scope) const {
+        auto mesh = std::make_shared<TriangleMesh>();
+        mesh->triangles_ = triangles_;
+        mesh->vertices_.resize(vertices_.size());
+        mesh->edge_list_ = edge_list_;
+        if (!mesh->HasEdgeList()) mesh->ComputeEdgeList();
+        const int mask = scope == FilterScope::All ? 7 : scope == FilterScope::Vertex ? 1 : scope == FilterScope::Normal ? 2 : 4;
+        const bool vn = HasVertexNormals(), vc = HasVertexColors();
+        if (vn) mesh->vertex_normals_.resize(vertices_.size());
+        if (vc) mesh->vertex_colors_.resize(vertices_.size());
+        utility::check(cphb_mesh_filter(kind, iterations, c0, c1, (const int32_t *)mesh->edge_list_.data(), mesh->edge_list_.size(),
+                                        vertices_.size(), (const float *)vertices_.data(), vn ? (const float *)vertex_normals_.data() : nullptr,
+                                        vc ? (const float *)vertex_colors_.data() : nullptr, mask, (float *)mesh->vertices_.data(),
+                                        vn ? (float *)mesh->vertex_normals_.data() : nullptr, vc ? (float *)mesh->vertex_colors_.data() : nullptr,
+                                        nullptr));
+        return mesh;
+    }
+    float SurfaceArea(float *areas) const {
+        float a = 0.f;
+        if (triangles_.size())
+            utility::check(cphb_mesh_surface_area((const float *)vertices_.data(), vertices_.size(), (const int32_t *)triangles_.data(),
+                                                  triangles_.size(), areas, &a, nullptr));
+        return a;
+    }
 };
 }  // namespace geometry
 

@@ -633,8 +633,9 @@ int cphb_stsdf_data(const cphb_stsdf *volume, size_t *h_units, uint64_t **keys, 
 int cphb_stsdf_info(const cphb_stsdf *volume, size_t *h_units, size_t *h_capacity, size_t *h_device_bytes);
 
 /* ------------------------------------------------------------------------ *
- * TriangleMesh normals (geometry/trianglemesh.cu), on device arrays: vertices [n_vertices][3] float32, triangles
- * [n_triangles][3] int32.  A vertex index outside [0, n_vertices) is CPHB_ERR_INVALID.  Synchronise.
+ * TriangleMesh normals, edge list, filters, area and sampling (geometry/trianglemesh.cu), on device arrays: vertices
+ * [n_vertices][3] float32, triangles [n_triangles][3] int32.  A vertex index outside [0, n_vertices) is
+ * CPHB_ERR_INVALID.  Synchronise.
  * ------------------------------------------------------------------------ */
 /* ComputeTriangleNormals: (v1 - v0) x (v2 - v0) per triangle, normalised (NormalizeNormals' rule) when asked */
 int cphb_mesh_triangle_normals(const float *vertices, size_t n_vertices, const int32_t *triangles, size_t n_triangles, int normalized,
@@ -643,6 +644,46 @@ int cphb_mesh_triangle_normals(const float *vertices, size_t n_vertices, const i
  * order, normalised when asked; a vertex in no triangle gets 0, so the rows stay aligned with the vertices */
 int cphb_mesh_vertex_normals(const int32_t *triangles, size_t n_triangles, const float *triangle_normals, size_t n_vertices,
                              int normalized, float *vertex_normals, void *stream);
+/* ComputeEdgeList: the 6 directed edges (a, b), (b, a) of every triangle edge, sorted lexicographically and unique, as
+ * edges [n_edges][2] int32 (a triangle with a repeated vertex gives the self-edge (a, a)).  *h_n_edges is the count; the
+ * rows are written only when capacity >= it (capacity 0 sizes; 6 n_triangles always holds them).  More than 2^31 - 1
+ * directed edges (6 n_triangles) or vertices is CPHB_ERR_INVALID. */
+int cphb_mesh_edge_list(const int32_t *triangles, size_t n_triangles, size_t n_vertices, int32_t *edges, size_t capacity,
+                        size_t *h_n_edges, void *stream);
+/* FilterSharpen / FilterSmoothSimple / FilterSmoothLaplacian / FilterSmoothTaubin over a sorted edge list (as
+ * cphb_mesh_edge_list gives it; an index outside [0, n_vertices) or a pair out of order is CPHB_ERR_INVALID).  Each
+ * attribute given (vertices, normals, colours [n_vertices][3], NULL when absent) is filtered into its output when its
+ * bit is set in filter_mask (1 vertices, 2 normals, 4 colours) and number_of_iterations > 0, and copied to it otherwise.
+ * Per pass, vertex v with N > 0 neighbours nb (its row of the edge list, summed left to right):
+ *   Sharpen   prv + strength * (prv * N - sum(prev[nb]))
+ *   Simple    (prv + sum(prev[nb])) / (float)(1.0 + N)
+ *   Laplacian prv + lambda * (sum(w * prev[nb]) / sum(w) - prv),  w = (float)(1.0 / (|v - nb| + 1e-12)) from the input
+ *   Taubin    Laplacian with lambda, then with mu, per iteration
+ * and a vertex without neighbours keeps its value.  strength_or_lambda is the strength (Sharpen) or lambda; mu is read by
+ * Taubin only.  Outputs must not alias inputs. */
+#define CPHB_MESH_SHARPEN 0
+#define CPHB_MESH_SIMPLE 1
+#define CPHB_MESH_LAPLACIAN 2
+#define CPHB_MESH_TAUBIN 3
+int cphb_mesh_filter(int kind, int number_of_iterations, float strength_or_lambda, float mu, const int32_t *edges, size_t n_edges,
+                     size_t n_vertices, const float *vertices, const float *normals, const float *colors, int filter_mask,
+                     float *out_vertices, float *out_normals, float *out_colors, void *stream);
+/* GetSurfaceArea: per triangle 0.5 |(p0 - p1) x (p0 - p2)| in float32, written to triangle_areas [n_triangles] when it
+ * is not NULL; *h_area = their float64 sum in the fixed order of the engine's reductions, rounded to float32. */
+int cphb_mesh_surface_area(const float *vertices, size_t n_vertices, const int32_t *triangles, size_t n_triangles,
+                           float *triangle_areas, float *h_area, void *stream);
+/* SamplePointsUniformly: exactly number_of_points points [n][3]; triangle i gets the points [b_i, b_i+1) with
+ * b_i+1 = llrint(cdf_i n) from a fixed-order float64 scan of the triangle areas (b_0 = 0, the last = n).  Point p uses
+ * draws 2p + 1 and 2p + 2 of thrust::default_random_engine with its default seed, mapped by
+ * uniform_real_distribution<float>(0, 1): a = 1 - sqrt(r1), b = sqrt(r1) (1 - r2), c = sqrt(r1) r2.  normals (may be
+ * NULL): triangle_normals[i] when triangle_normals is given, else the interpolated vertex_normals; colors (may be NULL):
+ * the interpolated vertex_colors.  number_of_points 0 or above CPHB_MESH_MAX_SAMPLES (the draws must stay inside the
+ * generator's period 2^31 - 2), no triangles, a bad index, or a total area that is not positive and finite is
+ * CPHB_ERR_INVALID. */
+#define CPHB_MESH_MAX_SAMPLES 1073741823u
+int cphb_mesh_sample_points_uniformly(const float *vertices, size_t n_vertices, const int32_t *triangles, size_t n_triangles,
+                                      const float *vertex_normals, const float *triangle_normals, const float *vertex_colors,
+                                      size_t number_of_points, float *points, float *normals, float *colors, void *stream);
 
 /* ------------------------------------------------------------------------ *
  * PointCloud::CreateFromDepthImage / CreateFromRGBDImage (geometry/pointcloud_factory.cu:43-200, 329-373).  Images are

@@ -52,7 +52,12 @@ def main():
                          "after 8 ring-camera sphere views")
     ap.add_argument("--depth-cloud", action="store_true",
                     help="instead: time PointCloud.create_from_rgbd_image and create_from_depth_image at 640x480 and 1280x720")
+    ap.add_argument("--mesh-ops", action="store_true",
+                    help="instead: time TriangleMesh.compute_edge_list, the four filters at 1 and 100 iterations, "
+                         "get_surface_area and sample_points_uniformly (1 M, 10 M points) on the --tsdf-mesh sphere meshes")
     args = ap.parse_args()
+    if args.mesh_ops:
+        return mesh_ops(args.reps, args.out)
     if args.depth_cloud:
         return depth_cloud(args.reps, args.out)
     if args.tsdf_mesh:
@@ -1217,6 +1222,91 @@ def tsdf_mesh(reps, out=None):
         del mesh, vol
     obj = {"op": "UniformTSDFVolume(2.0, res, 0.04, RGB8) after 8 640x480 ring-camera views of a sphere (radius 0.6, cameras "
                  "at 2.5): ExtractTriangleMesh and ComputeVertexNormals", "gpu": gpu, "reps": reps, "rows": rows}
+    line = json.dumps(obj)
+    print(line)
+    if out:
+        with open(out, "w") as f:
+            f.write(line + "\n")
+
+
+
+def mesh_pass_bytes(nv, ne, n_attrs, weighted):
+    """least HBM traffic of one filter pass: the row starts (4 bytes a vertex) and the edge list's neighbour column
+    (4 bytes an edge, the pairs' 8 bytes as the edges are read whole) once, the weights (4 an edge) and the weight totals
+    (4 a vertex) when weighted, and per filtered attribute the previous values read once and the new ones written once
+    (12 + 12 bytes a vertex).  Neighbour values are counted once: each vertex is everybody's neighbour a few times, which
+    the caches absorb."""
+    return 4 * (nv + 1) + 8 * ne + (4 * ne + 4 * nv if weighted else 0) + 24 * nv * n_attrs
+
+
+def mesh_ops(reps, out=None):
+    """TriangleMesh operations on the --tsdf-mesh scene's meshes (UniformTSDFVolume(2.0, res, 0.04, RGB8), res = 256 and
+    512, 8 ring-camera 640 x 480 sphere views) with vertex normals and colours: compute_edge_list; each filter at 1 and
+    100 iterations over all three attributes; get_surface_area; sample_points_uniformly at 1 M and 10 M points.
+    CUDA-event median and minimum of `reps` calls after a warm-up call, the engine launches of one call, and for the
+    100-iteration filters the per-pass time ((t100 - t1) / 99 passes, / 198 for Taubin) against the bytes bound of
+    mesh_pass_bytes at 3.35 TB/s."""
+    import subprocess
+    import cupoch_b200 as cph
+    from cupoch_b200 import _lib
+    from cupoch_b200.testing.datagen import ring_cameras, sphere_depth
+    L = _lib.lib()
+    G, I = cph.geometry, cph.integration
+    gpu = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                         capture_output=True, text=True).stdout.strip()
+    ev = [L.cphb_event_create() for _ in range(2)]
+
+    def timed(fn):
+        times, launches = [], 0
+        for r in range(reps + 1):
+            n0 = L.cphb_launch_count()
+            L.cphb_event_record(ev[0], None)
+            fn()
+            L.cphb_event_record(ev[1], None)
+            ms = C.c_float(0)
+            _lib.check(L.cphb_event_elapsed_ms(ev[0], ev[1], C.byref(ms)))
+            launches = L.cphb_launch_count() - n0
+            if r:
+                times.append(ms.value)
+        return {"call_ms_median": float(np.median(times)), "call_ms_min": float(np.min(times)), "launches": int(launches)}
+
+    w, h = 640, 480
+    rng = np.random.default_rng(2)
+    rows = []
+    for res in (256, 512):
+        vol = I.UniformTSDFVolume(2.0, res, 0.04, I.TSDFVolumeColorType.RGB8)
+        for K, E in ring_cameras(8, w, h):
+            d16 = np.round(sphere_depth(K, E, w, h, 0.6) * 1000).astype(np.uint16)
+            intr = cph.camera.PinholeCameraIntrinsic(w, h, K[0, 0], K[1, 1], K[0, 2], K[1, 2])
+            col = rng.integers(0, 256, (h, w, 3), dtype=np.uint8)
+            vol.integrate(G.RGBDImage.create_from_color_and_depth(G.Image(col), G.Image(d16), 1000.0, 100.0, False), intr, E)
+        mesh = vol.extract_triangle_mesh()
+        del vol
+        mesh.compute_vertex_normals()
+        nv, nt = len(mesh.vertices), len(mesh.triangles)
+        base = {"res": res, "vertices": nv, "triangles": nt}
+        rows.append(dict(base, op="compute_edge_list", **timed(mesh.compute_edge_list)))
+        ne = len(mesh.edge_list)
+        rows[-1]["edges"] = ne
+        for name, fn, per_it, weighted in (
+                ("filter_sharpen", lambda it: mesh.filter_sharpen(it, 0.01), 1, False),
+                ("filter_smooth_simple", lambda it: mesh.filter_smooth_simple(it), 1, False),
+                ("filter_smooth_laplacian", lambda it: mesh.filter_smooth_laplacian(it, 0.5), 1, True),
+                ("filter_smooth_taubin", lambda it: mesh.filter_smooth_taubin(it, 0.5, -0.53), 2, True)):
+            t1 = timed(lambda: fn(1))
+            t100 = timed(lambda: fn(100))
+            rows.append(dict(base, op=name, iterations=1, **t1))
+            per_pass = (t100["call_ms_median"] - t1["call_ms_median"]) / (99 * per_it)
+            nbytes = mesh_pass_bytes(nv, ne, 3, weighted)
+            rows.append(dict(base, op=name, iterations=100, **t100, pass_ms=per_pass, pass_bytes_bound=nbytes,
+                             pass_share_of_3_35TBps_bytes_bound=nbytes / (per_pass * 1e-3) / HBM_BYTES_PER_S if per_pass > 0 else None))
+        rows.append(dict(base, op="get_surface_area", **timed(mesh.get_surface_area)))
+        for n in (1_000_000, 10_000_000):
+            rows.append(dict(base, op="sample_points_uniformly", points=n, **timed(lambda: mesh.sample_points_uniformly(n))))
+        del mesh
+    obj = {"op": "TriangleMesh edge list, filters, surface area and uniform sampling on the ExtractTriangleMesh meshes of "
+                 "UniformTSDFVolume(2.0, res, 0.04, RGB8) after 8 640x480 ring-camera sphere views, with vertex normals and "
+                 "colours", "gpu": gpu, "reps": reps, "rows": rows}
     line = json.dumps(obj)
     print(line)
     if out:

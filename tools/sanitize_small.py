@@ -62,3 +62,9 @@ print("tsdf mesh vertices", len(mesh.vertices), "triangles", len(mesh.triangles)
 print("rgbd points", len(G.PointCloud.create_from_rgbd_image(im, intr, E, True, -1.0, True)),
       len(G.PointCloud.create_from_rgbd_image(im, intr, E, False, 2.4, True)),
       "depth points", len(G.PointCloud.create_from_depth_image(G.Image(d16), intr, E, 1000.0, 4.0, 3)))
+mesh.compute_edge_list()
+filtered = [mesh.filter_sharpen(2, 0.1), mesh.filter_smooth_simple(2, G.FilterScope.Color),
+            mesh.filter_smooth_laplacian(2, 0.5, G.FilterScope.Vertex), mesh.filter_smooth_taubin(2)]
+sampled = mesh.sample_points_uniformly(3000, True)
+print("mesh edges", len(mesh.edge_list), "filtered", [len(m.vertices) for m in filtered], "area %.4f" % mesh.get_surface_area(),
+      "sampled", len(sampled.points), len(sampled.normals), len(sampled.colors))

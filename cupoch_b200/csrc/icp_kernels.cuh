@@ -10,7 +10,10 @@
 //        ROLE 1, certified regime  (>= 90 % of the previous launch's tiles were skipped by their certificates): static round-
 //                          robin tile schedule, cp.async pipeline, the normal-equation sums of every tile on the FP64 tensor
 //                          cores (one 8 x 8 Gram fragment per warp), block rows -> last-arriving block adds them in block
-//                          order, exchanges them with the other ranks and runs the solve IN THE SAME LAUNCH.
+//                          order, exchanges them with the other ranks and runs the solve IN THE SAME LAUNCH.  The per-
+//                          point stream is marked evict-first in L2, and the blocks that are not last run the grid sum
+//                          and the solve once on their own sums, so that the last block's serial tail runs warm code
+//                          (the working set evicts the kernel's instructions from L2 every launch).
 //        ROLE 1 after a searching launch: fixed-order sum of the tile sums + (exchange +) solve (icp_reduce_body).
 //   icp_finalize_kernel    the solve alone, after an NCCL all-reduce of the sums (multi-GPU, --comm nccl).
 //
@@ -26,6 +29,26 @@ __device__ __forceinline__ void cp_async_16(void *smem, const void *gmem) {  // 
 }
 __device__ __forceinline__ void cp_async_8(void *smem, const void *gmem) {
     asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(smem_u32(smem)), "l"(gmem) : "memory");
+}
+// Certified regime: the per-point stream (the working copy and the (match, slack) pairs, read and rewritten once per
+// launch) is marked evict-first in L2, so that it does not push out what is reused across launches -- the gathered target
+// rows and the kernel's own code (config 2 on the H100: 1.5 % on the launch loop, DESIGN section 5)
+__device__ __forceinline__ uint64_t l2_evict_first() {
+    uint64_t p;
+    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
+    return p;
+}
+__device__ __forceinline__ void cp_async_16(void *smem, const void *gmem, uint64_t pol) {
+    asm volatile("cp.async.cg.shared.global.L2::cache_hint [%0], [%1], 16, %2;" ::"r"(smem_u32(smem)), "l"(gmem), "l"(pol) : "memory");
+}
+__device__ __forceinline__ void cp_async_8(void *smem, const void *gmem, uint64_t pol) {
+    asm volatile("cp.async.ca.shared.global.L2::cache_hint [%0], [%1], 8, %2;" ::"r"(smem_u32(smem)), "l"(gmem), "l"(pol) : "memory");
+}
+__device__ __forceinline__ void st_hint(float4 *p, float4 v, uint64_t pol) {
+    asm volatile("st.global.L2::cache_hint.v4.f32 [%0], {%1, %2, %3, %4}, %5;" ::"l"(p), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w), "l"(pol) : "memory");
+}
+__device__ __forceinline__ void st_hint(int2 *p, int2 v, uint64_t pol) {
+    asm volatile("st.global.L2::cache_hint.v2.s32 [%0], {%1, %2}, %3;" ::"l"(p), "r"(v.x), "r"(v.y), "l"(pol) : "memory");
 }
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void cp_async_wait_0() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
@@ -179,6 +202,18 @@ __device__ __forceinline__ void lane_writeback(const IcpArgs &a, const LaunchCtx
 #pragma unroll
         for (int r = 0; r < 3; ++r) a.src_cov[(size_t)r * a.n_pad + i] = make_float4(Cs[3 * r], Cs[3 * r + 1], Cs[3 * r + 2], 0.f);
 }
+// the same stores with an L2 cache policy (certified regime)
+template <int KIND>
+__device__ __forceinline__ void lane_writeback(const IcpArgs &a, const LaunchCtx &c, unsigned i, const float4 &s,
+                                               const float (&sn)[3], const float (&Cs)[9], uint64_t pol) {
+    if (!c.apply || a.step_mode) return;
+    st_hint(&a.src[i], s, pol);
+    if (KIND == CPHB_EST_SYMMETRIC && a.src_nrm) st_hint(&a.src_nrm[i], make_float4(sn[0], sn[1], sn[2], 0.f), pol);
+    if (KIND == CPHB_EST_GENERALIZED_ICP && a.src_cov)
+#pragma unroll
+        for (int r = 0; r < 3; ++r)
+            st_hint(&a.src_cov[(size_t)r * a.n_pad + i], make_float4(Cs[3 * r], Cs[3 * r + 1], Cs[3 * r + 2], 0.f), pol);
+}
 
 // Warm start + certificate (DESIGN.md 3.1.8).  prev[i].y is a lower bound (rounded down) on the distance from this point's
 // position at the time it was last searched (minus the displacements since) to every target point other than its match.
@@ -242,6 +277,13 @@ __device__ __forceinline__ void lane_store_match(const IcpArgs &a, const LaunchC
         const float fresh = __fmul_rd(sqrt_approx(l2), 0.99999f);
         a.prev[i] = make_int2(found ? pos : -1, __float_as_int(cert ? slk : fresh));
     }
+    if (c.write_corr && in_range) a.corr_index[orig] = found ? (int32_t)j : -1;
+}
+// lane_store_match of a certified tile (every in-range lane keeps its match and its decremented slack), with an L2
+// cache policy on the (match, slack) store
+__device__ __forceinline__ void lane_store_certified(const IcpArgs &a, const LaunchCtx &c, unsigned i, unsigned orig, bool in_range,
+                                                     bool found, int pos, unsigned j, float slk, uint64_t pol) {
+    if (a.prev && !a.step_mode) st_hint(&a.prev[i], make_int2(found ? pos : -1, __float_as_int(slk)), pol);
     if (c.write_corr && in_range) a.corr_index[orig] = found ? (int32_t)j : -1;
 }
 
@@ -539,10 +581,11 @@ icp_iteration_kernel(const __grid_constant__ IcpArgs a) {
         unsigned tile = gw;
         float4 *pipe_s = reinterpret_cast<float4 *>(s_pipe[warp]);                // [NS][32] float4, then [NS][32] int2
         int2 *pipe_pv = reinterpret_cast<int2 *>(s_pipe[warp] + ICP_NS * 32 * 16);
+        const uint64_t pol_stream = l2_evict_first();
         auto stage_load = [&](unsigned t, int slot) {  // tile t -> stage slot (this lane's entries only)
             if (t < n_tiles) {
-                cp_async_16(&pipe_s[slot * 32 + lane], &a.src[t * 32 + lane]);
-                cp_async_8(&pipe_pv[slot * 32 + lane], &a.prev[t * 32 + lane]);
+                cp_async_16(&pipe_s[slot * 32 + lane], &a.src[t * 32 + lane], pol_stream);
+                cp_async_8(&pipe_pv[slot * 32 + lane], &a.prev[t * 32 + lane], pol_stream);
             }
         };
         // Pipeline (all copies are cp.async, one commit group per tile iteration, so the group arithmetic is uniform):
@@ -607,7 +650,7 @@ icp_iteration_kernel(const __grid_constant__ IcpArgs a) {
                 break;
             }
             ++n_skipped;
-            lane_writeback<KIND>(a, c, i, s, sn, Cs);
+            lane_writeback<KIND>(a, c, i, s, sn, Cs, pol_stream);
             if (a.dbg) {
                 const unsigned nc = __popc(__ballot_sync(CPHB_FULL, cert));
                 if (lane == 0) {
@@ -619,8 +662,7 @@ icp_iteration_kernel(const __grid_constant__ IcpArgs a) {
             const unsigned j = (unsigned)(best & 0xffffffffull);
             const float d2 = __uint_as_float((unsigned)(best >> 32));
             // (every in-range lane is certified: it keeps its decremented slack, the match is unchanged)
-            lane_store_match(a, c, i, orig, in_range, found, pv.x, j, true, slk, (unsigned)(best >> 32), 0x7f800000u,
-                             0x7f800000u, (unsigned)(best >> 32));
+            lane_store_certified(a, c, i, orig, in_range, found, pv.x, j, slk, pol_stream);
             if (c.materialize) continue;  // fitness / rmse / T of this pose are already in the state
             float J[NROWS][6], r[NROWS];
             lane_rows_vals<KIND, NROWS>(a, found, tv, s, sn, Cs, i, J, r);
@@ -733,6 +775,24 @@ icp_iteration_kernel(const __grid_constant__ IcpArgs a) {
     }
 }
 
+// Warp g of the last block adds the block rows g, g+W, ... (W warps per block) in that order, with 32 loads in flight.
+// Not inlined: the blocks that are not last run it once on a single row (icp_static_tail), so that its code is warm.
+__device__ __noinline__ double grid_row_sum(const double *partials, unsigned nb) {
+    const int warp = threadIdx.x >> 5, lane = lane_id();
+    double t = 0.0;
+    for (unsigned b = warp; b < nb; b += 32 * ICP_SEARCH_WARPS) {
+        double v[32];
+#pragma unroll
+        for (int u = 0; u < 32; ++u) {
+            const unsigned bb = b + u * ICP_SEARCH_WARPS;
+            v[u] = (bb < nb) ? __ldcg(&partials[(size_t)bb * 32 + lane]) : 0.0;  // x + 0.0 is exact
+        }
+#pragma unroll
+        for (int u = 0; u < 32; ++u) t += v[u];
+    }
+    return t;
+}
+
 // Tail of a certified-regime launch: block rows -> last-arriving block adds them in block order -> (multi-GPU exchange) ->
 // solve.  `row`: lane p of every warp holds column p of the warp's
 // sums.
@@ -752,6 +812,7 @@ __device__ void icp_static_tail(const IcpArgs &a, IcpState *st, double (*s_rowbu
 #pragma unroll
         for (int k = 0; k < ICP_SEARCH_WARPS; ++k) t += s_rowbuf[k][lane];  // fixed order: warps of the block
         a.partials[(size_t)blockIdx.x * 32 + lane] = t;
+        s_solve.S[lane] = t;  // (input of the warm-up below)
         __threadfence();
         __syncwarp();
         if (lane == 0) {
@@ -760,7 +821,16 @@ __device__ void icp_static_tail(const IcpArgs &a, IcpState *st, double (*s_rowbu
         }
     }
     __syncthreads();
-    if (!*s_flag) return;
+    if (!*s_flag) {
+        // not the last block: run the grid sum (on this block's own row) and the solve once and drop the results, so that
+        // the last block finds their instructions warm (warm_solve, icp_solve.cuh)
+        if (!materialize) {
+            if (warp == 0) s_solve.S[lane] += 0.0 * grid_row_sum(a.partials + (size_t)blockIdx.x * 32, 1);
+            __syncthreads();
+            warm_solve<KIND>(a, s_solve);
+        }
+        return;
+    }
     __threadfence();
     if (threadIdx.x == 0) {
         dbg_time(a, 2, false);
@@ -784,21 +854,8 @@ __device__ void icp_static_tail(const IcpArgs &a, IcpState *st, double (*s_rowbu
         }
         return;
     }
-    double t = 0.0;
-    {   // all warps of the block share the grid sum: warp g adds blocks g, g+W, ... in that order, with 32 loads in flight
-        // (the accumulators of the tile loop are dead here, so the registers are free)
-        const unsigned nb = gridDim.x;
-        for (unsigned b = warp; b < nb; b += 32 * ICP_SEARCH_WARPS) {
-            double v[32];
-#pragma unroll
-            for (int u = 0; u < 32; ++u) {
-                const unsigned bb = b + u * ICP_SEARCH_WARPS;
-                v[u] = (bb < nb) ? __ldcg(&a.partials[(size_t)bb * 32 + lane]) : 0.0;  // x + 0.0 is exact
-            }
-#pragma unroll
-            for (int u = 0; u < 32; ++u) t += v[u];
-        }
-    }
+    // all warps of the block share the grid sum (the accumulators of the tile loop are dead here, so the registers are free)
+    const double t = grid_row_sum(a.partials, gridDim.x);
     __syncthreads();
     s_rowbuf[warp][lane] = t;
     __syncthreads();
@@ -871,6 +928,7 @@ __device__ void icp_reduce_body(const IcpArgs &a, double (*s_acc)[32], unsigned 
 #pragma unroll
         for (int k = 0; k < GROUPS; ++k) t += s_acc[k][threadIdx.x];
         a.partials[(size_t)blockIdx.x * 32 + threadIdx.x] = t;
+        s_solve.S[threadIdx.x] = t;  // (input of the warm-up below)
         __threadfence();
     }
     __syncthreads();
@@ -879,7 +937,10 @@ __device__ void icp_reduce_body(const IcpArgs &a, double (*s_acc)[32], unsigned 
         *s_last = (t == a.reduce_grid - 1) ? 1u : 0u;
     }
     __syncthreads();
-    if (!*s_last) return;
+    if (!*s_last) {
+        warm_solve<KIND>(a, s_solve);  // (see icp_static_tail)
+        return;
+    }
     __threadfence();
     if (threadIdx.x == 0) {
         prefetch_l1(&st->T[0]);

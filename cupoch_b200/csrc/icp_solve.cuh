@@ -169,11 +169,35 @@ __device__ bool solve_jtj(const double *S, float det_thresh, float *T) {
     se3_exp(x, T);
     return true;
 }
+__device__ __noinline__ float det_core(const double *S) {
+    float A[36], b[6];
+    jtj_system(S, A, b);
+    return det6_partial_piv(A);
+}
+__device__ __noinline__ void solve_core(const double *S, float *T) {
+    float A[36], b[6], x[6];
+    jtj_system(S, A, b);
+    ldlt6_solve(A, b, x);
+    se3_exp(x, T);
+}
 struct SolveSmem {
     float T[16];
     double S[32];  // the iteration's 32 sums, staged for the solving lane
     float det;     // icp_finalize<KIND, true>: the determinant, computed by a second warp while the first one solves
 };
+// Called by every warp of a block that is NOT the last to arrive, after a __syncthreads that made m.S (this block's own
+// partial sums) visible: lane 0 of warp 0 runs the solve and lane 0 of warp 1 the determinant, the very functions
+// icp_finalize<KIND, true> calls, and the results are dropped.  Only their instructions matter: the iteration's working
+// set evicts the kernel's code from L2 between launches, so the last block's single-lane solve would otherwise fetch its
+// unrolled code line by line from HBM (config 2 on the H100, launch 20: 9.1 us cold, 2.6 us warm; DESIGN section 5).
+template <int KIND>
+__device__ void warm_solve(const IcpArgs &a, SolveSmem &m) {
+    if (KIND == CPHB_EST_POINT_TO_POINT || lane_id() != 0) return;  // (Kabsch: a different, shorter epilogue)
+    constexpr bool uses_det = (KIND != CPHB_EST_GENERALIZED_ICP);
+    const int warp = threadIdx.x >> 5;
+    if (warp == 0) solve_core(m.S, m.T);
+    else if (warp == 1 && uses_det && a.det_thresh > 0) m.det = det_core(m.S);
+}
 
 __device__ void matmul4(const float *A, const float *B, float *C) {  // registration.cu:159
     float R[16];
@@ -279,11 +303,7 @@ __device__ void icp_finalize(const IcpArgs &a, IcpState *st, SolveSmem &m) {
     if (PAR) {
         const int warp = threadIdx.x >> 5;
         constexpr bool uses_det = (KIND != CPHB_EST_POINT_TO_POINT && KIND != CPHB_EST_GENERALIZED_ICP);
-        if (warp == 1 && lane == 0 && uses_det && a.det_thresh > 0) {
-            float A[36], b[6];
-            jtj_system(S, A, b);
-            m.det = det6_partial_piv(A);
-        }
+        if (warp == 1 && lane == 0 && uses_det && a.det_thresh > 0) m.det = det_core(S);
         if (warp != 0) {
             __syncthreads();
             return;
@@ -339,12 +359,7 @@ __device__ void icp_finalize(const IcpArgs &a, IcpState *st, SolveSmem &m) {
                 // __syncwarp-separated steps)
                 bool ok = true;
                 if (PAR) {
-                    if (lane == 0) {  // solve first, learn the determinant afterwards (it only decides accept / reject)
-                        float A[36], b[6], x[6];
-                        jtj_system(S, A, b);
-                        ldlt6_solve(A, b, x);
-                        se3_exp(x, m.T);
-                    }
+                    if (lane == 0) solve_core(S, m.T);  // solve first, learn the determinant afterwards (it only decides accept / reject)
                     __syncthreads();
                     joined = true;
                     if (lane == 0) {

@@ -62,6 +62,8 @@ _SIGNATURES = {
                                             C.POINTER(C.c_size_t), _P]),
     "cphb_voxel_grid_create_dense": (C.c_int, [C.c_float, C.c_float, C.c_float, C.c_float, _P, _P, C.c_size_t,
                                                C.POINTER(C.c_size_t), _P]),
+    "cphb_voxel_grid_from_triangle_mesh": (C.c_int, [_P, C.c_size_t, _P, C.c_size_t, C.c_float, C.POINTER(C.c_float),
+                                                     C.POINTER(C.c_float), _P, _P, C.c_size_t, C.POINTER(C.c_size_t), _P]),
     "cphb_voxel_grid_check_if_included": (C.c_int, [_P, C.c_size_t, C.c_float, _F3, _P, C.c_size_t, _P, _P]),
     "cphb_voxel_grid_has_key": (C.c_int, [_P, C.c_size_t, _I3, C.POINTER(C.c_int), _P]),
     "cphb_voxel_grid_carve": (C.c_int, [_P, _P, C.c_size_t, C.c_float, _F3, _P, C.c_int, C.c_int, C.c_int, C.c_int, _F3, _F3,

@@ -171,6 +171,8 @@ int cphb_sort_pairs_u32(const uint32_t *keys_in, uint32_t *keys_out, const uint3
                         uint32_t *vals_out, size_t n, int bits, cudaStream_t s);
 int cphb_sort_pairs_u64(const uint64_t *keys_in, uint64_t *keys_out, const uint32_t *vals_in,
                         uint32_t *vals_out, size_t n, int bits, cudaStream_t s);
+// the same sort of u64 keys alone (VoxelGrid::CreateFromTriangleMesh's packed keys)
+int cphb_sort_keys_u64(const uint64_t *keys_in, uint64_t *keys_out, size_t n, int bits, cudaStream_t s);
 
 // stable compaction (filters.cu): ascending positions i < n with keep[i] != 0 -> indices_out, their number to
 // *h_n_out (synchronises the stream)

@@ -9,6 +9,8 @@
 // bit-exact.
 #include <math.h>
 
+#include <cub/device/device_scan.cuh>
+
 #include "voxelkey.cuh"
 
 struct VgParams {
@@ -664,4 +666,447 @@ extern "C" int cphb_point_cloud_from_occgrid(const cphb_occgrid *grid, float *ou
     const float c = (float)(-(res / 2) + 0.5);
     CPHB_LAUNCH(vgo_occ_points_kernel, vgo_grid(cnt), VGO_BLOCK, 0, s, cells, cnt, c, vs, o[0], o[1], o[2], out_points, out_colors);
     return cphb_read_back(nullptr, nullptr, 0, s, who);
+}
+
+// ------------------------------------------------------------------------------------------------ from a TriangleMesh
+// CreateFromTriangleMeshWithinBounds (voxelgrid_factory.cu:229-272; DESIGN section 4 item 25).  The reference runs
+// one thread per cell of the dense box and tests every triangle against it; here the work follows the surface:
+//   1. one thread per triangle checks its indices and finds, per axis, the exact range of cells whose centre passes
+//      the test's own box-axis comparison (a binary search on the float predicate, which is monotone in k), and its
+//      dominant normal axis d.  Its work items are the columns of that box along d (the cells in the other two axes);
+//   2. a 64-bit CUB exclusive scan of the column counts, then one thread per (triangle, column) finds its triangle by
+//      binary search and walks the cells of the column whose centre lies within the triangle plane's reach (the
+//      plane's slab in float64, widened by a bound on the float test's own rounding), testing each exactly;
+//   3. the hits go through the block compaction as packed keys, the radix sort and a head-flag unique, then are
+//      unpacked to [m][3].
+// A degenerate triangle (zero float64 normal) walks its whole box.  The walk only has to be a superset of the cells
+// that pass: the exact test decides every key, so the result does not depend on how the work is split.
+#define MV_BLOCK 256
+
+// component a of (x, y, z) for a run-time a, by selects (an indexed local array would live in local memory)
+template <class T>
+__host__ __device__ __forceinline__ T mv_pick(int a, T x, T y, T z) { return a == 0 ? x : (a == 1 ? y : z); }
+
+struct MvTri {
+    int lo[3], hi[3];  // per axis, the cells that pass the box-axis comparison
+    int d;             // column axis; + 4 when degenerate (the whole range is walked)
+};
+
+// cell centre on one axis: ((float)k + 0.5f) * vs + o, each step rounded (carving's rule, DESIGN item 17)
+// (plain operators: -fmad=false keeps every one rounded, and the host build of the tests' harness does the same)
+__host__ __device__ __forceinline__ float mv_centre(int k, float vs, float o) { return ((float)k + 0.5f) * vs + o; }
+
+__host__ __device__ __forceinline__ void mv_order(float a, float b, float &mn, float &mx) {
+    if (a < b) {
+        mn = a;
+        mx = b;
+    } else {
+        mn = b;
+        mx = a;
+    }
+}
+
+// Akenine-Moeller's triangle/box overlap test (the separating axes: 9 edge x box-axis cross products, then the 3 box
+// axes, then the triangle's plane), with the operand order and comparisons of the published triBoxOverlap.  c: box
+// centre, h: half size, A, B, C: the triangle.  IEEE float32, no contraction (-fmad=false); oracle/mesh_voxel.c
+// restates it.
+__host__ __device__ __forceinline__ bool mv_tri_box(const float c[3], float h, const float A[3], const float B[3], const float C[3]) {
+    float v0[3], v1[3], v2[3], e0[3], e1[3], e2[3];
+#pragma unroll
+    for (int q = 0; q < 3; ++q) {
+        v0[q] = A[q] - c[q];
+        v1[q] = B[q] - c[q];
+        v2[q] = C[q] - c[q];
+    }
+#pragma unroll
+    for (int q = 0; q < 3; ++q) {
+        e0[q] = v1[q] - v0[q];
+        e1[q] = v2[q] - v1[q];
+        e2[q] = v0[q] - v2[q];
+    }
+    float mn, mx, p0, p1, p2, rad, fx, fy, fz;
+    fx = fabsf(e0[0]), fy = fabsf(e0[1]), fz = fabsf(e0[2]);
+    p0 = e0[2] * v0[1] - e0[1] * v0[2], p2 = e0[2] * v2[1] - e0[1] * v2[2];  // x * e0
+    mv_order(p0, p2, mn, mx), rad = fz * h + fy * h;
+    if (mn > rad || mx < -rad) return false;
+    p0 = -e0[2] * v0[0] + e0[0] * v0[2], p2 = -e0[2] * v2[0] + e0[0] * v2[2];  // y * e0
+    mv_order(p0, p2, mn, mx), rad = fz * h + fx * h;
+    if (mn > rad || mx < -rad) return false;
+    p1 = e0[1] * v1[0] - e0[0] * v1[1], p2 = e0[1] * v2[0] - e0[0] * v2[1];  // z * e0
+    mv_order(p2, p1, mn, mx), rad = fy * h + fx * h;
+    if (mn > rad || mx < -rad) return false;
+    fx = fabsf(e1[0]), fy = fabsf(e1[1]), fz = fabsf(e1[2]);
+    p0 = e1[2] * v0[1] - e1[1] * v0[2], p2 = e1[2] * v2[1] - e1[1] * v2[2];  // x * e1
+    mv_order(p0, p2, mn, mx), rad = fz * h + fy * h;
+    if (mn > rad || mx < -rad) return false;
+    p0 = -e1[2] * v0[0] + e1[0] * v0[2], p2 = -e1[2] * v2[0] + e1[0] * v2[2];  // y * e1
+    mv_order(p0, p2, mn, mx), rad = fz * h + fx * h;
+    if (mn > rad || mx < -rad) return false;
+    p0 = e1[1] * v0[0] - e1[0] * v0[1], p1 = e1[1] * v1[0] - e1[0] * v1[1];  // z * e1
+    mv_order(p0, p1, mn, mx), rad = fy * h + fx * h;
+    if (mn > rad || mx < -rad) return false;
+    fx = fabsf(e2[0]), fy = fabsf(e2[1]), fz = fabsf(e2[2]);
+    p0 = e2[2] * v0[1] - e2[1] * v0[2], p1 = e2[2] * v1[1] - e2[1] * v1[2];  // x * e2
+    mv_order(p0, p1, mn, mx), rad = fz * h + fy * h;
+    if (mn > rad || mx < -rad) return false;
+    p0 = -e2[2] * v0[0] + e2[0] * v0[2], p1 = -e2[2] * v1[0] + e2[0] * v1[2];  // y * e2
+    mv_order(p0, p1, mn, mx), rad = fz * h + fx * h;
+    if (mn > rad || mx < -rad) return false;
+    p1 = e2[1] * v1[0] - e2[0] * v1[1], p2 = e2[1] * v2[0] - e2[0] * v2[1];  // z * e2
+    mv_order(p2, p1, mn, mx), rad = fy * h + fx * h;
+    if (mn > rad || mx < -rad) return false;
+#pragma unroll
+    for (int q = 0; q < 3; ++q) {  // the box axes
+        mn = mx = v0[q];
+        if (v1[q] < mn) mn = v1[q];
+        if (v1[q] > mx) mx = v1[q];
+        if (v2[q] < mn) mn = v2[q];
+        if (v2[q] > mx) mx = v2[q];
+        if (mn > h || mx < -h) return false;
+    }
+    const float n[3] = {e0[1] * e1[2] - e0[2] * e1[1], e0[2] * e1[0] - e0[0] * e1[2], e0[0] * e1[1] - e0[1] * e1[0]};
+    float vmin[3], vmax[3];
+#pragma unroll
+    for (int q = 0; q < 3; ++q) {
+        if (n[q] > 0.f) {
+            vmin[q] = -h - v0[q];
+            vmax[q] = h - v0[q];
+        } else {
+            vmin[q] = h - v0[q];
+            vmax[q] = -h - v0[q];
+        }
+    }
+    if (n[0] * vmin[0] + n[1] * vmin[1] + n[2] * vmin[2] > 0.f) return false;
+    return n[0] * vmax[0] + n[1] * vmax[1] + n[2] * vmax[2] >= 0.f;
+}
+
+// the first k in [lo, hi] at which a predicate that is false, then true, turns true; hi + 1 when it never does
+template <class P>
+__host__ __device__ __forceinline__ int mv_first(int lo, int hi, P p) {
+    int a = lo, b = hi + 1;
+    while (a < b) {
+        const int m = a + ((b - a) >> 1);
+        if (p(m)) b = m;
+        else a = m + 1;
+    }
+    return a;
+}
+
+struct MvGrid {
+    float o[3], vs, h;
+    int n[3];
+};
+
+__host__ __device__ __forceinline__ bool mv_load(const float *__restrict__ vtx, const int32_t *__restrict__ tri, size_t t, float P[3][3]) {
+    bool finite = true;
+#pragma unroll
+    for (int j = 0; j < 3; ++j) {
+        const size_t v = (size_t)tri[3 * t + j];
+#pragma unroll
+        for (int q = 0; q < 3; ++q) {
+            P[j][q] = vtx[3 * v + q];
+            finite = finite && isfinite(P[j][q]);
+        }
+    }
+    return finite;
+}
+
+// the triangle's normal (v1 - v0) x (v2 - v1) in float64, the orientation of the float test's normal
+__host__ __device__ __forceinline__ void mv_normal64(const float P[3][3], double nD[3]) {
+    double e0[3], e1[3];
+#pragma unroll
+    for (int q = 0; q < 3; ++q) {
+        e0[q] = (double)P[1][q] - (double)P[0][q];
+        e1[q] = (double)P[2][q] - (double)P[1][q];
+    }
+    nD[0] = e0[1] * e1[2] - e0[2] * e1[1];
+    nD[1] = e0[2] * e1[0] - e0[0] * e1[2];
+    nD[2] = e0[0] * e1[1] - e0[1] * e1[0];
+}
+
+// a finite triangle's record and its column count (0 when its box misses the grid)
+__host__ __device__ __forceinline__ unsigned long long mv_setup(const float P[3][3], const MvGrid &g, MvTri &r) {
+    long long span[3];
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+        const float mn = fminf(fminf(P[0][a], P[1][a]), P[2][a]), mx = fmaxf(fmaxf(P[0][a], P[1][a]), P[2][a]);
+        const float o = g.o[a], vs = g.vs, h = g.h;
+        // the test's box-axis comparison: min_j (v_j - c) > h or max_j (v_j - c) < -h rejects, and v - c is monotone in c
+        r.lo[a] = mv_first(0, g.n[a] - 1, [&](int k) { return mn - mv_centre(k, vs, o) <= h; });
+        r.hi[a] = mv_first(0, g.n[a] - 1, [&](int k) { return !(mx - mv_centre(k, vs, o) >= -h); }) - 1;
+        span[a] = (long long)r.hi[a] - r.lo[a] + 1;
+        if (span[a] <= 0) return 0ull;
+    }
+    double nD[3];
+    mv_normal64(P, nD);
+    const double m0 = fabs(nD[0]), m1 = fabs(nD[1]), m2 = fabs(nD[2]);
+    if (m0 + m1 + m2 > 0.0) {
+        r.d = (m0 >= m1 && m0 >= m2) ? 0 : (m1 >= m2 ? 1 : 2);
+    } else {  // degenerate: walk the longest axis of the box
+        r.d = (span[0] >= span[1] && span[0] >= span[2]) ? 0 : (span[1] >= span[2] ? 1 : 2);
+        r.d += 4;
+    }
+    const int d = r.d & 3;
+    return (unsigned long long)mv_pick((d + 1) % 3, span[0], span[1], span[2]) * (unsigned long long)mv_pick((d + 2) % 3, span[0], span[1], span[2]);
+}
+
+__global__ void __launch_bounds__(MV_BLOCK) mv_setup_kernel(const float *__restrict__ vtx, size_t nv, const int32_t *__restrict__ tri, size_t nt,
+                                                            MvGrid g, MvTri *__restrict__ info, unsigned long long *__restrict__ cols,
+                                                            unsigned long long *__restrict__ bad) {
+    const size_t t = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+    if (t > nt) return;
+    if (t == nt) {  // the scan's extra entry: its exclusive sum is the total
+        cols[nt] = 0ull;
+        return;
+    }
+    cols[t] = 0ull;
+    bool ok = true;
+#pragma unroll
+    for (int j = 0; j < 3; ++j) {
+        const int32_t v = tri[3 * t + j];
+        ok = ok && v >= 0 && (size_t)v < nv;
+    }
+    if (!ok) {
+        *bad = 1ull;
+        return;
+    }
+    float P[3][3];
+    if (!mv_load(vtx, tri, t, P)) return;  // a non-finite vertex meets no cell
+    MvTri r;
+    const unsigned long long c = mv_setup(P, g, r);
+    if (c) {
+        info[t] = r;
+        cols[t] = c;
+    }
+}
+
+// one work item: a column of one triangle along axis d, at cells ki, kj on axes i = (d + 1) % 3, j = (d + 2) % 3
+// (centres ci, cj); the walk tests cells k0 .. k0 + len - 1 along d
+struct MvColumn {
+    float P[3][3];
+    float ci, cj;
+    int ki, kj, k0, d;
+};
+
+__host__ __device__ __forceinline__ int mv_column(const float *__restrict__ vtx, const int32_t *__restrict__ tri, size_t nt, const MvTri *__restrict__ info,
+                                         const unsigned long long *__restrict__ off, unsigned long long w, unsigned long long W, const MvGrid &g,
+                                         MvColumn &col) {
+    col.d = 0;
+    col.ci = col.cj = 0.f;
+    col.ki = col.kj = col.k0 = 0;
+    if (w >= W) return 0;
+    size_t a = 0, b = nt;  // the last triangle whose first item is <= w
+    while (b - a > 1) {
+        const size_t m = (a + b) >> 1;
+        if (off[m] <= w) a = m;
+        else b = m;
+    }
+    const size_t t = a;
+    const MvTri r = info[t];
+    const int d = r.d & 3, i = (d + 1) % 3, j = (d + 2) % 3;
+    col.d = d;
+    const int loi = mv_pick(i, r.lo[0], r.lo[1], r.lo[2]), loj = mv_pick(j, r.lo[0], r.lo[1], r.lo[2]);
+    const int hij = mv_pick(j, r.hi[0], r.hi[1], r.hi[2]);
+    const unsigned long long local = w - off[t], nj = (unsigned long long)(hij - loj + 1);
+    col.ki = loi + (int)(local / nj);
+    col.kj = loj + (int)(local % nj);
+    col.ci = mv_centre(col.ki, g.vs, mv_pick(i, g.o[0], g.o[1], g.o[2]));
+    col.cj = mv_centre(col.kj, g.vs, mv_pick(j, g.o[0], g.o[1], g.o[2]));
+    mv_load(vtx, tri, t, col.P);
+    int k0 = mv_pick(d, r.lo[0], r.lo[1], r.lo[2]), k1 = mv_pick(d, r.hi[0], r.hi[1], r.hi[2]);
+    if (!(r.d & 4)) {
+        // The plane meets the closed cell of centre c when |n . (P0 - c)| <= h (|n0| + |n1| + |n2|), i.e. c_d within
+        // rr of tc.  The float test computes its normal per cell from centre-relative vertices (|v| <= V = E + vs for
+        // every cell that passes the box axes, E the triangle's extent), so its normal is off by about u E V and its
+        // dot by about u |n| V (u = 2^-24): the slab is widened by 2^-16 (E V^2 / |n_d| + 4 V), far above those, plus
+        // 2^-140 / |n_d| for underflow in the float products.
+        double nD[3];
+        mv_normal64(col.P, nD);
+        const double nd = mv_pick(d, nD[0], nD[1], nD[2]), ni = mv_pick(i, nD[0], nD[1], nD[2]), nj2 = mv_pick(j, nD[0], nD[1], nD[2]);
+        double E = 0.0;
+#pragma unroll
+        for (int q = 0; q < 3; ++q) {
+            const double lo = fmin(fmin((double)col.P[0][q], (double)col.P[1][q]), (double)col.P[2][q]);
+            const double hi = fmax(fmax((double)col.P[0][q], (double)col.P[1][q]), (double)col.P[2][q]);
+            E = fmax(E, hi - lo);
+        }
+        const double V = E + (double)g.vs, ad = fabs(nd);
+        const double slack = 0x1p-16 * (E * V * V / ad + 4.0 * V) + 0x1p-140 / ad;
+        const double p0i = mv_pick(i, col.P[0][0], col.P[0][1], col.P[0][2]), p0j = mv_pick(j, col.P[0][0], col.P[0][1], col.P[0][2]);
+        const double p0d = mv_pick(d, col.P[0][0], col.P[0][1], col.P[0][2]);
+        const double tc = p0d + (ni * (p0i - (double)col.ci) + nj2 * (p0j - (double)col.cj)) / nd;
+        const double rr = (double)g.h * (fabs(nD[0]) + fabs(nD[1]) + fabs(nD[2])) / ad;
+        const double clo = tc - rr - slack, chi = tc + rr + slack;
+        const float o = mv_pick(d, g.o[0], g.o[1], g.o[2]), vs = g.vs;
+        const int lo = k0, hi = k1;
+        k0 = mv_first(lo, hi, [&](int k) { return (double)mv_centre(k, vs, o) >= clo; });
+        k1 = mv_first(lo, hi, [&](int k) { return (double)mv_centre(k, vs, o) > chi; }) - 1;
+    }
+    col.k0 = k0;
+    return k1 >= k0 ? k1 - k0 + 1 : 0;
+}
+
+// step s of the walk: whether cell k0 + s of the column passes the test; its key to key[]
+__host__ __device__ __forceinline__ bool mv_step_hit(int s, int len, const MvColumn &col, const MvGrid &g, int key[3]) {
+    if (s >= len) return false;
+    const int kd = col.k0 + s, d = col.d;
+    const float cd = mv_centre(kd, g.vs, mv_pick(d, g.o[0], g.o[1], g.o[2]));
+    float c[3];
+#pragma unroll
+    for (int q = 0; q < 3; ++q) {
+        c[q] = q == d ? cd : (q == (d + 1) % 3 ? col.ci : col.cj);
+        key[q] = q == d ? kd : (q == (d + 1) % 3 ? col.ki : col.kj);
+    }
+    return mv_tri_box(c, g.h, col.P[0], col.P[1], col.P[2]);
+}
+
+// per block: the number of hits (block_flag_count per step of the walk); their total to *hits
+__global__ void __launch_bounds__(MV_BLOCK) mv_count_kernel(const float *__restrict__ vtx, const int32_t *__restrict__ tri, size_t nt,
+                                                            const MvTri *__restrict__ info, const unsigned long long *__restrict__ off,
+                                                            unsigned long long W, MvGrid g, unsigned *__restrict__ counts,
+                                                            unsigned long long *__restrict__ hits) {
+    MvColumn col;
+    int key[3];
+    const int len = mv_column(vtx, tri, nt, info, off, blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x, W, g, col);
+    unsigned total = 0;
+    for (int s = 0; __syncthreads_or(s < len); ++s) total += block_flag_count(mv_step_hit(s, len, col, g, key));
+    if (threadIdx.x == 0) {
+        counts[blockIdx.x] = total;
+        atomicAdd(hits, (unsigned long long)total);
+    }
+}
+
+// the same walk; hit r of the block goes to keys[offsets[block] + r], packed x | y | z with z lowest.  keys[n_hits]
+// gets the sentinel (every sorted bit set), which sorts last, so the sort and the unique run on every non-empty input.
+__global__ void __launch_bounds__(MV_BLOCK) mv_write_kernel(const float *__restrict__ vtx, const int32_t *__restrict__ tri, size_t nt,
+                                                            const MvTri *__restrict__ info, const unsigned long long *__restrict__ off,
+                                                            unsigned long long W, MvGrid g, const unsigned *__restrict__ offsets, int sy,
+                                                            int sz, uint64_t sentinel, size_t n_hits, uint64_t *__restrict__ keys) {
+    MvColumn col;
+    int key[3];
+    const int len = mv_column(vtx, tri, nt, info, off, blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x, W, g, col);
+    if (blockIdx.x == 0 && threadIdx.x == 0) keys[n_hits] = sentinel;
+    size_t base = offsets[blockIdx.x];
+    for (int s = 0; __syncthreads_or(s < len); ++s) {
+        const bool hit = mv_step_hit(s, len, col, g, key);
+        const unsigned r = block_flag_rank(hit);
+        if (hit) keys[base + r] = ((uint64_t)key[0] << sy) | ((uint64_t)key[1] << sz) | (uint64_t)key[2];
+        base += __syncthreads_count(hit);
+    }
+}
+
+// thrust::unique of the sorted keys [0, n) as a block compaction (the sentinel at n is never kept)
+__device__ __forceinline__ bool mv_first_of_run(const uint64_t *k, size_t i, size_t n) { return i < n && (i == 0 || k[i] != k[i - 1]); }
+__global__ void __launch_bounds__(MV_BLOCK) mv_unique_count_kernel(const uint64_t *__restrict__ k, size_t n, unsigned *__restrict__ counts) {
+    const unsigned c = block_flag_count(mv_first_of_run(k, blockIdx.x * (size_t)blockDim.x + threadIdx.x, n));
+    if (threadIdx.x == 0) counts[blockIdx.x] = c;
+}
+// rows are written only when the total fits the capacity
+__global__ void __launch_bounds__(MV_BLOCK) mv_unique_write_kernel(const uint64_t *__restrict__ k, size_t n, const unsigned *__restrict__ offsets,
+                                                                   const unsigned *__restrict__ total, size_t capacity, int sy, int sz,
+                                                                   int32_t *__restrict__ out_keys, float *__restrict__ out_colors) {
+    const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+    const bool v = mv_first_of_run(k, i, n);
+    const unsigned r = block_flag_rank(v);
+    if (v && out_keys && *total <= capacity) {
+        const size_t o = offsets[blockIdx.x] + (size_t)r;
+        const uint64_t key = k[i];
+        out_keys[3 * o] = (int32_t)(key >> sy);
+        out_keys[3 * o + 1] = (int32_t)((key >> sz) & ((1ull << (sy - sz)) - 1ull));
+        out_keys[3 * o + 2] = (int32_t)(key & ((1ull << sz) - 1ull));
+        out_colors[3 * o] = 1.f;  // Voxel's default colour (voxelgrid.h:61)
+        out_colors[3 * o + 1] = 1.f;
+        out_colors[3 * o + 2] = 1.f;
+    }
+}
+
+extern "C" int cphb_voxel_grid_from_triangle_mesh(const float *vertices, size_t n_vertices, const int32_t *triangles, size_t n_triangles,
+                                                  float voxel_size, const float h_min_bound[3], const float h_max_bound[3], int32_t *out_keys,
+                                                  float *out_colors, size_t capacity, size_t *h_n, void *stream) {
+    cudaStream_t s = (cudaStream_t)stream;
+    const char *who = "cphb_voxel_grid_from_triangle_mesh";
+    if (!h_n || !h_min_bound || !h_max_bound) return vgo_invalid(who, "null argument");
+    *h_n = 0;
+    if (!(isfinite(voxel_size) && voxel_size > 0.f)) return vgo_invalid(who, "voxel_size is not positive and finite");
+    MvGrid g;
+    g.vs = voxel_size;
+    g.h = voxel_size * 0.5f;
+    for (int a = 0; a < 3; ++a) {
+        if (!isfinite(h_min_bound[a]) || !isfinite(h_max_bound[a])) return vgo_invalid(who, "the bounds are not finite");
+        const volatile float ext = h_max_bound[a] - h_min_bound[a];
+        const volatile float q = ext / voxel_size;  // int(std::round(extent / voxel_size)) in float, as CreateDense
+        const float c = roundf(q);
+        if (!(c >= 0.f && c < (float)(1 << CPHB_KEY_AXIS_BITS))) {
+            cphb_set_error("%s: axis %d count round(%g / %g) is negative or >= 2^%d", who, a, (double)ext, (double)voxel_size,
+                           CPHB_KEY_AXIS_BITS);
+            return CPHB_ERR_INVALID;
+        }
+        g.n[a] = (int)c;
+        g.o[a] = h_min_bound[a];
+    }
+    if (n_triangles == 0) return CPHB_OK;
+    if (!triangles || (n_vertices && !vertices) || (capacity && (!out_keys || !out_colors))) return vgo_invalid(who, "null argument");
+    if (n_triangles > (size_t)INT32_MAX) return vgo_invalid(who, "more than 2^31-1 triangles");
+    const int bx = bits_for_span(g.n[0]), by = bits_for_span(g.n[1]), bz = bits_for_span(g.n[2]);
+    const int sz = bz, sy = by + bz, bits = bx + by + bz;
+    const uint64_t sentinel = ~0ull >> (64 - bits);
+
+    cphb_scratch sc(s);
+    unsigned long long *meta = nullptr, *cols = nullptr, *off = nullptr;  // meta: index error, columns, hits
+    MvTri *info = nullptr;
+    int rc = sc.alloc(&meta, 4);
+    if (!rc) rc = sc.alloc(&cols, n_triangles + 1);
+    if (!rc) rc = sc.alloc(&off, n_triangles + 1);
+    if (!rc) rc = sc.alloc(&info, n_triangles);
+    if (rc) return rc;
+    CPHB_CUDA(cudaMemsetAsync(meta, 0, 4 * sizeof(unsigned long long), s));
+    CPHB_LAUNCH(mv_setup_kernel, vgo_grid(n_triangles + 1), MV_BLOCK, 0, s, vertices, n_vertices, triangles, n_triangles, g, info, cols, meta);
+    size_t tmp_bytes = 0;
+    CPHB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, cols, off, (int64_t)(n_triangles + 1), s));
+    char *tmp = nullptr;
+    rc = sc.alloc(&tmp, tmp_bytes ? tmp_bytes : 16);
+    if (rc) return rc;
+    CPHB_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, cols, off, (int64_t)(n_triangles + 1), s));
+    g_cphb_launches += 2;  // CUB's init and scan kernels
+    CPHB_CUDA(cudaMemcpyAsync(meta + 1, off + n_triangles, sizeof(unsigned long long), cudaMemcpyDeviceToDevice, s));
+    unsigned long long h_meta[2] = {0ull, 0ull};
+    rc = cphb_read_back(h_meta, meta, 2 * sizeof(unsigned long long), s, who);
+    if (rc) return rc;
+    if (h_meta[0]) return vgo_invalid(who, "a triangle's vertex index is outside [0, n_vertices)");
+    const unsigned long long W = h_meta[1];
+    if (W > (unsigned long long)INT32_MAX * MV_BLOCK) return vgo_invalid(who, "more than 2^39 triangle columns");
+    const unsigned nb = W ? (unsigned)((W + MV_BLOCK - 1) / MV_BLOCK) : 1u;
+
+    unsigned *counts = nullptr, *total = nullptr;
+    rc = sc.alloc(&counts, (size_t)nb + 4);
+    if (!rc) rc = sc.alloc(&total, 1);
+    if (rc) return rc;
+    CPHB_LAUNCH(mv_count_kernel, nb, MV_BLOCK, 0, s, vertices, triangles, n_triangles, info, off, W, g, counts, meta + 2);
+    cphb_scan_block_counts(counts, nb, total, s);
+    unsigned long long H = 0;
+    rc = cphb_read_back(&H, meta + 2, sizeof(H), s, who);
+    if (rc) return rc;
+    if (H >= (unsigned long long)INT32_MAX) return vgo_invalid(who, "2^31-1 or more triangle/cell hits");
+
+    uint64_t *keys = nullptr, *skeys = nullptr;
+    unsigned *ucounts = nullptr, *utotal = nullptr;
+    const size_t nk = (size_t)H + 1;
+    const unsigned nbu = (unsigned)((nk + MV_BLOCK - 1) / MV_BLOCK);
+    rc = sc.alloc(&keys, nk);
+    if (!rc) rc = sc.alloc(&skeys, nk);
+    if (!rc) rc = sc.alloc(&ucounts, (size_t)nbu + 4);
+    if (!rc) rc = sc.alloc(&utotal, 1);
+    if (rc) return rc;
+    CPHB_LAUNCH(mv_write_kernel, nb, MV_BLOCK, 0, s, vertices, triangles, n_triangles, info, off, W, g, counts, sy, sz, sentinel, (size_t)H,
+                keys);
+    rc = cphb_sort_keys_u64(keys, skeys, nk, bits, s);
+    if (rc) return rc;
+    CPHB_LAUNCH(mv_unique_count_kernel, nbu, MV_BLOCK, 0, s, skeys, (size_t)H, ucounts);
+    cphb_scan_block_counts(ucounts, nbu, utotal, s);
+    CPHB_LAUNCH(mv_unique_write_kernel, nbu, MV_BLOCK, 0, s, skeys, (size_t)H, ucounts, utotal, capacity, sy, sz, out_keys, out_colors);
+    unsigned m = 0;
+    rc = cphb_read_back(&m, utotal, sizeof(m), s, who);
+    if (rc) return rc;
+    *h_n = m;
+    return CPHB_OK;
 }

@@ -516,8 +516,9 @@ _SCOPE_MASK = {FilterScope.All: 7, FilterScope.Vertex: 1, FilterScope.Normal: 2,
 class TriangleMesh:
     """geometry::TriangleMesh (trianglemesh.h): vertices_, triangles_ (int32 vertex indices), vertex_colors_,
     vertex_normals_, triangle_normals_ and edge_list_ (int32 pairs) on the device.  The normal computations,
-    ComputeEdgeList, the four vertex filters, GetSurfaceArea and SamplePointsUniformly run here; mesh IO, cleanup,
-    primitives and textures are not provided."""
+    ComputeEdgeList, the four vertex filters, GetSurfaceArea, SamplePointsUniformly and the bounds run here, and
+    VoxelGrid.create_from_triangle_mesh[_within_bounds] turns a mesh into a grid; mesh IO, cleanup, primitives and
+    textures are not provided."""
 
     def __init__(self, vertices=None, triangles=None):
         self._vertices = self._triangles = self._vertex_colors = self._vertex_normals = self._triangle_normals = None
@@ -562,6 +563,21 @@ class TriangleMesh:
 
     def has_edge_list(self):
         return self._n(self._edge_list) > 0
+
+    def get_min_bound(self):
+        """MeshBase::GetMinBound: the smallest coordinate of all vertices per axis, (0, 0, 0) without vertices"""
+        return self._bounds()[0]
+
+    def get_max_bound(self):
+        """MeshBase::GetMaxBound: the largest coordinate of all vertices per axis, (0, 0, 0) without vertices"""
+        return self._bounds()[1]
+
+    def _bounds(self):
+        mn, mx = (C.c_float * 3)(), (C.c_float * 3)()
+        n = self._n(self._vertices)
+        if n:
+            _lib.check(_lib.lib().cphb_min_max_bound(self._vertices.ptr, n, mn, mx, None))
+        return np.array(mn, np.float32), np.array(mx, np.float32)
 
     def compute_triangle_normals(self, normalized=True):
         """ComputeTriangleNormals (trianglemesh.cu:466-477): (v1 - v0) x (v2 - v0) per triangle, then normalised when
@@ -1002,6 +1018,39 @@ class VoxelGrid:
             _lib.check(_lib.lib().cphb_voxel_grid_create_dense(*args, keys.ptr, cols.ptr, m, C.byref(n), None))
             out.voxels_keys, out.voxels_colors = keys, cols
         return out
+
+    @staticmethod
+    def create_from_triangle_mesh_within_bounds(input, voxel_size, min_bound, max_bound):
+        """VoxelGrid::CreateFromTriangleMeshWithinBounds (voxelgrid_factory.cu:229-272): origin = min_bound,
+        int(round(extent / voxel_size)) cells per axis; a cell is a voxel when Akenine-Moeller's triangle/box test says
+        some triangle meets it.  The cell tested for key k is centred at (k + 0.5) * voxel_size + origin, the cell
+        get_voxel gives (the reference tests the box centred on the voxel's lower corner).  Keys unique and in
+        lexicographic order, colours (1, 1, 1).  A triangle with a non-finite vertex meets no cell.  A bad vertex
+        index, a voxel size that is not positive and finite, non-finite bounds, or a count that is negative or >= 2^21
+        on an axis raise."""
+        out = VoxelGrid()
+        out.voxel_size = float(np.float32(voxel_size))
+        out.origin = np.asarray(min_bound, np.float32).reshape(3).copy()
+        nv, nt = TriangleMesh._n(input._vertices), TriangleMesh._n(input._triangles)
+        mn, mx = out._f3(), out._f3(max_bound)
+        args = (input._vertices.ptr if nv else None, nv, input._triangles.ptr if nt else None, nt, out.voxel_size, mn, mx)
+        L, n = _lib.lib(), C.c_size_t(0)
+        _lib.check(L.cphb_voxel_grid_from_triangle_mesh(*args, None, None, 0, C.byref(n), None))
+        m = n.value
+        if m:
+            keys, cols = DeviceArray((m, 3), np.int32), DeviceArray((m, 3), np.float32)
+            _lib.check(L.cphb_voxel_grid_from_triangle_mesh(*args, keys.ptr, cols.ptr, m, C.byref(n), None))
+            out.voxels_keys, out.voxels_colors = keys, cols
+        return out
+
+    @staticmethod
+    def create_from_triangle_mesh(input, voxel_size):
+        """VoxelGrid::CreateFromTriangleMesh (voxelgrid_factory.cu:274-281): the bounds of all vertices widened by half a
+        voxel"""
+        v = np.float32(voxel_size)
+        mn, mx = input._bounds()
+        return VoxelGrid.create_from_triangle_mesh_within_bounds(input, voxel_size, mn - v * np.float32(0.5),
+                                                                  mx + v * np.float32(0.5))
 
     @staticmethod
     def create_from_occupancy_grid(occupancy_grid):

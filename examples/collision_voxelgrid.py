@@ -1,6 +1,6 @@
 """collision::ComputeIntersection: a voxelised shape slid through a copy of itself (the reference's
 examples/python/robotics/collision_voxelgrid.py without the visualiser; the reference voxelises a mesh, here the
-VoxelGrid comes from a synthetic cloud on a sphere, and the query is moved by assigning its origin because there is no
+VoxelGrid comes from a synthetic cloud on a sphere (examples/voxelize_mesh.py voxelises a mesh), and the query is moved by assigning its origin because there is no
 VoxelGrid::Translate in this engine).  Then a box, a sphere and a capsule against the same grid."""
 import numpy as np
 

@@ -1,6 +1,6 @@
 """geometry::DistanceTransform: the Euclidean distance field of a voxelised shape (the reference's
 examples/python/robotics/distancetransform.py voxelises a mesh; here the VoxelGrid comes from a synthetic cloud on a
-sphere, because mesh voxelisation is not part of this engine)."""
+sphere, and examples/voxelize_mesh.py runs the mesh flow with VoxelGrid.create_from_triangle_mesh_within_bounds)."""
 import numpy as np
 
 import cupoch_b200 as cph

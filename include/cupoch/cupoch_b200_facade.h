@@ -486,6 +486,7 @@ inline OrientedBoundingBox OrientedBoundingBox::CreateFromAxisAlignedBoundingBox
 class OccupancyGrid;
 class Image;
 class RGBDImage;
+class TriangleMesh;
 class PointCloud {
 public:
     PointCloud() {}
@@ -843,7 +844,8 @@ public:
     utility::device_vector<uint8_t> data_;
 };
 
-/// geometry::VoxelGrid (voxelgrid.h:84-160): creation from a point cloud (voxelgrid_factory.cu:164-228) and the
+/// geometry::VoxelGrid (voxelgrid.h:84-160): creation from a point cloud (voxelgrid_factory.cu:164-228) or a triangle
+/// mesh (:229-281) and the
 /// accessors, CreateDense, CheckIfIncluded, carving, += / AddVoxels, painting, SelectByIndex and CreateFromOccupancyGrid
 /// (voxelgrid.cu:235-475).  Keys and colours are kept as two device vectors (the reference zips keys with
 /// Voxel{grid_index, color}); GetVoxels() hands back the reference's pair.
@@ -906,6 +908,14 @@ public:
     }
     /// CreateFromOccupancyGrid (voxelgrid_factory.cu:283-305), defined after OccupancyGrid
     static std::shared_ptr<VoxelGrid> CreateFromOccupancyGrid(const OccupancyGrid &input);
+    /// CreateFromTriangleMeshWithinBounds (voxelgrid_factory.cu:229-272): int(round(extent / voxel_size)) cells per axis
+    /// from min_bound; a cell is a voxel when Akenine-Moeller's triangle/box test says some triangle meets it.  The cell
+    /// tested for key k is centred at (k + 0.5) voxel_size + origin, the cell GetVoxel gives (the reference tests the box
+    /// centred on the lower corner).  A bad vertex index, voxel size, bounds or count throws.  Defined after TriangleMesh.
+    static std::shared_ptr<VoxelGrid> CreateFromTriangleMeshWithinBounds(const TriangleMesh &input, float voxel_size,
+                                                                         const Eigen::Vector3f &min_bound, const Eigen::Vector3f &max_bound);
+    /// CreateFromTriangleMesh (voxelgrid_factory.cu:274-281): the mesh's vertex bounds widened by half a voxel
+    static std::shared_ptr<VoxelGrid> CreateFromTriangleMesh(const TriangleMesh &input, float voxel_size);
     /// CheckIfIncluded (voxelgrid.cu:365-376): whether each query's GetVoxel cell is a voxel (false for non-finite queries)
     std::vector<bool> CheckIfIncluded(const std::vector<Eigen::Vector3f> &queries) const {
         std::vector<bool> out(queries.size(), false);
@@ -1979,7 +1989,8 @@ public:
 
 /// geometry::TriangleMesh (trianglemesh.h, meshbase.h): vertices_, vertex_normals_, vertex_colors_, triangles_ (int32
 /// vertex indices), triangle_normals_ and edge_list_ on the device.  The two normal computations, ComputeEdgeList,
-/// the four vertex filters, GetSurfaceArea and SamplePointsUniformly are provided (no IO, cleanup or primitives).
+/// the four vertex filters, GetSurfaceArea, SamplePointsUniformly and GetMinBound / GetMaxBound are provided (no IO,
+/// cleanup or primitives).
 class TriangleMesh : public MeshBase {
 public:
     TriangleMesh() {}
@@ -2015,6 +2026,11 @@ public:
                                                     vertices_.size(), normalized ? 1 : 0, (float *)vertex_normals_.data(), nullptr));
         return *this;
     }
+
+    /// MeshBase::GetMinBound / GetMaxBound: the smallest / largest coordinate of all vertices per axis, (0, 0, 0)
+    /// without vertices
+    Eigen::Vector3f GetMinBound() const { return Bound(0); }
+    Eigen::Vector3f GetMaxBound() const { return Bound(1); }
 
     bool HasEdgeList() const { return edge_list_.size() > 0; }
     /// ComputeEdgeList (trianglemesh.cu:505-519): the directed edges (a, b) and (b, a) of every triangle edge, sorted and
@@ -2103,6 +2119,11 @@ private:
                                         nullptr));
         return mesh;
     }
+    Eigen::Vector3f Bound(int which) const {
+        float mn[3] = {0, 0, 0}, mx[3] = {0, 0, 0};
+        if (vertices_.size()) utility::check(cphb_min_max_bound((const float *)vertices_.data(), vertices_.size(), mn, mx, nullptr));
+        return which ? Eigen::Vector3f(mx[0], mx[1], mx[2]) : Eigen::Vector3f(mn[0], mn[1], mn[2]);
+    }
     float SurfaceArea(float *areas) const {
         float a = 0.f;
         if (triangles_.size())
@@ -2111,6 +2132,30 @@ private:
         return a;
     }
 };
+
+inline std::shared_ptr<VoxelGrid> VoxelGrid::CreateFromTriangleMeshWithinBounds(const TriangleMesh &input, float voxel_size,
+                                                                                const Eigen::Vector3f &min_bound,
+                                                                                const Eigen::Vector3f &max_bound) {
+    auto out = std::make_shared<VoxelGrid>();
+    out->voxel_size_ = voxel_size;
+    out->origin_ = min_bound;
+    const float mn[3] = {min_bound[0], min_bound[1], min_bound[2]}, mx[3] = {max_bound[0], max_bound[1], max_bound[2]};
+    const float *v = (const float *)input.vertices_.data();
+    const int32_t *t = (const int32_t *)input.triangles_.data();
+    const size_t nv = input.vertices_.size(), nt = input.triangles_.size();
+    size_t n = 0;
+    utility::check(cphb_voxel_grid_from_triangle_mesh(v, nv, t, nt, voxel_size, mn, mx, nullptr, nullptr, 0, &n, nullptr));
+    out->voxels_keys_.resize(n);
+    out->voxels_colors_.resize(n);
+    if (n) utility::check(cphb_voxel_grid_from_triangle_mesh(v, nv, t, nt, voxel_size, mn, mx, out->keys(), out->colors(), n, &n, nullptr));
+    return out;
+}
+inline std::shared_ptr<VoxelGrid> VoxelGrid::CreateFromTriangleMesh(const TriangleMesh &input, float voxel_size) {
+    const Eigen::Vector3f lo = input.GetMinBound(), hi = input.GetMaxBound();
+    const float h = voxel_size * 0.5f;
+    return CreateFromTriangleMeshWithinBounds(input, voxel_size, Eigen::Vector3f(lo[0] - h, lo[1] - h, lo[2] - h),
+                                              Eigen::Vector3f(hi[0] + h, hi[1] + h, hi[2] + h));
+}
 }  // namespace geometry
 
 namespace integration {

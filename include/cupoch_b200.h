@@ -489,6 +489,18 @@ int cphb_voxel_grid_select_by_index(const int32_t *keys, const float *colors, si
  * count; rows are written only when capacity >= it (capacity 0 sizes).  Synchronises. */
 int cphb_voxel_grid_from_occgrid(const cphb_occgrid *grid, int32_t *out_keys, float *out_colors, size_t capacity,
                                  size_t *h_count, float h_origin[3], void *stream);
+/* VoxelGrid::CreateFromTriangleMeshWithinBounds (voxelgrid_factory.cu:229-272, DESIGN section 4 item 25): origin =
+ * h_min_bound, n_a = int(roundf((max_a - min_a) / voxel_size)) cells per axis.  Key k (0 <= k_a < n_a) is a voxel when
+ * Akenine-Moeller's triangle/box overlap test, in IEEE float32, says some triangle meets the closed cell of centre
+ * ((float)k + 0.5f) * voxel_size + origin and half size 0.5f * voxel_size.  A triangle with a non-finite vertex
+ * meets no cell.  Keys are unique and in lexicographic order, colours (1, 1, 1).  vertices [n_vertices][3] float32,
+ * triangles [n_triangles][3] int32 (device).  *h_n = the voxel count; keys and colours are written only when capacity
+ * >= it (capacity 0 sizes; the sizing call does the same work).  A vertex index outside [0, n_vertices), a voxel size
+ * that is not positive and finite, non-finite bounds, or a count that is negative or >= 2^21 on an axis:
+ * CPHB_ERR_INVALID.  Synchronises. */
+int cphb_voxel_grid_from_triangle_mesh(const float *vertices, size_t n_vertices, const int32_t *triangles, size_t n_triangles,
+                                       float voxel_size, const float h_min_bound[3], const float h_max_bound[3], int32_t *out_keys,
+                                       float *out_colors, size_t capacity, size_t *h_n, void *stream);
 int cphb_point_cloud_from_occgrid(const cphb_occgrid *grid, float *out_points, float *out_colors, size_t capacity,
                                   size_t *h_count, void *stream);
 

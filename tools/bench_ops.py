@@ -55,7 +55,13 @@ def main():
     ap.add_argument("--mesh-ops", action="store_true",
                     help="instead: time TriangleMesh.compute_edge_list, the four filters at 1 and 100 iterations, "
                          "get_surface_area and sample_points_uniformly (1 M, 10 M points) on the --tsdf-mesh sphere meshes")
+    ap.add_argument("--mesh-voxel", action="store_true",
+                    help="instead: time VoxelGrid.create_from_triangle_mesh_within_bounds (sizing and writing call apart) on "
+                         "the --mesh-ops sphere meshes at 1x and 2x their voxel size, a two-triangle 512^2 plane and a coarse "
+                         "20-triangle solid in a 512^3 grid, with per-kernel times from torch.profiler")
     args = ap.parse_args()
+    if args.mesh_voxel:
+        return mesh_voxel(args.reps, args.out)
     if args.mesh_ops:
         return mesh_ops(args.reps, args.out)
     if args.depth_cloud:
@@ -1307,6 +1313,114 @@ def mesh_ops(reps, out=None):
     obj = {"op": "TriangleMesh edge list, filters, surface area and uniform sampling on the ExtractTriangleMesh meshes of "
                  "UniformTSDFVolume(2.0, res, 0.04, RGB8) after 8 640x480 ring-camera sphere views, with vertex normals and "
                  "colours", "gpu": gpu, "reps": reps, "rows": rows}
+    line = json.dumps(obj)
+    print(line)
+    if out:
+        with open(out, "w") as f:
+            f.write(line + "\n")
+
+
+def mesh_voxel_bytes(nv, nt, voxels):
+    """the compulsory bytes of one cphb_voxel_grid_from_triangle_mesh call, from shapes: the mesh read once (12 B a vertex,
+    12 B a triangle) and the keys and colours written (24 B a voxel).  The walk is bound by the exact test's arithmetic
+    and the sort, not by these bytes, so their share of 3.35 TB/s says how far the call is from a pure copy."""
+    return 12 * nv + 12 * nt + 24 * voxels
+
+
+def mesh_voxel(reps, out=None):
+    """VoxelGrid.create_from_triangle_mesh_within_bounds on: the --mesh-ops sphere meshes (UniformTSDFVolume(2.0, res,
+    0.04, RGB8), res 256 and 512, 8 ring-camera 640 x 480 views) at 1x and 2x their voxel size 2 / res over their
+    bounds widened by half a voxel; a tilted two-triangle plane over a 512^2 x 10 grid; an icosahedron of radius 200
+    in a 512^3 grid.  The sizing call (capacity 0) and the writing call are timed apart with CUDA events (median and
+    minimum of `reps` after a warm-up), with the engine launches of each; then one profiled pair per workload gives each
+    kernel's device time (torch.profiler).  mesh_voxel_bytes has the bytes model."""
+    import subprocess
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    import cupoch_b200 as cph
+    from cupoch_b200 import _lib
+    from cupoch_b200.testing.datagen import ring_cameras, sphere_depth
+    L = _lib.lib()
+    G, I = cph.geometry, cph.integration
+    gpu = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                         capture_output=True, text=True).stdout.strip()
+    ev = [L.cphb_event_create() for _ in range(2)]
+
+    def timed(fn):
+        times, launches = [], 0
+        for r in range(reps + 1):
+            n0 = L.cphb_launch_count()
+            L.cphb_event_record(ev[0], None)
+            fn()
+            L.cphb_event_record(ev[1], None)
+            ms = C.c_float(0)
+            _lib.check(L.cphb_event_elapsed_ms(ev[0], ev[1], C.byref(ms)))
+            launches = L.cphb_launch_count() - n0
+            if r:
+                times.append(ms.value)
+        return {"ms_median": float(np.median(times)), "ms_min": float(np.min(times)), "launches": int(launches)}
+
+    workloads = []
+    w, h = 640, 480
+    rng = np.random.default_rng(2)
+    for res in (256, 512):
+        vol = I.UniformTSDFVolume(2.0, res, 0.04, I.TSDFVolumeColorType.RGB8)
+        for K, E in ring_cameras(8, w, h):
+            d16 = np.round(sphere_depth(K, E, w, h, 0.6) * 1000).astype(np.uint16)
+            intr = cph.camera.PinholeCameraIntrinsic(w, h, K[0, 0], K[1, 1], K[0, 2], K[1, 2])
+            col = rng.integers(0, 256, (h, w, 3), dtype=np.uint8)
+            vol.integrate(G.RGBDImage.create_from_color_and_depth(G.Image(col), G.Image(d16), 1000.0, 100.0, False), intr, E)
+        mesh = vol.extract_triangle_mesh()
+        del vol
+        mn, mx = mesh.get_min_bound(), mesh.get_max_bound()
+        for f in (1, 2):
+            vs = np.float32(2.0 * f / res)
+            hv = vs * np.float32(0.5)
+            workloads.append(("sphere_res%d_x%d" % (res, f), mesh, float(vs), mn - hv, mx + hv))
+    plane = G.TriangleMesh(np.array([[0.1, 0.1, 3.2], [511.9, 0.1, 4.9], [0.1, 511.9, 3.7], [511.9, 511.9, 5.3]], np.float32),
+                           np.array([[0, 1, 2], [1, 3, 2]], np.int32))
+    workloads.append(("plane_512x512", plane, 1.0, np.zeros(3, np.float32), np.float32([512, 512, 10])))
+    p = (1 + 5 ** 0.5) / 2
+    iv = np.array([[-1, p, 0], [1, p, 0], [-1, -p, 0], [1, -p, 0], [0, -1, p], [0, 1, p], [0, -1, -p], [0, 1, -p], [p, 0, -1],
+                   [p, 0, 1], [-p, 0, -1], [-p, 0, 1]])
+    iv = (iv / np.linalg.norm(iv[0]) * 200.0 + [256.3, 255.7, 256.1]).astype(np.float32)
+    it = np.array([[0, 11, 5], [0, 5, 1], [0, 1, 7], [0, 7, 10], [0, 10, 11], [1, 5, 9], [5, 11, 4], [11, 10, 2], [10, 7, 6],
+                   [7, 1, 8], [3, 9, 4], [3, 4, 2], [3, 2, 6], [3, 6, 8], [3, 8, 9], [4, 9, 5], [2, 4, 11], [6, 2, 10], [8, 6, 7],
+                   [9, 8, 1]], np.int32)
+    workloads.append(("icosahedron_r200_in_512", G.TriangleMesh(iv, it), 1.0, np.zeros(3, np.float32), np.float32([512] * 3)))
+
+    rows = []
+    for name, mesh, vs, lo, hi in workloads:
+        nv, nt = len(mesh.vertices), len(mesh.triangles)
+        f3 = lambda a: (C.c_float * 3)(*[float(x) for x in a])
+        args = (mesh.vertices.ptr, nv, mesh.triangles.ptr, nt, vs, f3(lo), f3(hi))
+        n = C.c_size_t(0)
+        _lib.check(L.cphb_voxel_grid_from_triangle_mesh(*args, None, None, 0, C.byref(n), None))
+        m = n.value
+        keys, cols = cph.utility.DeviceArray((max(m, 1), 3), np.int32), cph.utility.DeviceArray((max(m, 1), 3), np.float32)
+        sizing = timed(lambda: _lib.check(L.cphb_voxel_grid_from_triangle_mesh(*args, None, None, 0, C.byref(n), None)))
+        writing = timed(lambda: _lib.check(L.cphb_voxel_grid_from_triangle_mesh(*args, keys.ptr, cols.ptr, m, C.byref(n), None)))
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            _lib.check(L.cphb_voxel_grid_from_triangle_mesh(*args, None, None, 0, C.byref(n), None))
+            _lib.check(L.cphb_voxel_grid_from_triangle_mesh(*args, keys.ptr, cols.ptr, m, C.byref(n), None))
+            torch.cuda.synchronize()
+        kernels = {}
+        for e in prof.key_averages():
+            t = getattr(e, "device_time_total", None) or getattr(e, "cuda_time_total", 0)
+            if t:
+                kernels[e.key[:80]] = {"calls": int(e.count), "us_total": float(t)}
+        cnt = [int(round((float(hi[a]) - float(lo[a])) / vs)) for a in range(3)]
+        bits = sum(max(1, int(np.ceil(np.log2(max(c, 2))))) for c in cnt)
+        nbytes = mesh_voxel_bytes(nv, nt, m)
+        row = {"workload": name, "vertices": nv, "triangles": nt, "voxel_size": vs, "grid": cnt, "voxels": m, "sizing_call": sizing,
+               "writing_call": writing, "both_calls_ms_median": sizing["ms_median"] + writing["ms_median"],
+               "compulsory_bytes": nbytes, "writing_call_share_of_3_35TBps": nbytes / (writing["ms_median"] * 1e-3) / HBM_BYTES_PER_S,
+               "kernels_us_both_calls": kernels, "sort_passes": (bits + 7) // 8}
+        rows.append(row)
+        print(json.dumps({k: row[k] for k in ("workload", "triangles", "voxels", "both_calls_ms_median")}), flush=True)
+    obj = {"op": "VoxelGrid.create_from_triangle_mesh_within_bounds (C entry point, sizing call then writing call)",
+           "gpu": gpu, "reps": reps, "rows": rows}
     line = json.dumps(obj)
     print(line)
     if out:

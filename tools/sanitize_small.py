@@ -68,3 +68,5 @@ filtered = [mesh.filter_sharpen(2, 0.1), mesh.filter_smooth_simple(2, G.FilterSc
 sampled = mesh.sample_points_uniformly(3000, True)
 print("mesh edges", len(mesh.edge_list), "filtered", [len(m.vertices) for m in filtered], "area %.4f" % mesh.get_surface_area(),
       "sampled", len(sampled.points), len(sampled.normals), len(sampled.colors))
+mesh_grid = G.VoxelGrid.create_from_triangle_mesh(mesh, 0.05)
+print("mesh voxels", len(mesh_grid), "within bounds", len(G.VoxelGrid.create_from_triangle_mesh_within_bounds(mesh, 0.1, (-1, -1, -1), (0.2, 1, 1))))

@@ -119,6 +119,12 @@ _SIGNATURES = {
                                    _P]),
     "cphb_mesh_surface_area": (C.c_int, [_P, C.c_size_t, _P, C.c_size_t, _P, C.POINTER(C.c_float), _P]),
     "cphb_mesh_sample_points_uniformly": (C.c_int, [_P, C.c_size_t, _P, C.c_size_t, _P, _P, _P, C.c_size_t, _P, _P, _P, _P]),
+    "cphb_mesh_remove_duplicated_vertices": (C.c_int, [_P, _P, _P, C.c_size_t, _P, C.c_size_t, _P, _P, _P, _P, C.POINTER(C.c_size_t), _P]),
+    "cphb_mesh_remove_duplicated_triangles": (C.c_int, [_P, _P, C.c_size_t, C.c_size_t, _P, _P, C.POINTER(C.c_size_t), _P]),
+    "cphb_mesh_remove_unreferenced_vertices": (C.c_int, [_P, _P, _P, C.c_size_t, _P, C.c_size_t, _P, _P, _P, _P, C.POINTER(C.c_size_t), _P]),
+    "cphb_mesh_remove_degenerate_triangles": (C.c_int, [_P, _P, C.c_size_t, C.c_size_t, _P, _P, C.POINTER(C.c_size_t), _P]),
+    "cphb_mesh_append_triangles": (C.c_int, [_P, C.c_size_t, C.c_size_t, _P, C.c_size_t, C.c_size_t, _P, _P]),
+    "cphb_mesh_self_intersecting_triangles": (C.c_int, [_P, C.c_size_t, _P, C.c_size_t, _P, C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t), _P]),
     "cphb_stsdf_create": (C.c_int, [C.c_float, C.c_float, C.c_int, C.c_int, C.c_int, _P, C.POINTER(_P)]),
     "cphb_stsdf_destroy": (None, [_P]),
     "cphb_stsdf_reset": (C.c_int, [_P, _P]),

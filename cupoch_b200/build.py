@@ -21,7 +21,7 @@ OBJ = os.path.join(SRC, "_build")
 LIB = os.path.join(HERE, "lib", "libcupoch_b200.so")
 SOURCES = ["index.cu", "sort.cu", "search.cu", "icp.cu", "voxel.cu", "features.cu", "filters.cu", "voxelgrid.cu", "comm.cu",
            "reduce.cu", "fpfh.cu", "cluster.cu", "occgrid.cu", "segment.cu", "fps.cu", "iss.cu", "edt.cu", "shot.cu",
-           "crop.cu", "collision.cu", "tsdf.cu", "mesh.cu", "depth_cloud.cu", "stsdf.cu"]
+           "crop.cu", "collision.cu", "tsdf.cu", "mesh.cu", "mesh_clean.cu", "depth_cloud.cu", "stsdf.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-fmad=false",
          "-Xcompiler", "-fPIC", "-I" + os.path.join(ROOT, "include"), "-I" + SRC]

@@ -517,8 +517,9 @@ class TriangleMesh:
     """geometry::TriangleMesh (trianglemesh.h): vertices_, triangles_ (int32 vertex indices), vertex_colors_,
     vertex_normals_, triangle_normals_ and edge_list_ (int32 pairs) on the device.  The normal computations,
     ComputeEdgeList, the four vertex filters, GetSurfaceArea, SamplePointsUniformly and the bounds run here, and
-    VoxelGrid.create_from_triangle_mesh[_within_bounds] turns a mesh into a grid; mesh IO, cleanup, primitives and
-    textures are not provided."""
+    VoxelGrid.create_from_triangle_mesh[_within_bounds] turns a mesh into a grid.  The cleanup operations
+    (remove_duplicated_vertices / _triangles, remove_unreferenced_vertices, remove_degenerate_triangles),
+    get_self_intersecting_triangles and + / += run here too; mesh IO, primitives and textures are not provided."""
 
     def __init__(self, vertices=None, triangles=None):
         self._vertices = self._triangles = self._vertex_colors = self._vertex_normals = self._triangle_normals = None
@@ -699,6 +700,152 @@ class TriangleMesh:
         pc = PointCloud()
         pc._points, pc._normals, pc._colors = pts, nrm, col
         return pc
+
+    # ------------------------------------------------------------------ cleanup (trianglemesh.cu:903-1141)
+    def _vertex_attrs(self):
+        return (self._vertex_normals if self.has_vertex_normals() else None,
+                self._vertex_colors if self.has_vertex_colors() else None)
+
+    def _vertex_pass(self, fn):
+        """the common path of the two vertex removals -> whether vertices were removed"""
+        n, m = self._n(self._vertices), self._n(self._triangles)
+        vn, vc = self._vertex_attrs()
+        ov = DeviceArray((n, 3), np.float32)
+        on, oc = [None if a is None else DeviceArray((n, 3), np.float32) for a in (vn, vc)]
+        ot = DeviceArray((m, 3), np.int32)
+        k = C.c_size_t(0)
+        _lib.check(fn(self._vertices.ptr if n else None, None if vn is None else vn.ptr, None if vc is None else vc.ptr, n,
+                      self._triangles.ptr if m else None, m, ov.ptr, None if on is None else on.ptr, None if oc is None else oc.ptr,
+                      ot.ptr, C.byref(k), None))
+        k = k.value
+        if n:
+            self._vertices = _rows(ov, k)
+            if on is not None:
+                self._vertex_normals = _rows(on, k)
+            if oc is not None:
+                self._vertex_colors = _rows(oc, k)
+        if m:
+            self._triangles = ot
+        return k < n
+
+    def _triangle_pass(self, fn):
+        """the common path of the two triangle removals -> whether triangles were removed"""
+        m = self._n(self._triangles)
+        if m == 0:
+            return False
+        tn = self._triangle_normals if self.has_triangle_normals() else None
+        ot = DeviceArray((m, 3), np.int32)
+        otn = None if tn is None else DeviceArray((m, 3), np.float32)
+        k = C.c_size_t(0)
+        _lib.check(fn(self._triangles.ptr, None if tn is None else tn.ptr, m, self._n(self._vertices), ot.ptr,
+                      None if otn is None else otn.ptr, C.byref(k), None))
+        k = k.value
+        self._triangles = _rows(ot, k)
+        if otn is not None:
+            self._triangle_normals = _rows(otn, k)
+        return k < m
+
+    def remove_duplicated_vertices(self):
+        """RemoveDuplicatedVertices (trianglemesh.cu:903-969): the distinct positions (IEEE ==, so -0 and +0 are one) in
+        lexicographic (x, y, z) order, each keeping the normal and colour of its lowest original index; triangles are
+        remapped.  A vertex with a NaN coordinate merges with nothing and goes last, in original order.  The edge list
+        is recomputed when the mesh has one.  A vertex index outside [0, len(vertices)) raises and changes nothing."""
+        self._vertex_pass(_lib.lib().cphb_mesh_remove_duplicated_vertices)
+        if self.has_edge_list():
+            self.compute_edge_list()
+        return self
+
+    def remove_duplicated_triangles(self):
+        """RemoveDuplicatedTriangles (trianglemesh.cu:971-1009): every triangle rotated so its smallest index comes first
+        (orientation kept: (a, b, c) and (a, c, b) differ), sorted, and the first of each run kept with its normal.  The
+        mesh keeps the rotated triangles in sorted order.  The edge list is recomputed when triangles were removed."""
+        if self._triangle_pass(_lib.lib().cphb_mesh_remove_duplicated_triangles) and self.has_edge_list():
+            self.compute_edge_list()
+        return self
+
+    def remove_unreferenced_vertices(self):
+        """RemoveUnreferencedVertices (trianglemesh.cu:1011-1080): keeps, in order, the vertices some triangle uses, with
+        their normals and colours; triangles are remapped.  The edge list is recomputed when vertices were removed."""
+        if self._vertex_pass(_lib.lib().cphb_mesh_remove_unreferenced_vertices) and self.has_edge_list():
+            self.compute_edge_list()
+        return self
+
+    def remove_degenerate_triangles(self):
+        """RemoveDegenerateTriangles (trianglemesh.cu:1082-1121): drops, keeping the order, the triangles with two equal
+        indices (a zero-area triangle with three distinct indices stays).  The edge list is recomputed when triangles
+        were removed."""
+        if self._triangle_pass(_lib.lib().cphb_mesh_remove_degenerate_triangles) and self.has_edge_list():
+            self.compute_edge_list()
+        return self
+
+    def get_self_intersecting_triangles(self):
+        """GetSelfIntersectingTriangles (trianglemesh.cu:1123-1141) -> (n, 2) int32 device array of the pairs i < j, in
+        ascending order, that share no vertex index, have only finite vertices, have overlapping closed boxes, and
+        that the reference's TriangleTriangle3d says intersect.  Found by an exact grid search (DESIGN section 4 item
+        26): memory grows with the triangles and the hits, not with their square."""
+        return self._self_intersections()[0]
+
+    def _self_intersections(self):
+        """-> (pairs, the number of box-overlapping pairs the predicate was evaluated on)"""
+        m, n = self._n(self._triangles), self._n(self._vertices)
+        L = _lib.lib()
+        args = (self._vertices.ptr if n else None, n, self._triangles.ptr if m else None, m)
+        cnt, cand = C.c_size_t(0), C.c_size_t(0)
+        _lib.check(L.cphb_mesh_self_intersecting_triangles(*args, None, 0, C.byref(cnt), C.byref(cand), None))
+        out = DeviceArray((cnt.value, 2), np.int32)
+        if cnt.value:
+            _lib.check(L.cphb_mesh_self_intersecting_triangles(*args, out.ptr, cnt.value, C.byref(cnt), C.byref(cand), None))
+        return out, cand.value
+
+    # ------------------------------------------------------------------ + and += (trianglemesh.cu:411-452, meshbase.cu:124-151)
+    def __iadd__(self, other):
+        """appends other's vertices and its triangles shifted by the old vertex count.  Vertex normals, vertex colours
+        and triangle normals survive when other has them and this mesh has them or has no vertices (triangles for
+        triangle normals); the edge list is recomputed when this mesh had one.  An empty other changes nothing."""
+        if not isinstance(other, TriangleMesh):
+            return NotImplemented
+        if other.is_empty():
+            return self
+        na, nb = self._n(self._vertices), len(other._vertices)
+        ta, tb = self._n(self._triangles), other._n(other._triangles)
+        tri = DeviceArray((ta + tb, 3), np.int32)
+        _lib.check(_lib.lib().cphb_mesh_append_triangles(self._triangles.ptr if ta else None, ta, na,
+                                                         other._triangles.ptr if tb else None, tb, nb, tri.ptr, None))
+        # the reference asks HasTriangles() after appending the vertices, so this mesh's own triangle count decides
+        keep_tn = (ta == 0 or self.has_triangle_normals()) and other.has_triangle_normals()
+        vn = (na == 0 or self.has_vertex_normals()) and other.has_vertex_normals()
+        vc = (na == 0 or self.has_vertex_colors()) and other.has_vertex_colors()
+        self._vertex_normals = _cat(self._vertex_normals if na else None, na, other._vertex_normals, nb) if vn else None
+        self._vertex_colors = _cat(self._vertex_colors if na else None, na, other._vertex_colors, nb) if vc else None
+        self._triangle_normals = (_cat(self._triangle_normals if ta else None, ta, other._triangle_normals, tb) if keep_tn
+                                  else None)
+        self._vertices = _cat(self._vertices, na, other._vertices, nb)
+        self._triangles = tri
+        if self.has_edge_list():
+            self.compute_edge_list()
+        return self
+
+    def __add__(self, other):
+        if not isinstance(other, TriangleMesh):
+            return NotImplemented
+        out = TriangleMesh()
+        out._vertices, out._triangles, out._vertex_colors = self._vertices, self._triangles, self._vertex_colors
+        out._vertex_normals, out._triangle_normals, out._edge_list = self._vertex_normals, self._triangle_normals, self._edge_list
+        out += other
+        return out
+
+
+def _cat(a, na, b, nb):
+    """rows [0, na) of a, then rows [0, nb) of b, as a new (na + nb, 3) device array"""
+    out = DeviceArray((na + nb,) + b.shape[1:], b.dtype)
+    L = _lib.lib()
+    row = out.nbytes // max(na + nb, 1)
+    if na:
+        _lib.check(L.cphb_memcpy_d2d(out.ptr, a.ptr, row * na, None))
+    if nb:
+        _lib.check(L.cphb_memcpy_d2d(out.ptr + row * na, b.ptr, row * nb, None))
+    _lib.check(L.cphb_stream_synchronize(None))
+    return out
 
 
 _MAX_SAMPLES = 2 ** 30 - 1  # CPHB_MESH_MAX_SAMPLES: draw 2 n must stay inside minstd_rand's period 2^31 - 2

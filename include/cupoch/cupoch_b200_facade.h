@@ -1989,8 +1989,8 @@ public:
 
 /// geometry::TriangleMesh (trianglemesh.h, meshbase.h): vertices_, vertex_normals_, vertex_colors_, triangles_ (int32
 /// vertex indices), triangle_normals_ and edge_list_ on the device.  The two normal computations, ComputeEdgeList,
-/// the four vertex filters, GetSurfaceArea, SamplePointsUniformly and GetMinBound / GetMaxBound are provided (no IO,
-/// cleanup or primitives).
+/// the four vertex filters, GetSurfaceArea, SamplePointsUniformly, GetMinBound / GetMaxBound, the four Remove*
+/// cleanup operations, GetSelfIntersectingTriangles and + / += are provided (no IO or primitives).
 class TriangleMesh : public MeshBase {
 public:
     TriangleMesh() {}
@@ -2091,6 +2091,70 @@ public:
         return pc;
     }
 
+    /// RemoveDuplicatedVertices (trianglemesh.cu:903-969): the distinct positions (IEEE ==, so -0 and +0 are one) in
+    /// lexicographic (x, y, z) order, each keeping the normal and colour of its lowest original index; triangles are
+    /// remapped.  A vertex with a NaN coordinate merges with nothing and goes last.  The edge list is recomputed when
+    /// the mesh has one.  A vertex index outside [0, vertices_.size()) throws and changes nothing.
+    TriangleMesh &RemoveDuplicatedVertices() {
+        VertexPass(cphb_mesh_remove_duplicated_vertices);
+        if (HasEdgeList()) ComputeEdgeList();
+        return *this;
+    }
+    /// RemoveDuplicatedTriangles (trianglemesh.cu:971-1009): each triangle rotated so its smallest index is first
+    /// (orientation kept), sorted, the first of each run kept with its normal; the edge list is recomputed when
+    /// triangles were removed
+    TriangleMesh &RemoveDuplicatedTriangles() {
+        if (TrianglePass(cphb_mesh_remove_duplicated_triangles) && HasEdgeList()) ComputeEdgeList();
+        return *this;
+    }
+    /// RemoveUnreferencedVertices (trianglemesh.cu:1011-1080): the vertices some triangle uses, in order, with their
+    /// normals and colours; triangles are remapped; the edge list is recomputed when vertices were removed
+    TriangleMesh &RemoveUnreferencedVertices() {
+        if (VertexPass(cphb_mesh_remove_unreferenced_vertices) && HasEdgeList()) ComputeEdgeList();
+        return *this;
+    }
+    /// RemoveDegenerateTriangles (trianglemesh.cu:1082-1121): drops, in order, the triangles with two equal indices;
+    /// the edge list is recomputed when triangles were removed
+    TriangleMesh &RemoveDegenerateTriangles() {
+        if (TrianglePass(cphb_mesh_remove_degenerate_triangles) && HasEdgeList()) ComputeEdgeList();
+        return *this;
+    }
+    /// GetSelfIntersectingTriangles (trianglemesh.cu:1123-1141): the pairs i < j, ascending, that share no vertex index,
+    /// have only finite vertices and overlapping closed boxes, and that TriangleTriangle3d says intersect
+    utility::device_vector<Eigen::Vector2i> GetSelfIntersectingTriangles() const {
+        const float *v = (const float *)vertices_.data();
+        const int32_t *t = (const int32_t *)triangles_.data();
+        size_t n = 0;
+        utility::check(cphb_mesh_self_intersecting_triangles(v, vertices_.size(), t, triangles_.size(), nullptr, 0, &n, nullptr, nullptr));
+        utility::device_vector<Eigen::Vector2i> out(n);
+        if (n)
+            utility::check(cphb_mesh_self_intersecting_triangles(v, vertices_.size(), t, triangles_.size(), (int32_t *)out.data(), n, &n,
+                                                                 nullptr, nullptr));
+        return out;
+    }
+    /// operator+= (trianglemesh.cu:411-452, meshbase.cu:124-151): other's vertices appended and its triangles shifted by
+    /// the old vertex count.  Vertex normals, vertex colours and triangle normals survive when other has them and this
+    /// mesh has them or has no vertices (triangles); the edge list is recomputed when this mesh had one.  An empty
+    /// other changes nothing; a vertex index outside its mesh's range throws and changes nothing.
+    TriangleMesh &operator+=(const TriangleMesh &other) {
+        if (other.IsEmpty()) return *this;
+        const size_t na = vertices_.size(), nb = other.vertices_.size(), ta = triangles_.size(), tb = other.triangles_.size();
+        utility::device_vector<Eigen::Vector3i> tri(ta + tb);
+        utility::check(cphb_mesh_append_triangles((const int32_t *)triangles_.data(), ta, na, (const int32_t *)other.triangles_.data(), tb, nb,
+                                                  (int32_t *)tri.data(), nullptr));
+        const bool vn = (na == 0 || HasVertexNormals()) && other.HasVertexNormals();
+        const bool vc = (na == 0 || HasVertexColors()) && other.HasVertexColors();
+        const bool tn = (ta == 0 || HasTriangleNormals()) && other.HasTriangleNormals();
+        Append(vertex_normals_, na, other.vertex_normals_, vn);
+        Append(vertex_colors_, na, other.vertex_colors_, vc);
+        Append(triangle_normals_, ta, other.triangle_normals_, tn);
+        Append(vertices_, na, other.vertices_, true);
+        triangles_ = std::move(tri);
+        if (HasEdgeList()) ComputeEdgeList();
+        return *this;
+    }
+    TriangleMesh operator+(const TriangleMesh &other) const { return TriangleMesh(*this) += other; }
+
 public:
     utility::device_vector<Eigen::Vector3f> vertices_;
     utility::device_vector<Eigen::Vector3f> vertex_normals_;
@@ -2100,6 +2164,56 @@ public:
     utility::device_vector<Eigen::Vector2i> edge_list_;
 
 private:
+    typedef int (*VertexPassFn)(const float *, const float *, const float *, size_t, const int32_t *, size_t, float *, float *, float *,
+                                int32_t *, size_t *, void *);
+    typedef int (*TrianglePassFn)(const int32_t *, const float *, size_t, size_t, int32_t *, float *, size_t *, void *);
+    // the two vertex removals' common path -> whether vertices were removed
+    bool VertexPass(VertexPassFn fn) {
+        const size_t n = vertices_.size(), m = triangles_.size();
+        const bool vn = HasVertexNormals(), vc = HasVertexColors();
+        utility::device_vector<Eigen::Vector3f> ov(n), on(vn ? n : 0), oc(vc ? n : 0);
+        utility::device_vector<Eigen::Vector3i> ot(m);
+        size_t k = 0;
+        utility::check(fn((const float *)vertices_.data(), vn ? (const float *)vertex_normals_.data() : nullptr,
+                          vc ? (const float *)vertex_colors_.data() : nullptr, n, (const int32_t *)triangles_.data(), m, (float *)ov.data(),
+                          vn ? (float *)on.data() : nullptr, vc ? (float *)oc.data() : nullptr, (int32_t *)ot.data(), &k, nullptr));
+        if (n) {
+            ov.resize(k);
+            vertices_ = std::move(ov);
+            if (vn) on.resize(k), vertex_normals_ = std::move(on);
+            if (vc) oc.resize(k), vertex_colors_ = std::move(oc);
+        }
+        if (m) triangles_ = std::move(ot);
+        return k < n;
+    }
+    // the two triangle removals' common path -> whether triangles were removed
+    bool TrianglePass(TrianglePassFn fn) {
+        const size_t m = triangles_.size();
+        if (m == 0) return false;
+        const bool tn = HasTriangleNormals();
+        utility::device_vector<Eigen::Vector3i> ot(m);
+        utility::device_vector<Eigen::Vector3f> otn(tn ? m : 0);
+        size_t k = 0;
+        utility::check(fn((const int32_t *)triangles_.data(), tn ? (const float *)triangle_normals_.data() : nullptr, m, vertices_.size(),
+                          (int32_t *)ot.data(), tn ? (float *)otn.data() : nullptr, &k, nullptr));
+        ot.resize(k);
+        triangles_ = std::move(ot);
+        if (tn) otn.resize(k), triangle_normals_ = std::move(otn);
+        return k < m;
+    }
+    // a += b for one attribute when keep, else a is cleared
+    template <class T>
+    static void Append(utility::device_vector<T> &a, size_t na, const utility::device_vector<T> &b, bool keep) {
+        if (!keep) {
+            a.clear();
+            return;
+        }
+        a.resize(na + b.size());
+        if (b.size()) {
+            utility::check(cphb_memcpy_d2d(a.data() + na, b.data(), b.size() * sizeof(T), nullptr));
+            utility::check(cphb_stream_synchronize(nullptr));
+        }
+    }
     // the filters' common path: a new mesh with the triangles, the edge list (this mesh's own when it has one, checked
     // for range and order) and every vertex attribute, filtered or copied; triangle normals are not carried
     std::shared_ptr<TriangleMesh> Filter(int kind, int iterations, float c0, float c1, FilterScope scope) const {

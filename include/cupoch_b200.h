@@ -698,6 +698,44 @@ int cphb_mesh_sample_points_uniformly(const float *vertices, size_t n_vertices, 
                                       size_t number_of_points, float *points, float *normals, float *colors, void *stream);
 
 /* ------------------------------------------------------------------------ *
+ * TriangleMesh cleanup, operator+= and GetSelfIntersectingTriangles (geometry/trianglemesh.cu:903-1141, DESIGN section 4
+ * item 26), on device arrays.  Every entry first checks each vertex index against [0, n_vertices) (CPHB_ERR_INVALID
+ * when one is outside) and rejects more than 2^31 - 1 vertices or triangles.  Outputs are separate buffers as large as
+ * the inputs; optional attributes (normals, colours, triangle normals) are NULL when absent.  Synchronise.
+ * ------------------------------------------------------------------------ */
+/* RemoveDuplicatedVertices: the distinct positions (IEEE ==, so -0 == +0) in lexicographic (x, y, z) order, each with
+ * the attributes of its lowest original index; a vertex with a NaN coordinate merges with nothing and goes after the
+ * others, in original order.  Triangles are remapped (order kept).  *h_n_vertices = the new count. */
+int cphb_mesh_remove_duplicated_vertices(const float *vertices, const float *vertex_normals, const float *vertex_colors, size_t n_vertices,
+                                         const int32_t *triangles, size_t n_triangles, float *out_vertices, float *out_normals,
+                                         float *out_colors, int32_t *out_triangles, size_t *h_n_vertices, void *stream);
+/* RemoveDuplicatedTriangles: each triangle rotated so its smallest index is first (orientation kept), sorted
+ * lexicographically (stable) and the first of each run kept, with its triangle normal.  *h_n_triangles = the count. */
+int cphb_mesh_remove_duplicated_triangles(const int32_t *triangles, const float *triangle_normals, size_t n_triangles, size_t n_vertices,
+                                          int32_t *out_triangles, float *out_triangle_normals, size_t *h_n_triangles, void *stream);
+/* RemoveUnreferencedVertices: stable compaction of the vertices some triangle references (with their normals and
+ * colours); triangles are remapped.  *h_n_vertices = the count. */
+int cphb_mesh_remove_unreferenced_vertices(const float *vertices, const float *vertex_normals, const float *vertex_colors, size_t n_vertices,
+                                           const int32_t *triangles, size_t n_triangles, float *out_vertices, float *out_normals,
+                                           float *out_colors, int32_t *out_triangles, size_t *h_n_vertices, void *stream);
+/* RemoveDegenerateTriangles: stable compaction of the triangles with three distinct indices, with their normals.
+ * *h_n_triangles = the count. */
+int cphb_mesh_remove_degenerate_triangles(const int32_t *triangles, const float *triangle_normals, size_t n_triangles, size_t n_vertices,
+                                          int32_t *out_triangles, float *out_triangle_normals, size_t *h_n_triangles, void *stream);
+/* operator+='s triangles: out [n_triangles_a + n_triangles_b][3] = a, then b shifted by n_vertices_a */
+int cphb_mesh_append_triangles(const int32_t *triangles_a, size_t n_triangles_a, size_t n_vertices_a, const int32_t *triangles_b,
+                               size_t n_triangles_b, size_t n_vertices_b, int32_t *out_triangles, void *stream);
+/* GetSelfIntersectingTriangles: every pair (i, j), i < j, of triangles that share no vertex index, whose vertices are
+ * all finite, whose closed float32 boxes overlap, and which the reference's TriangleTriangle3d (mean / sigma
+ * normalisation, then Moller's NoDivTriTriIsect with its epsilon test) says intersect; pairs [n][2] int32 in ascending
+ * (i, j) order.  *h_n_pairs is the count; the pairs are written only when capacity >= it (capacity 0 sizes).
+ * *h_n_candidates (may be NULL) = the box-overlapping pairs the predicate was evaluated on.  Memory grows with the
+ * triangles, the grid's candidate pairs (the pairs of triangles sharing a grid cell) and the hits; the candidate pairs
+ * reach n_triangles^2 / 2 only when every triangle falls into one cell (DESIGN section 4 item 26). */
+int cphb_mesh_self_intersecting_triangles(const float *vertices, size_t n_vertices, const int32_t *triangles, size_t n_triangles,
+                                          int32_t *pairs, size_t capacity, size_t *h_n_pairs, size_t *h_n_candidates, void *stream);
+
+/* ------------------------------------------------------------------------ *
  * PointCloud::CreateFromDepthImage / CreateFromRGBDImage (geometry/pointcloud_factory.cu:43-200, 329-373).  Images are
  * device buffers, row-major; outputs are caller-allocated device [rows][3] float32.
  * ------------------------------------------------------------------------ */

@@ -55,6 +55,8 @@ def main():
     ap.add_argument("--mesh-ops", action="store_true",
                     help="instead: time TriangleMesh.compute_edge_list, the four filters at 1 and 100 iterations, "
                          "get_surface_area and sample_points_uniformly (1 M, 10 M points) on the --tsdf-mesh sphere meshes")
+    ap.add_argument("--mesh-clean", action="store_true",
+                    help="time the TriangleMesh Remove* operations and GetSelfIntersectingTriangles on the --mesh-ops sphere meshes")
     ap.add_argument("--mesh-voxel", action="store_true",
                     help="instead: time VoxelGrid.create_from_triangle_mesh_within_bounds (sizing and writing call apart) on "
                          "the --mesh-ops sphere meshes at 1x and 2x their voxel size, a two-triangle 512^2 plane and a coarse "
@@ -62,6 +64,8 @@ def main():
     args = ap.parse_args()
     if args.mesh_voxel:
         return mesh_voxel(args.reps, args.out)
+    if args.mesh_clean:
+        return mesh_clean(args.reps, args.out)
     if args.mesh_ops:
         return mesh_ops(args.reps, args.out)
     if args.depth_cloud:
@@ -1427,6 +1431,109 @@ def mesh_voxel(reps, out=None):
         with open(out, "w") as f:
             f.write(line + "\n")
 
+
+def mesh_clean(reps, out=None):
+    """TriangleMesh cleanup and GetSelfIntersectingTriangles (C entry points) on the --mesh-ops sphere meshes
+    (UniformTSDFVolume(2.0, res, 0.04, RGB8), res 256 and 512, 8 ring-camera 640 x 480 views): each Remove* on the welded
+    mesh and on its un-welded soup (every triangle its own three vertices), and the self-intersection search on the
+    welded mesh, on the += union with a copy shifted by (0.3, 0.1, 0) and on the soup.  CUDA-event median and minimum of
+    `reps` after a warm-up, with the engine launches; the search's sizing and writing calls apart, with its candidate
+    pairs and hits; then one profiled call of each for per-kernel device times (torch.profiler)."""
+    import subprocess
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    import cupoch_b200 as cph
+    from cupoch_b200 import _lib
+    from cupoch_b200.testing.datagen import ring_cameras, sphere_depth
+    L = _lib.lib()
+    G, I = cph.geometry, cph.integration
+    DA = cph.utility.DeviceArray
+    gpu = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                         capture_output=True, text=True).stdout.strip()
+    ev = [L.cphb_event_create() for _ in range(2)]
+
+    def timed(fn):
+        times, launches = [], 0
+        for r in range(reps + 1):
+            n0 = L.cphb_launch_count()
+            L.cphb_event_record(ev[0], None)
+            fn()
+            L.cphb_event_record(ev[1], None)
+            ms = C.c_float(0)
+            _lib.check(L.cphb_event_elapsed_ms(ev[0], ev[1], C.byref(ms)))
+            launches = L.cphb_launch_count() - n0
+            if r:
+                times.append(ms.value)
+        return {"ms_median": float(np.median(times)), "ms_min": float(np.min(times)), "launches": int(launches)}
+
+    def kernels(fn):
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            fn()
+            torch.cuda.synchronize()
+        k = {}
+        for e in prof.key_averages():
+            t = getattr(e, "device_time_total", None) or getattr(e, "cuda_time_total", 0)
+            if t:
+                k[e.key[:80]] = {"calls": int(e.count), "us_total": float(t)}
+        return k
+
+    meshes = []
+    w, h = 640, 480
+    rng = np.random.default_rng(2)
+    for res in (256, 512):
+        vol = I.UniformTSDFVolume(2.0, res, 0.04, I.TSDFVolumeColorType.RGB8)
+        for K, E in ring_cameras(8, w, h):
+            d16 = np.round(sphere_depth(K, E, w, h, 0.6) * 1000).astype(np.uint16)
+            intr = cph.camera.PinholeCameraIntrinsic(w, h, K[0, 0], K[1, 1], K[0, 2], K[1, 2])
+            col = rng.integers(0, 256, (h, w, 3), dtype=np.uint8)
+            vol.integrate(G.RGBDImage.create_from_color_and_depth(G.Image(col), G.Image(d16), 1000.0, 100.0, False), intr, E)
+        mesh = vol.extract_triangle_mesh()
+        del vol
+        v, t = mesh.vertices.cpu(), mesh.triangles.cpu()
+        soup = G.TriangleMesh(v[t.reshape(-1)], np.arange(3 * len(t), dtype=np.int32).reshape(-1, 3))
+        union = mesh + G.TriangleMesh(v + np.float32([0.3, 0.1, 0.0]), t)
+        meshes.append((res, mesh, soup, union))
+
+    rows = []
+    for res, mesh, soup, union in meshes:
+        for kind, m in (("welded", mesh), ("soup", soup)):
+            nv, nt = len(m.vertices), len(m.triangles)
+            ov, ot, otn = DA((nv, 3), np.float32), DA((nt, 3), np.int32), DA((nt, 3), np.float32)
+            k = C.c_size_t(0)
+            vargs = (m.vertices.ptr, None, None, nv, m.triangles.ptr, nt, ov.ptr, None, None, ot.ptr, C.byref(k), None)
+            targs = (m.triangles.ptr, None, nt, nv, ot.ptr, None, C.byref(k), None)
+            for op, fn, a in (("remove_duplicated_vertices", L.cphb_mesh_remove_duplicated_vertices, vargs),
+                              ("remove_unreferenced_vertices", L.cphb_mesh_remove_unreferenced_vertices, vargs),
+                              ("remove_duplicated_triangles", L.cphb_mesh_remove_duplicated_triangles, targs),
+                              ("remove_degenerate_triangles", L.cphb_mesh_remove_degenerate_triangles, targs)):
+                call = lambda fn=fn, a=a: _lib.check(fn(*a))
+                row = {"workload": "sphere_res%d_%s" % (res, kind), "op": op, "vertices": nv, "triangles": nt, "call": timed(call)}
+                row["kept"] = int(k.value)
+                row["kernels_us"] = kernels(call)
+                rows.append(row)
+                print(json.dumps({x: row[x] for x in ("workload", "op", "kept")} | {"ms": row["call"]["ms_median"]}), flush=True)
+        for kind, m in (("welded", mesh), ("union", union), ("soup", soup)):
+            nv, nt = len(m.vertices), len(m.triangles)
+            n, cand = C.c_size_t(0), C.c_size_t(0)
+            args = (m.vertices.ptr, nv, m.triangles.ptr, nt)
+            _lib.check(L.cphb_mesh_self_intersecting_triangles(*args, None, 0, C.byref(n), C.byref(cand), None))
+            hits = n.value
+            pairs = DA((max(hits, 1), 2), np.int32)
+            sizing = lambda: _lib.check(L.cphb_mesh_self_intersecting_triangles(*args, None, 0, C.byref(n), C.byref(cand), None))
+            writing = lambda: _lib.check(L.cphb_mesh_self_intersecting_triangles(*args, pairs.ptr, hits, C.byref(n), C.byref(cand), None))
+            row = {"workload": "sphere_res%d_%s" % (res, kind), "op": "get_self_intersecting_triangles", "vertices": nv, "triangles": nt,
+                   "hits": hits, "n_candidates": int(cand.value), "sizing_call": timed(sizing), "writing_call": timed(writing),
+                   "kernels_us_writing_call": kernels(writing)}
+            row["both_calls_ms_median"] = row["sizing_call"]["ms_median"] + row["writing_call"]["ms_median"]
+            rows.append(row)
+            print(json.dumps({x: row[x] for x in ("workload", "triangles", "hits", "n_candidates", "both_calls_ms_median")}), flush=True)
+    obj = {"op": "TriangleMesh Remove* and GetSelfIntersectingTriangles (C entry points)", "gpu": gpu, "reps": reps, "rows": rows}
+    line = json.dumps(obj)
+    print(line)
+    if out:
+        with open(out, "w") as f:
+            f.write(line + "\n")
 
 if __name__ == "__main__":
     main()

@@ -1,7 +1,7 @@
 #!/bin/bash
 # compute-sanitizer over tools/sanitize_small.py (all five estimators through both regimes of the iteration kernel, k-NN /
 # radius search, VoxelDownSample, fused EstimateNormals, OccupancyGrid, FPFH, DBSCAN, filters, the TSDF
-# mesh and its edge list, filters, area, sampling and voxelisation).  Logs go to OUTDIR.
+# mesh and its edge list, filters, area, sampling and voxelisation, and the mesh cleanup and self-intersection search).  Logs go to OUTDIR.
 #   tools/gpu_sanitize.sh [OUTDIR]
 OUT=${1:-sanitizer_logs}
 mkdir -p "$OUT"

@@ -70,3 +70,11 @@ print("mesh edges", len(mesh.edge_list), "filtered", [len(m.vertices) for m in f
       "sampled", len(sampled.points), len(sampled.normals), len(sampled.colors))
 mesh_grid = G.VoxelGrid.create_from_triangle_mesh(mesh, 0.05)
 print("mesh voxels", len(mesh_grid), "within bounds", len(G.VoxelGrid.create_from_triangle_mesh_within_bounds(mesh, 0.1, (-1, -1, -1), (0.2, 1, 1))))
+soup = G.TriangleMesh(mesh.vertices.cpu()[mesh.triangles.cpu().reshape(-1)], np.arange(3 * len(mesh.triangles), dtype=np.int32).reshape(-1, 3))
+both = mesh + soup
+print("self-intersections", len(both.get_self_intersecting_triangles()), "soup", len(soup.get_self_intersecting_triangles()))
+big = G.TriangleMesh(np.concatenate([mesh.vertices.cpu(), np.float32([[-2, -2, 0], [2, -2, 0.1], [0, 2, -0.1], [-2, 0, -1], [2, 0.2, 1], [0, -0.2, 1]])]),
+                     np.concatenate([mesh.triangles.cpu(), len(mesh.vertices) + np.int32([[0, 1, 2], [3, 4, 5]])]).astype(np.int32))
+print("large-tier self-intersections", len(big.get_self_intersecting_triangles()))
+soup.remove_duplicated_vertices().remove_duplicated_triangles().remove_degenerate_triangles().remove_unreferenced_vertices()
+print("welded soup", len(soup.vertices), len(soup.triangles))

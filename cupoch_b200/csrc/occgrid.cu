@@ -106,8 +106,9 @@ __global__ void __launch_bounds__(256) occ_mark_kernel(const float *__restrict__
     const long long idx = occ_index_of(v[0], v[1], v[2], res);
     atomicOr(&occ_bits[idx >> 5], 1u << (idx & 31));
 }
-// Insert step 3: VoxelTraversal (occupancygrid.cu:57-132) of every ray; a cell that is not occupied and whose free bit
-// this thread raises first gets prob_miss_log.  The end voxel of a ray is never part of its free list (:119-121).
+// Insert step 3: VoxelTraversal (occupancygrid.cu:57-132) of every ray, with the first boundary on the face of the start
+// cell (DESIGN §4 item 27); a cell that is not occupied and whose free bit this thread raises first gets prob_miss_log.
+// The end voxel of a ray is never part of its free list (:119-121) unless it is also the start voxel.
 __global__ void __launch_bounds__(128) occ_traverse_kernel(const float *__restrict__ ranged, size_t n, float sx, float sy, float sz,
                                                            float ox, float oy, float oz, float vs, int res, int n_buffer,
                                                            const unsigned *__restrict__ occ_bits, unsigned *free_bits, float *prob,
@@ -129,7 +130,9 @@ __global__ void __launch_bounds__(128) occ_traverse_kernel(const float *__restri
                 cur[a] = (int)floorf(__fdiv_rn(start[a], vs));
                 last[a] = (int)floorf(__fdiv_rn(end[a], vs));
                 step[a] = (ray[a] > 0) ? 1.f : ((ray[a] < 0) ? -1.f : 0.f);
-                const float boundary = (float)(((double)cur[a] + 0.5 * (double)step[a]) * (double)vs);
+                // the face the ray leaves cell cur = [cur vs, (cur + 1) vs) through (DESIGN §4 item 27: the reference's
+                // (cur + 0.5 step) vs is half a voxel off it)
+                const float boundary = (float)(((double)cur[a] + ((step[a] > 0) ? 1.0 : 0.0)) * (double)vs);
                 tmax[a] = (step[a] != 0) ? __fdiv_rn(boundary - start[a], ray[a]) : INFINITY;
                 tdelta[a] = (step[a] != 0) ? __fdiv_rn(vs, fabsf(ray[a])) : INFINITY;
             }

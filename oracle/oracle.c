@@ -1711,10 +1711,13 @@ static void occ_add_one(float *prob, uint8_t *has_index, const int v[3], int res
     prob[idx] = fminf(fmaxf(p, params[0]), params[1]);
     has_index[idx] = 1;
 }
-/* VoxelTraversal (occupancygrid.cu:57-132): voxels the segment start -> end passes through, the end voxel excluded,
- * at most n_buffer of them; returns their number.  Mirrors the reference statement by statement, including its
- * half-voxel boundary offset (:81-83) and the int += float steps. */
-static int occ_voxel_traversal(int (*voxels)[3], int n_buffer, int half, const float start[3], const float end[3], float vs) {
+/* VoxelTraversal (occupancygrid.cu:57-132): voxels the segment start -> end passes through, the end voxel excluded
+ * (unless it is the start voxel), at most n_buffer of them; returns their number.  Mirrors the reference statement by
+ * statement (the int += float steps, the tie order, both stop tests) except for the first boundary: cell k is
+ * [k vs, (k + 1) vs), and the ray leaves it through (k + 1) vs going up and k vs going down (DESIGN §4 item 27).
+ * ref_rule != 0 puts it at (k + 0.5 step) vs like the reference (:83-85), half a voxel off that cell's faces. */
+static int occ_voxel_traversal(int (*voxels)[3], int n_buffer, int half, const float start[3], const float end[3], float vs,
+                               int ref_rule) {
     int n = 0;
     float ray[3] = {end[0] - start[0], end[1] - start[1], end[2] - start[2]};
     const float length = sqrtf((ray[0] * ray[0] + ray[1] * ray[1]) + ray[2] * ray[2]);
@@ -1726,7 +1729,8 @@ static int occ_voxel_traversal(int (*voxels)[3], int n_buffer, int half, const f
         cur[a] = (int)floorf(start[a] / vs);
         last[a] = (int)floorf(end[a] / vs);
         step[a] = (ray[a] > 0) ? 1.f : ((ray[a] < 0) ? -1.f : 0.f);
-        const float boundary = (float)(((double)cur[a] + 0.5 * (double)step[a]) * (double)vs);
+        const double off = ref_rule ? 0.5 * (double)step[a] : ((step[a] > 0) ? 1.0 : 0.0);
+        const float boundary = (float)(((double)cur[a] + off) * (double)vs);
         tmax[a] = (step[a] != 0) ? (boundary - start[a]) / ray[a] : INFINITY;
         tdelta[a] = (step[a] != 0) ? vs / fabsf(ray[a]) : INFINITY;
     }
@@ -1767,10 +1771,11 @@ void orc_occgrid_add_voxels(float *prob, uint8_t *has_index, uint16_t bounds[6],
 }
 /* OccupancyGrid::Insert (occupancygrid.cu:462-526).  Every voxel is updated at most once per call (the reference sorts and
  * uniques the voxel lists, :179-183,:239-243); free voxels that are also occupied are dropped (set_difference, :516-520).
- * stamp: scratch [res^3] bytes, all zero on entry and on return. */
+ * stamp: scratch [res^3] bytes, all zero on entry and on return.  ref_rule: the traversal's boundary rule (see
+ * occ_voxel_traversal); 0 is the library's. */
 void orc_occgrid_insert(float *prob, uint8_t *has_index, uint8_t *stamp, uint16_t bounds[6], int res, float voxel_size,
                         const float origin[3], const float params[4], const float *points, int n, const float viewpoint[3],
-                        float max_range) {
+                        float max_range, int ref_rule) {
     if (n <= 0) return;
     const int half = res / 2;
     float *ranged = (float *)malloc(sizeof(float) * 3 * (size_t)n);
@@ -1810,7 +1815,7 @@ void orc_occgrid_insert(float *prob, uint8_t *has_index, uint8_t *stamp, uint16_
         const float start[3] = {viewpoint[0] - origin[0], viewpoint[1] - origin[1], viewpoint[2] - origin[2]};
         for (int i = 0; i < n; ++i) {
             const float end[3] = {ranged[3 * i] - origin[0], ranged[3 * i + 1] - origin[1], ranged[3 * i + 2] - origin[2]};
-            const int m = occ_voxel_traversal(buf, n_step, half, start, end, voxel_size);
+            const int m = occ_voxel_traversal(buf, n_step, half, start, end, voxel_size, ref_rule);
             for (int k = 0; k < m; ++k) {
                 if (!occ_in_range(buf[k], res)) continue;
                 const long idx = occ_index_of(buf[k][0], buf[k][1], buf[k][2], res);
@@ -1827,7 +1832,7 @@ void orc_occgrid_insert(float *prob, uint8_t *has_index, uint8_t *stamp, uint16_
         /* clear the free stamps again (second traversal: cheaper than an n_free list for the oracle's sizes) */
         for (int i = 0; i < n; ++i) {
             const float end[3] = {ranged[3 * i] - origin[0], ranged[3 * i + 1] - origin[1], ranged[3 * i + 2] - origin[2]};
-            const int m = occ_voxel_traversal(buf, n_step, half, start, end, voxel_size);
+            const int m = occ_voxel_traversal(buf, n_step, half, start, end, voxel_size, ref_rule);
             for (int k = 0; k < m; ++k)
                 if (occ_in_range(buf[k], res)) {
                     const long idx = occ_index_of(buf[k][0], buf[k][1], buf[k][2], res);

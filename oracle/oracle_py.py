@@ -351,12 +351,13 @@ class OccupancyGrid:
                                      _p(self._params()), _p(v), C.c_int(len(v)), C.c_int(int(occupied)))
         return self
 
-    def insert(self, points, viewpoint, max_range=-1.0):
+    def insert(self, points, viewpoint, max_range=-1.0, ref_rule=False):
+        """ref_rule: walk with the reference's half-voxel boundary instead of the library's (DESIGN §4 item 27)"""
         pts = _f(points).reshape(-1, 3)
         vp = np.asarray(viewpoint, np.float32).reshape(3)
         lib().orc_occgrid_insert(_p(self.prob), _p(self.has_index), _p(self._stamp), _p(self.bounds), C.c_int(self.resolution),
                                  C.c_float(self.voxel_size), _p(self.origin), _p(self._params()), _p(pts), C.c_int(len(pts)),
-                                 _p(vp), C.c_float(max_range))
+                                 _p(vp), C.c_float(max_range), C.c_int(int(bool(ref_rule))))
         return self
 
     def set_free_area(self, min_bound, max_bound):
